@@ -5,6 +5,7 @@ FastConformer-RNNT 619 M transcribe path, BASELINE.json configs[1] per GPU
 
     python bench.py --gpus N --steps K --warmup W            # this framework (one rank per GPU under torchrun)
     python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on the host CPU (oracle port)
+    python bench.py --gpus 1 --steps K --dump-outputs DIR    # + what the last timed step returned, as DIR/<name>.npy
 
 One JSON line on stdout (rank 0).  `value` times rs_transcribe_device with the waveforms already
 resident in HBM; `e2e` times rs_transcribe_batch (the model.transcribe seam of the C ABI) with
@@ -33,18 +34,16 @@ METRIC = "RTFx (audio-s/wall-s) FastConformer-RNNT 619M"
 UNIT = "audio-s/wall-s"
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1407.1), d.get("bf16_tflops", 1691.8), d.get("hbm_gbs", 6564.5), "measured"
-    return 1400.0, 1590.0, 6650.0, "fallback"
+# NVIDIA's data sheet for the H100 SXM at 700 W: dense bf16 TFLOP/s and HBM3 GB/s.  Ceilings, not measurements; the card
+# the numbers were taken on and its power limit are reported beside them ("gpu").
+DATA_SHEET_BF16_TFLOPS, DATA_SHEET_HBM_GBS = 989.0, 3350.0
 
 
 class ClockSampler:
     """nvidia-smi clocks / throttle reasons sampled every 200 ms while the timed region runs."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
-         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,"
+         "name,power.limit")
 
     def __init__(self, index: int):
         self.index, self.proc, self.lines = index, None, []
@@ -59,10 +58,10 @@ class ClockSampler:
 
     def stop(self):
         if self.proc is None:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"], "gpu": None, "power_limit_w": None}
         time.sleep(0.25)
         self.proc.terminate()
-        sm, mx, reasons = [], [], set()
+        sm, mx, reasons, gpu, limit = [], [], set(), None, None
         for l in self.lines:
             f = [x.strip() for x in l.split(",")]
             if len(f) < 9:
@@ -74,9 +73,11 @@ class ClockSampler:
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[5:9]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
+            if len(f) >= 11:
+                gpu, limit = f[9], f[10]
         busy = [s for s in sm if s > 0]
         return {"sm_mhz": float(np.median(busy)) if busy else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "reasons": sorted(reasons), "samples": len(sm), "gpu": gpu, "power_limit_w": limit}
 
 
 def python_api_rtfx(eng, n_clips: int, seconds: float, rank: int, batches: int = 4):
@@ -279,6 +280,8 @@ def main():
     ap.add_argument("--seconds", type=float, default=NOMINAL_SECONDS)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip python_api / decode_sensitivity / config2 (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (tokens, frames, n_tok of every clip) as DIR/<name>.npy, float32")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -341,6 +344,14 @@ def main():
     ms_step = ms_total / args.steps
     value = world * B * args.seconds / (ms_step / 1e3)
     n_tok = out_dev[2].cpu()
+    if args.dump_outputs and rank == 0:
+        # the arrays rs_transcribe_device hands its caller, from the last timed step: entries at or beyond a clip's token
+        # count are not part of the result and are written as -1
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        live = torch.arange(U)[None, :] < n_tok[:, None]
+        for name, t in (("tokens", out_dev[0]), ("frames", out_dev[1])):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), torch.where(live, t.cpu(), -1).numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "n_tok.npy"), n_tok.numpy().astype(np.float32))
 
     # ---------------- end-to-end through the host-buffer C-ABI call (`e2e`)
     for _ in range(2):
@@ -355,8 +366,8 @@ def main():
     h2d = wav_host.numel() * 4 + len_host.numel() * 4
     d2h = (out_host[0].numel() + out_host[1].numel() + out_host[2].numel()) * 4
 
-    # ---------------- roofline of the dominant kernel (tcgen05 GEMM), CUDA events per launch
-    sus, burst, hbm, src = measured_peaks()
+    # ---------------- roofline of the dominant kernel (wgmma GEMM), CUDA events per launch
+    sus, hbm, src = DATA_SHEET_BF16_TFLOPS, DATA_SHEET_HBM_GBS, "H100 SXM data sheet (700 W), dense bf16"
     eng.enable_gemm_timing(True)
     for _ in range(args.steps):
         eng.transcribe_device(wav_dev, len_dev, U, out_dev)
@@ -380,7 +391,7 @@ def main():
     attn_cycles = eng.attention_cycles()
     if not any(attn_cycles.values()):
         attn_cycles = None
-    # memory-bound kernels against the measured copy bandwidth: ALGORITHMIC bytes (SURVEY.md section 8d) over the
+    # memory-bound kernels against the data-sheet HBM bandwidth: ALGORITHMIC bytes (SURVEY.md section 8d) over the
     # in-pipeline time of their launches (event pairs above, so warm-L2 effects are included: a fraction can exceed 1)
     valid_T = eng.cfg.enc_frames(L)
     dm = eng.cfg.d_model
@@ -402,17 +413,10 @@ def main():
     # frames); the roofline numerator keeps only the valid rows
     g_flops *= eng.cfg.enc_frames(L) / max(eng.enc_frames(L), 1)
     achieved = g_flops / (g_ms * 1e-3) / 1e12 if g_ms > 0 else 0.0
-    # DRAM bytes per launch of the dominant kernel cannot be measured without a profiler: they are read from the committed
-    # summary of this round's `ncu --set full` capture of the same command (profiles/r02_gemm_traffic.json, written by
-    # scripts/summarize_ncu.py); null when that file is absent
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
-    roofline = {"bound": "tensor", "achieved": achieved, "peak": sus, "unit": "TFLOP/s", "frac": achieved / sus, "traffic": traffic,
-                "traffic_source": traffic_src,
-                "kernel": "gemm_bf16_tn_kernel (tcgen05.mma, all encoder/joint GEMMs)", "peak_source": f"{src} bf16_tflops_sustained",
+    # DRAM bytes per launch of the dominant kernel are not measured (that needs a hardware-counter profiler)
+    roofline = {"bound": "tensor", "achieved": achieved, "peak": sus, "unit": "TFLOP/s", "frac": achieved / sus, "traffic": None,
+                "traffic_source": None,
+                "kernel": "gemm_bf16_tn_kernel (wgmma.mma_async, all encoder/joint GEMMs)", "peak_source": src,
                 "launches_per_step": g_n // max(args.steps, 1), "gemm_ms_per_step": g_ms / max(args.steps, 1),
                 "algorithmic_gflop_per_step": g_flops / max(args.steps, 1) / 1e9,
                 "how": "CUDA events around every GEMM launch on its stream, separate pass of the same K steps"}
@@ -494,7 +498,7 @@ def main():
         "data": "synthetic 16 kHz AM/FM clips; seeded random weights (619 M architecture, no checkpoint offline)",
         "config": {"workload": f"nemo-asr FastConformer-RNNT 619M, batch={B}x{args.seconds:g} s clips per GPU",
                    "samples_per_clip": L, "enc_frames": eng.cfg.enc_frames(L), "parallelism": f"utterance-sharded x{world}, no collective",
-                   "l2": "per-step working set (~2 GB activations) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (~2 GB activations) exceeds the 50 MB L2; no explicit flush",
                    "tokens_per_clip": float(n_tok.float().mean())},
         "clocks": clocks, "gpu_launches": int(launches),
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),

@@ -1,5 +1,5 @@
 /*
- * rs_engine.h -- C ABI of the B200-native FastConformer-RNNT engine.
+ * rs_engine.h -- C ABI of the H100-native FastConformer-RNNT engine.
  *
  * The reference (reazon-research/ReazonSpeech) has no native layer: its hot path is one
  * opaque Python call into NeMo,
@@ -63,7 +63,7 @@ typedef struct rs_tensor {
 
 typedef struct rs_engine rs_engine;
 
-/* Epilogues of the tcgen05 GEMM  out = epi(A[M,K] * W[N,K]^T)  (SURVEY.md App. A.3). */
+/* Epilogues of the wgmma GEMM  out = epi(A[M,K] * W[N,K]^T)  (SURVEY.md App. A.3). */
 typedef enum rs_epilogue {
   RS_EPI_BIAS_BF16 = 0,       /* out_bf16[M,N]   = acc + bias                                  */
   RS_EPI_BIAS_RELU_BF16 = 1,  /* out_bf16[M,N]   = relu(acc + bias)                            */
@@ -178,13 +178,13 @@ int64_t rs_launch_count(const rs_engine* e);
 /* Per-stage device time of the last rs_transcribe_* call when timing was enabled. */
 int rs_enable_stage_timing(rs_engine* e, int on);
 int rs_stage_times_ms(const rs_engine* e, float* ms /*[8]*/);
-/* Per-launch CUDA-event timing of the tcgen05 GEMM (the dominant kernel): while enabled every GEMM
+/* Per-launch CUDA-event timing of the wgmma GEMM (the dominant kernel): while enabled every GEMM
  * launch is bracketed by two events on its stream.  rs_gemm_timing() synchronises, returns the summed
  * device time, the summed algorithmic FLOPs (2*M*N*K) and the launch count since it was enabled or
  * last read, and resets the accumulators. */
 int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* out8);   /* profiling aid, see engine.cu */
 int rs_debug_attention_cycles(rs_engine* e, int64_t* out16);   /* clock64 stamps of one CTA of the last attention launch */
-int rs_debug_gemm_cycles(rs_engine* e, int64_t* out64);        /* clock64 timeline of the last 2-CTA GEMM launch: first / last cluster x 32 stamps (gemm_tcgen05.cu) */
+int rs_debug_gemm_cycles(rs_engine* e, int64_t* out64);        /* clock64 stamps of CTA 0 of the last GEMM launch: [30] entry, [31] exit, only with -DRS_PROF (gemm_wgmma.cu) */
 int rs_enable_gemm_timing(rs_engine* e, int on);
 int rs_gemm_timing(rs_engine* e, double* ms, double* flops, int64_t* launches);
 /* Per-kernel CUDA-event timing of EVERY launch inside the real pipeline (warm caches, back-to-back launches, unlike

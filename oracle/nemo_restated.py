@@ -36,7 +36,7 @@ The reference-owned ``decode_hypothesis`` is pinned separately by importing the 
 
 Semantics are batch=1, exactly as the reference calls NeMo (transcribe.py:48-50): every
 function takes ONE utterance with no padding.  ``emulate`` switches on bf16 rounding of
-activations at the points where the sm_100a engine stores bf16 (used only to tighten the
+activations at the points where the sm_90a engine stores bf16 (used only to tighten the
 token-identity test; the reference semantics are ``emulate=False``).
 """
 from __future__ import annotations
@@ -296,7 +296,7 @@ class FollowResult:
 
 def greedy_follow(enc: torch.Tensor, sd: StateDict, cfg: ModelConfig, decisions: List[int], emulate: bool = False,
                   enc_ref: Optional[torch.Tensor] = None) -> FollowResult:
-    """Re-synchronising comparison with a greedy decode produced elsewhere (the sm_100a engine).
+    """Re-synchronising comparison with a greedy decode produced elsewhere (the sm_90a engine).
 
     Walks ``decisions`` (the argmax of EVERY joint evaluation, blanks included, as rebuilt from tokens + frames) through
     the same control flow as ``rnnt_greedy`` but TEACHER-FORCED: the predictor state always follows the given decision.

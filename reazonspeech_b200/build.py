@@ -1,4 +1,4 @@
-"""Build librs_engine.so (the C-ABI library of sm_100a kernels) in-tree with nvcc.
+"""Build librs_engine.so (the C-ABI library of sm_90a kernels) in-tree with nvcc.
 
 nvcc cross-compiles without a GPU.  Objects are cached under reazonspeech_b200/csrc/build/
 and rebuilt when the source (or any header) is newer.  Usage: ``python -m reazonspeech_b200.build``.
@@ -15,10 +15,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(HERE, "librs_engine.so")
-SOURCES = ["gemm_tcgen05.cu", "logmel.cu", "subsample.cu", "elementwise.cu", "resample.cu", "attention_tc.cu", "decode_spec.cu", "decode_alsd.cu", "host_staging.cu", "engine.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+SOURCES = ["gemm_wgmma.cu", "logmel.cu", "subsample.cu", "elementwise.cu", "resample.cu", "attention_tc.cu", "decode_spec.cu", "decode_alsd.cu", "host_staging.cu", "engine.cu"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
-FLAGS += os.environ.get("RS_BUILD_FLAGS", "").split()        # build-time only, e.g. -DRS_PROF for scripts/diag_gemm_timeline.py
+FLAGS += os.environ.get("RS_BUILD_FLAGS", "").split()        # build-time only, e.g. -DRS_PROF for the cycle stamps
 
 
 def _nvcc() -> str:

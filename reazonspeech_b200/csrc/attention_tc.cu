@@ -1,34 +1,29 @@
-// Relative-position local attention with a global token (N5) on the 5th-generation tensor cores.
+// Relative-position local attention with a global token (N5) on the Hopper tensor cores (wgmma).
 //
-// Same function as attention.cu::local_attention_kernel (NeMo RelPositionMultiHeadAttentionLongformer,
-// parts/submodules/multi_head_attention.py, reached through model.transcribe at
-// pkg/nemo-asr/src/transcribe.py:48-53; semantics restated in oracle/nemo_restated.py::local_attention_core).
-// The mma.sync kernel is bound by the legacy tensor path (one m16n8k16 per ~19 cycles and scheduler on
-// sm_100 -> ~250 TFLOP/s for the whole chip); this one puts both products on tcgen05.
+// NeMo RelPositionMultiHeadAttentionLongformer (parts/submodules/multi_head_attention.py, reached through
+// model.transcribe at pkg/nemo-asr/src/transcribe.py:48-53; semantics restated in
+// oracle/nemo_restated.py::local_attention_core).
 //
-// One CTA = 128 query rows of one (utterance, head).  With a band of +-w (w <= 128) those rows see the
-// 384 keys [q0-128, q0+256), so the whole score tile lives in tensor memory and no online softmax is needed:
+// One CTA = 128 query rows of one (utterance, head): two consumer warpgroups of 64 rows each and one producer warp.
+// With a band of +-w (w <= 128) those rows see the 384 keys [q0-128, q0+256), walked in six blocks of 64 keys:
 //
-//   TMA   Q' [128 x 128] (q + pos_bias_u, folded into the QKV projection's bias at pack time) and the head's positional
-//         table P [n_rel_pad x 128] (linear_pos(pos_emb), packed at load) -> shared memory, 128-byte swizzle, K-major
-//   UMMA  BD[128 x n_rel_pad] = Q' P^T     -> TMEM columns [0, n_rel_pad)   (the relative-position term; + the constant
-//         (pos_bias_v - pos_bias_u) . p[c] it equals (q + pos_bias_v) . p[c])
-//   8 softmax warps drain BD: (acc + bias[c]) / sqrt(dk) * log2 e -> IEEE half, row-major into shared memory
-//   TMA   K [384 x 128] over the positional table (dead once its product retired)
-//   UMMA  S[128 x 384] = Q' K^T            -> TMEM columns [0, 384)         (24 x tcgen05.mma 128x128x16)
-//   pass 1, one thread per (row, column half): t = S / sqrt(dk) + BD[i, j-i+w] (the rel_shift: row i reads its BD row at
-//         an offset that depends on i -- 32-bit shared loads + a funnel shift where the offset is odd) with the band /
-//         padding mask, row maximum (with the global key's score); t written back to tensor memory
-//   TMA   V^T [128 x 384] over the BD buffer (dead after pass 1; the QKV GEMM's epilogue writes V transposed, RS_EPI_QKV_VT)
-//   pass 2: p = exp2(t - m) -> bf16 P into the shared memory that held K (same swizzled K-major layout), row sums
-//   UMMA  O[128 x 128] = P V               -> TMEM columns [384, 512)       (24 x tcgen05.mma 128x128x16)
-//   epilogue  O + p_global * v_0, divided by the row sum -> bf16, staged and stored in whole 128-byte lines
+//   TMA    Q' [128 x 128] (q + pos_bias_u, folded into the QKV projection's bias at pack time) and the head's positional
+//          table P [n_rel_pad x 128] (linear_pos(pos_emb), packed at load) -> shared memory, 128-byte swizzle, K-major
+//   wgmma  BD[64 x n_rel_pad] = Q' P^T per warpgroup, 32 columns at a time (the relative-position term; + the constant
+//          (pos_bias_v - pos_bias_u) . p[c] it equals (q + pos_bias_v) . p[c]) -> (acc + bias[c]) / sqrt(dk) * log2 e as
+//          IEEE half, row-major in shared memory.  It never leaves the SM.
+//   TMA    K [64 x 128] and V^T [128 x 64] blocks through a three-stage ring laid over the positional table (dead once
+//          the BD product has retired); the QKV GEMM's epilogue writes V transposed (RS_EPI_QKV_VT)
+//   per key block and warpgroup:
+//     wgmma  S[64 x 64] = Q' K^T, accumulators in registers
+//     t = S / sqrt(dk) + BD[i, j-i+w] (the rel_shift: row i reads its BD row at an offset that depends on i) with the band /
+//         padding mask; running row maximum and sum (online softmax, log2 domain), O rescaled when the maximum moves
+//     wgmma  O[64 x 128] += P V with P = exp2(t - m) as bf16 taken straight from the S accumulator registers (the
+//            accumulator fragment of S is the A fragment of the next product)
+//   epilogue  O + p_global * v_0, divided by the row sum -> bf16, staged per warp and stored in whole rows
 //
-// Round 1 computed BD with a separate batched GEMM that wrote a row-skewed IEEE-half tensor [M, H, 384] (77 MB per layer at
-// 32 x 30 s, 3.7 GB per step of pure intermediate traffic, 1.05 ms) which this kernel read back; the positional product is a
-// 128 x 288 x 128 UMMA here and its result never leaves the SM.  Rows of the global token itself are overwritten afterwards
-// by global_row_attention_tc_kernel (full attention, no positional term).  Shared memory: 32 KB Q' + 96 KB P-table / K /
-// probabilities + 96 KB BD / V^T; tensor memory: all 512 columns.
+// Rows of the global token itself are overwritten afterwards by global_row_attention_tc_kernel (full attention, no
+// positional term).  Shared memory: 32 KB Q' + 96 KB positional table / K, V^T ring + 74 KB BD.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -39,24 +34,22 @@ namespace rs {
 namespace {
 
 constexpr int TQ = 128;                 // query rows per CTA
-constexpr int TK = 384;                 // key window
 constexpr int TDK = 128;                // head dim
+constexpr int KB = 64;                  // keys per block
+constexpr int kBlocks = 6;              // key window = 384 keys
 constexpr int kSlab = TQ * 128;         // bytes of one [128 rows x 64 bf16] swizzled slab
-constexpr int kAtcThreads = 32 * 9;     // warp 0: TMA + MMA issue; warps 1..8: softmax / epilogue
+constexpr int kAtcThreads = 32 * 9;     // warps 0..7: two consumer warpgroups; warp 8: TMA producer
+constexpr int kKvStages = 3;
+constexpr uint32_t kKvStageBytes = 2 * KB * 128 + TDK * 128;   // K block as two k-slabs of 64 rows + V^T block of 128 rows
 constexpr uint32_t kOffQ = 0;                       // 2 slabs
-constexpr uint32_t kOffK = 2 * kSlab;               // positional table (2 k-slabs x n_rel_pad rows), then K: 2 k-slabs x 3 row blocks, then P: 6 key-slabs
-constexpr uint32_t kOffV = kOffK + 6 * kSlab;       // BD as IEEE half [128][kBdPitch], then 6 key-slabs of V^T
-constexpr uint32_t kOffBar = kOffV + 6 * kSlab;     // 8 mbarriers + tmem slot
-constexpr int kBdPitch = 296;                       // halves per BD row: 592 B = 37 x 16 B (odd: 16-byte stores of 8 consecutive rows hit 8 different bank groups)
+constexpr uint32_t kOffKV = 2 * kSlab;              // positional table (2 k-slabs x n_rel_pad rows), then the K / V^T ring
+constexpr uint32_t kOffBD = kOffKV + kKvStages * kKvStageBytes;   // BD as IEEE half [128][kBdPitch]; a warp's rows stage its output at the end
+constexpr int kBdPitch = 296;                       // halves per BD row
 constexpr int kNrelPadMax = 288;                    // 2 * 128 + 1 relative offsets rounded up to 32
-constexpr uint32_t kAtcSmem = kOffBar + 1024 + 1024; // barriers, k_0 row, global-key scores, alignment slack
-// small arrays that alias the Q' tile once the S product has retired
-constexpr uint32_t kOffMax = kOffQ;                 // float [2][128]
-constexpr uint32_t kOffSum = kOffQ + 1024;          // float [2][128]
-constexpr uint32_t kOffPg = kOffQ + 2048;           // float [128]
-constexpr uint32_t kOffV0 = kOffQ + 2560;           // float [128]
-// k_0 (global key) sits in the barrier block's tail while Q' is still live
-constexpr int kStagePitch = 64 + 8;                 // bf16 per staged output row (144 B: conflict-free 16-byte accesses)
+constexpr uint32_t kOffBar = kOffBD + TQ * kBdPitch * 2;   // 8 mbarriers | k_0 [128] bf16 (+64) | u.k_0 (+320) | q'.k_0 [128] (+512) | v_0 [128] (+1024)
+constexpr uint32_t kAtcSmem = kOffBar + 1536 + 1024;       // + alignment slack
+constexpr int kOutPitch = 136;                      // bf16 per staged output row (272 B: conflict-free fragment writes)
+static_assert(2 * kNrelPadMax * 128 <= kKvStages * kKvStageBytes && kOutPitch <= kBdPitch && kAtcSmem <= 227 * 1024, "shared memory layout");
 
 struct AtcDev {
   const __nv_bfloat16* qk;      // [M, ld_qk]: q' at column h*128, k at column d + h*128
@@ -68,27 +61,9 @@ struct AtcDev {
   int T_max, H, w_left, w_right, n_global, n_rel_pad, ld_qk, ld_vt;
 };
 
-// cycle stamps of CTA (1, 0, 0): [0..7] control thread, [8..15] first softmax thread (profiling aid, rs_debug_attention_cycles)
+// cycle stamps of thread 0 of CTA (1, 0, 0): [0] kernel entry, [6] exit (profiling aid, rs_debug_attention_cycles; only with -DRS_PROF)
 __device__ long long g_atc_prof[16];
-#ifdef RS_PROF      // RS_BUILD_FLAGS=-DRS_PROF python -m reazonspeech_b200.build --force; not in the shipped build
-#define ATC_STAMP(cond, slot) do { if (prof_cta && (cond)) g_atc_prof[slot] = clock64(); } while (0)
-#else
-#define ATC_STAMP(cond, slot) do { (void)prof_cta; } while (0)
-#endif
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void softmax_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the 8 softmax warps
 __device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 // byte offset of the 16-byte chunk `chunk` (0..7) of row `row` inside a [rows x 64 bf16] 128B-swizzled slab
@@ -97,14 +72,18 @@ __device__ __forceinline__ uint32_t sw128(int row, int chunk) {
 }
 
 __global__ void __launch_bounds__(kAtcThreads, 1)
-local_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qk, const __grid_constant__ CUtensorMap tm_vt,
-                          const __grid_constant__ CUtensorMap tm_pos, const AtcDev p) {
+local_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+                          const __grid_constant__ CUtensorMap tm_vt, const __grid_constant__ CUtensorMap tm_pos, const AtcDev p) {
   extern __shared__ uint8_t atc_raw[];
   const uint32_t base = (smem_u32(atc_raw) + 1023u) & ~1023u;
   uint8_t* gen = atc_raw + (base - smem_u32(atc_raw));          // generic pointer to the aligned base
-  const uint32_t bar_qk = base + kOffBar, bar_v = bar_qk + 8, bar_s = bar_qk + 16, bar_o = bar_qk + 24, tmem_slot = bar_qk + 32;
-  const uint32_t bar_bd = bar_qk + 40, bar_k = bar_qk + 48, bar_drained = bar_qk + 56, bar_p1 = bar_qk + 320;   // behind s_k0 ([64, 320)), before s_uk (448) and s_sg ([512, 1024))
-  __nv_bfloat16* s_k0 = reinterpret_cast<__nv_bfloat16*>(gen + kOffBar + 64);   // [128] (fits: 64 + 256 <= 128 + slack)
+  const uint32_t bar_qk = base + kOffBar, bar_drained = bar_qk + 8;
+  auto full_bar = [&](int s) { return bar_qk + 16u + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_qk + 40u + 8u * s; };
+  __nv_bfloat16* s_k0 = reinterpret_cast<__nv_bfloat16*>(gen + kOffBar + 64);   // [128] global key
+  float* s_uk = reinterpret_cast<float*>(gen + kOffBar + 320);
+  float* s_sg = reinterpret_cast<float*>(gen + kOffBar + 512);                  // [128] raw q'.k_0
+  float* s_v0 = reinterpret_cast<float*>(gen + kOffBar + 1024);                 // [128] V row of frame 0
 
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * TQ;
   const int len = p.enc_len[b];
@@ -113,9 +92,10 @@ local_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qk, const __gri
   const size_t row0 = static_cast<size_t>(b) * p.T_max;
   __nv_bfloat16* obase = p.out + row0 * d + h * TDK;
 
-  const bool prof_cta = blockIdx.x == 1 && blockIdx.y == 0 && blockIdx.z == 0;
-  ATC_STAMP(threadIdx.x == 0, 0);
-  ATC_STAMP(threadIdx.x == 32, 8);
+#ifdef RS_PROF
+  const bool prof_cta = blockIdx.x == 1 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0;
+  if (prof_cta) g_atc_prof[0] = clock64();
+#endif
   if (q0 >= len) {                                   // fully padded tile: defined zeros
     for (int id = threadIdx.x; id < TQ * 16; id += blockDim.x) {
       const int r = id >> 4, c = (id & 15) * 8;
@@ -124,358 +104,238 @@ local_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qk, const __gri
     return;
   }
 
-  // key row blocks (128 keys each) that hold at least one key an in-range query of this tile may attend to
+  // key blocks (64 keys each) that hold at least one key an in-range query of this tile may attend to
   const int j_base = q0 - 128;
   const int q_hi = min(q0 + TQ, len) - 1;                                    // last valid query row of the tile
   const int key_lo = max(0, q0 - p.w_left), key_hi = min(len - 1, q_hi + p.w_right);
-  int rb_lo = (key_lo - j_base) >> 7, rb_hi = (key_hi - j_base) >> 7;        // inclusive, within [0, 2]
-  rb_lo = max(rb_lo, 0); rb_hi = min(rb_hi, 2);
-
-  const int n_rb = rb_hi - rb_lo + 1;
+  const int blk_lo = max((key_lo - j_base) >> 6, 0), blk_hi = min((key_hi - j_base) >> 6, kBlocks - 1);   // inclusive
   const uint32_t pos_slab = static_cast<uint32_t>(p.n_rel_pad) * 128u;          // bytes of one k-slab of the positional table
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tm_qk);
-      tma_prefetch_desc(&tm_vt);
-      tma_prefetch_desc(&tm_pos);
-      mbar_init(bar_qk, 1); mbar_init(bar_v, 1); mbar_init(bar_s, 1); mbar_init(bar_o, 1);
-      mbar_init(bar_bd, 1); mbar_init(bar_k, 1); mbar_init(bar_drained, kAtcThreads - 32); mbar_init(bar_p1, kAtcThreads - 32);
-      fence_barrier_init();
-      // ---- first loads (Q' and the head's positional table): issued before the tensor-memory allocation and the CTA-wide
-      // sync so they overlap both.  The table is two k-slabs of n_rel_pad rows, each fetched as two boxes of n_rel_pad / 2 rows.
-      ATC_STAMP(true, 1);
-      mbar_arrive_expect_tx(bar_qk, static_cast<uint32_t>(2 * kSlab + 2 * pos_slab));
-      for (int kb = 0; kb < 2; ++kb) {
-        tma_load_2d(base + kOffQ + kb * kSlab, &tm_qk, h * TDK + kb * 64, static_cast<int>(row0) + q0, bar_qk);
-        for (int hh = 0; hh < 2; ++hh)
-          tma_load_2d(base + kOffK + kb * pos_slab + hh * (pos_slab / 2), &tm_pos, kb * 64, h * p.n_rel_pad + hh * (p.n_rel_pad / 2), bar_qk);
-      }
+
+  if (threadIdx.x == 256) {
+    tma_prefetch_desc(&tm_q);
+    tma_prefetch_desc(&tm_k);
+    tma_prefetch_desc(&tm_vt);
+    tma_prefetch_desc(&tm_pos);
+    mbar_init(bar_qk, 1); mbar_init(bar_drained, 8);
+    for (int s = 0; s < kKvStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
+    fence_barrier_init();
+    // Q' and the head's positional table: two k-slabs of n_rel_pad rows, each fetched as two boxes of n_rel_pad / 2 rows
+    mbar_arrive_expect_tx(bar_qk, static_cast<uint32_t>(2 * kSlab + 2 * pos_slab));
+    for (int kb = 0; kb < 2; ++kb) {
+      tma_load_2d(base + kOffQ + kb * kSlab, &tm_q, h * TDK + kb * 64, static_cast<int>(row0) + q0, bar_qk);
+      for (int hh = 0; hh < 2; ++hh)
+        tma_load_2d(base + kOffKV + kb * pos_slab + hh * (pos_slab / 2), &tm_pos, kb * 64, h * p.n_rel_pad + hh * (p.n_rel_pad / 2), bar_qk);
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_slot);
   }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
+  if (warp == 8) {
+    // ---- producer: K / V^T blocks over the positional table once both warpgroups' BD products have retired
     if (lane == 0) {
-      // ---- BD = Q' P^T: two column halves of n_rel_pad / 2 (a multiple of 16, at most 144) per k16 step
-      constexpr uint32_t idesc = umma_idesc_bf16(128, 128);
-      mbar_wait(bar_qk, 0);
-      ATC_STAMP(true, 2);
-      tcgen05_fence_after();
-      {
-        const uint32_t idesc_bd = umma_idesc_bf16(128, p.n_rel_pad / 2);
-        for (int kb = 0; kb < 2; ++kb) {
-          const uint64_t da = umma_desc_k_sw128(base + kOffQ + kb * kSlab);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            for (int hh = 0; hh < 2; ++hh) {
-              const uint64_t db = umma_desc_k_sw128(base + kOffK + kb * pos_slab + hh * (pos_slab / 2));
-              umma_bf16_ss(tmem_base + hh * (p.n_rel_pad / 2), da + 2u * k, db + 2u * k, idesc_bd, (kb | k) != 0 ? 1u : 0u);
-            }
-        }
-        umma_commit(bar_bd);
-      }
-      // ---- K over the positional table once that product has retired
-      mbar_wait(bar_bd, 0);
-      mbar_arrive_expect_tx(bar_k, static_cast<uint32_t>(2 * n_rb * kSlab));
-      for (int kb = 0; kb < 2; ++kb)
-        for (int rb = rb_lo; rb <= rb_hi; ++rb)
-          tma_load_2d(base + kOffK + (kb * 3 + rb) * kSlab, &tm_qk, d + h * TDK + kb * 64, static_cast<int>(row0) + j_base + rb * 128, bar_k);
-      // ---- S = Q' K^T into the columns BD was drained from
       mbar_wait(bar_drained, 0);
-      mbar_wait(bar_k, 0);
-      tcgen05_fence_after();
-      for (int kb = 0; kb < 2; ++kb) {
-        const uint64_t da = umma_desc_k_sw128(base + kOffQ + kb * kSlab);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          for (int rb = rb_lo; rb <= rb_hi; ++rb) {
-            const uint64_t db = umma_desc_k_sw128(base + kOffK + (kb * 3 + rb) * kSlab);
-            umma_bf16_ss(tmem_base + rb * 128, da + 2u * k, db + 2u * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-        }
-      }
-      umma_commit(bar_s);
-      ATC_STAMP(true, 3);
-      // ---- V^T over the BD buffer once pass 1 has read it
-      mbar_wait(bar_p1, 0);
-      mbar_arrive_expect_tx(bar_v, static_cast<uint32_t>(2 * n_rb * kSlab));
-      for (int ks = 2 * rb_lo; ks <= 2 * rb_hi + 1; ++ks)
-        tma_load_2d(base + kOffV + ks * kSlab, &tm_vt, static_cast<int>(row0) + j_base + ks * 64, h * TDK, bar_v);
-    }
-    __syncwarp();
-  } else {
-    // ---- softmax warps: thread = (row r of the tile, column half)
-    const int qd = warp & 3, hf = (warp - 1) >> 2;
-    const int r = qd * 32 + lane, i = q0 + r;
-    const bool row_ok = i < len;
-    const float scale2 = rsqrtf(static_cast<float>(TDK)) * 1.4426950408889634f;       // 1/sqrt(dk) * log2(e)
-    float* s_max = reinterpret_cast<float*>(gen + kOffMax);
-    float* s_sum = reinterpret_cast<float*>(gen + kOffSum);
-    float* s_pg = reinterpret_cast<float*>(gen + kOffPg);
-    float* s_v0 = reinterpret_cast<float*>(gen + kOffV0);
-    const uint32_t t_row = tmem_base + (static_cast<uint32_t>(qd * 32) << 16);
-
-    // global token: score of its key against this row, without bias_u and without a positional term:
-    // (q' - u) . k_0 = q'.k_0 (per row, by the hf == 0 warps) - u.k_0 (one scalar per CTA, by warp 1)
-    float v0mine = 0.f;
-    float* s_sg = reinterpret_cast<float*>(gen + kOffBar + 512);                   // [128] raw q'.k_0
-    float* s_uk = reinterpret_cast<float*>(gen + kOffBar + 448);
-    if (p.n_global > 0) {
-      const int st = threadIdx.x - 32;                                             // 0..255
-      if (st < 16) *reinterpret_cast<uint4*>(s_k0 + st * 8) = __ldg(reinterpret_cast<const uint4*>(p.qk + row0 * p.ld_qk + d + h * TDK) + st);
-      if (st >= 128) v0mine = __bfloat162float(p.vt[static_cast<size_t>(h * TDK + (st - 128)) * p.ld_vt + row0]);   // V row of frame 0, one dim per thread
-      softmax_bar();
-      if (warp == 1) {
-        float uk = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) uk = fmaf(__ldg(p.bias_u + h * TDK + lane * 4 + e), __bfloat162float(s_k0[lane * 4 + e]), uk);
-        uk = warp_sum(uk);
-        if (lane == 0) *s_uk = uk;
-      }
-      if (hf == 0) {
-        mbar_wait(bar_qk, 0);                                                      // Q' has landed
-        float acc0 = 0.f, acc1 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          const uint4 qv = *reinterpret_cast<const uint4*>(gen + kOffQ + (c >> 3) * kSlab + sw128(r, c & 7));
-          const uint4 kv = *reinterpret_cast<const uint4*>(s_k0 + c * 8);
-          const uint32_t qw[4] = {qv.x, qv.y, qv.z, qv.w}, kw[4] = {kv.x, kv.y, kv.z, kv.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 q2 = unpack_bf16x2(qw[e]), k2 = unpack_bf16x2(kw[e]);
-            acc0 = fmaf(q2.x, k2.x, acc0); acc1 = fmaf(q2.y, k2.y, acc1);
-          }
-        }
-        s_sg[r] = acc0 + acc1;
+      int s = 0; uint32_t phase = 0;
+      for (int blk = blk_lo; blk <= blk_hi; ++blk) {
+        mbar_wait(empty_bar(s), phase ^ 1u);
+        mbar_arrive_expect_tx(full_bar(s), kKvStageBytes);
+        const uint32_t st = base + kOffKV + s * kKvStageBytes;
+        const int key0 = static_cast<int>(row0) + j_base + blk * KB;
+        for (int kb = 0; kb < 2; ++kb) tma_load_2d(st + kb * (KB * 128), &tm_k, d + h * TDK + kb * 64, key0, full_bar(s));
+        tma_load_2d(st + 2 * KB * 128, &tm_vt, key0, h * TDK, full_bar(s));
+        if (++s == kKvStages) { s = 0; phase ^= 1u; }
       }
     }
+    return;
+  }
 
-    // ---- drain the positional product: BD[r][c] = ((q' . p[c]) + bias[c]) / sqrt(dk) * log2 e as IEEE half, row-major
-    // [128][kBdPitch] in the region V^T will use later.  Thread (r, hf) takes half of the 32-column chunks of row r.
-    __half* s_bd = reinterpret_cast<__half*>(gen + kOffV);
+  // ---- consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile; a lane holds rows r0 and r1 = r0 + 8 of its warp's 16
+  const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
+  const int rbase = wg * 64 + (warp & 3) * 16;
+  const int r0 = rbase + g, r1 = r0 + 8;
+  const int i0 = q0 + r0, i1 = q0 + r1;
+  const bool ok0 = i0 < len, ok1 = i1 < len;
+  const float scale2 = rsqrtf(static_cast<float>(TDK)) * 1.4426950408889634f;       // 1/sqrt(dk) * log2(e)
+  __half* s_bd = reinterpret_cast<__half*>(gen + kOffBD);
+
+  // global token: score of its key against each row, without bias_u and without a positional term:
+  // (q' - u) . k_0 = q'.k_0 (per row, two threads each) - u.k_0 (one scalar per CTA, by warp 0)
+  float sg0 = -INFINITY, sg1 = -INFINITY;
+  if (p.n_global > 0) {
+    const int tid = threadIdx.x;                                                 // 0..255
+    if (tid < 16) *reinterpret_cast<uint4*>(s_k0 + tid * 8) = __ldg(reinterpret_cast<const uint4*>(p.qk + row0 * p.ld_qk + d + h * TDK) + tid);
+    if (tid >= 128) s_v0[tid - 128] = __bfloat162float(p.vt[static_cast<size_t>(h * TDK + (tid - 128)) * p.ld_vt + row0]);
+    named_bar_sync(1, 256);
+    if (warp == 0) {
+      float uk = 0.f;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) uk = fmaf(__ldg(p.bias_u + h * TDK + lane * 4 + e), __bfloat162float(s_k0[lane * 4 + e]), uk);
+      uk = warp_sum(uk);
+      if (lane == 0) *s_uk = uk;
+    }
+    mbar_wait(bar_qk, 0);                                                        // Q' has landed
     {
-      const int n_chunks = p.n_rel_pad >> 5;
-      const int c_lo = hf == 0 ? 0 : (n_chunks + 1) / 2, c_hi = hf == 0 ? (n_chunks + 1) / 2 : n_chunks;
-      // The head's positional bias (n_rel_pad floats) is parked in the 16 spare bytes at the end of the BD rows -- four floats
-      // in the padding of row k -- and read back below as broadcasts: fetching it from global memory inside the drain loop put
-      // an L1 / L2 round trip in front of every chunk (16 % of the kernel's stall samples, profiles/r02_attention_ncu.md).
-      {
-        const int st = threadIdx.x - 32;
-        if (st < (p.n_rel_pad >> 2))
-          *reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(s_bd) + st * (kBdPitch * 2) + kNrelPadMax * 2) =
-              __ldg(reinterpret_cast<const float4*>(p.bd_bias + h * p.n_rel_pad) + st);
-        softmax_bar();
-      }
-      const uint8_t* bias_rows = reinterpret_cast<const uint8_t*>(s_bd) + kNrelPadMax * 2;
-      mbar_wait(bar_bd, 0);
-      tcgen05_fence_after();
-#pragma unroll 1
-      for (int ch = c_lo; ch < c_hi; ++ch) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_row + ch * 32, v);
-        tmem_ld_wait();
-        uint4* dst = reinterpret_cast<uint4*>(s_bd + r * kBdPitch + ch * 32);
+      const int r = tid >> 1, hf = tid & 1;                                      // row, 64-column half
+      float acc0 = 0.f, acc1 = 0.f;
 #pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-          const float4 ba = *reinterpret_cast<const float4*>(bias_rows + (ch * 8 + q4 * 2) * (kBdPitch * 2));
-          const float4 bb = *reinterpret_cast<const float4*>(bias_rows + (ch * 8 + q4 * 2 + 1) * (kBdPitch * 2));
-          const float bq[8] = {ba.x, ba.y, ba.z, ba.w, bb.x, bb.y, bb.z, bb.w};
-          uint32_t w[4];
+      for (int c = 0; c < 8; ++c) {
+        const uint4 qv = *reinterpret_cast<const uint4*>(gen + kOffQ + hf * kSlab + sw128(r, c));
+        const uint4 kv = *reinterpret_cast<const uint4*>(s_k0 + hf * 64 + c * 8);
+        const uint32_t qw[4] = {qv.x, qv.y, qv.z, qv.w}, kw[4] = {kv.x, kv.y, kv.z, kv.w};
 #pragma unroll
-          for (int e = 0; e < 4; ++e)
-            w[e] = pack_f16x2((__uint_as_float(v[q4 * 8 + 2 * e]) + bq[2 * e]) * scale2, (__uint_as_float(v[q4 * 8 + 2 * e + 1]) + bq[2 * e + 1]) * scale2);
-          dst[q4] = make_uint4(w[0], w[1], w[2], w[3]);
+        for (int e = 0; e < 4; ++e) {
+          const float2 q2 = unpack_bf16x2(qw[e]), k2 = unpack_bf16x2(kw[e]);
+          acc0 = fmaf(q2.x, k2.x, acc0); acc1 = fmaf(q2.y, k2.y, acc1);
         }
       }
-      tcgen05_fence_before();
-      mbar_arrive(bar_drained);                          // the S product may overwrite these tensor-memory columns
+      float acc = acc0 + acc1;
+      acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+      if (hf == 0) s_sg[r] = acc;
     }
-    // rel_shift: key column jj of the window (rel = jj - 128 - r) is BD[r][jj - (128 - w_left) - r]; a chunk's 32 scores
-    // are 17 32-bit words of the row, realigned with a funnel shift where that start is odd
-    const uint32_t* bdwords = reinterpret_cast<const uint32_t*>(s_bd + r * kBdPitch);
-    float mx = -INFINITY;
-    unsigned live = 0;                                   // chunks of this warp that intersect the band
-    // rel = j - i = 32m + e - 128 - r; warp rows r in [32qd, 32qd+31]: the chunk matters to this warp iff ... (warp-uniform)
-    auto chunk_live = [&](int m) {
-      const int rel_max = 32 * m + 31 - 128 - 32 * qd, rel_min = 32 * m - 128 - 32 * qd - 31;
-      const int jl = j_base + 32 * m;
-      return !(rel_max < -p.w_left || rel_min > p.w_right || jl + 31 < 0 || jl >= len || (m >> 2) < rb_lo || (m >> 2) > rb_hi ||
-               q0 + 32 * qd >= len);                     // every row of this warp lies beyond the utterance (last tile)
-    };
-#pragma unroll
-    for (int k = 0; k < 6; ++k) live |= chunk_live(hf * 6 + k) ? (1u << k) : 0u;
-    unsigned todo = live;
-    ATC_STAMP(threadIdx.x == 32, 9);
-    mbar_wait(bar_s, 0);
-    ATC_STAMP(threadIdx.x == 32, 10);
-    tcgen05_fence_after();
-    softmax_bar();                                       // every warp is done reading Q' (global-key scores)
-    const float sg2 = p.n_global > 0 ? (s_sg[r] - *s_uk) * scale2 : -INFINITY;
-    // the Q' tile is dead now: its memory holds the row statistics and v_0
-    if (p.n_global > 0 && threadIdx.x - 32 >= 128) s_v0[threadIdx.x - 32 - 128] = v0mine;
+    named_bar_sync(1, 256);
+    sg0 = (s_sg[r0] - *s_uk) * scale2;
+    sg1 = (s_sg[r1] - *s_uk) * scale2;
+  } else {
+    mbar_wait(bar_qk, 0);
+  }
 
-    // ---- pass 1: t = (S + BD) * scale2 (log2 domain), masked; row maximum; t written back to tensor memory
+  const uint32_t q_addr = base + kOffQ + wg * (64 * 128);       // the warpgroup's 64 rows inside each k-slab of Q'
+  // ---- the positional product: BD[r][c] = ((q' . p[c]) + bias[c]) / sqrt(dk) * log2 e as IEEE half, row-major
 #pragma unroll 1
-    while (todo) {
-      const int k = __ffs(todo) - 1;
-      todo &= todo - 1;
-      const int m = hf * 6 + k;
-      const int jlo = j_base + 32 * m;
-      const int cs = 32 * m - (128 - p.w_left) - r;     // first BD column of the chunk for this row (may lie outside [0, n_rel): masked below)
-      const uint32_t* wp = bdwords + (cs >> 1);
-      const int sh = (cs & 1) * 16;
-      uint32_t braw[17];
+  for (int ch = 0; ch < (p.n_rel_pad >> 5); ++ch) {
+    float acc[16];
+    wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 17; ++c) braw[c] = wp[c];
-      // columns e of this chunk the row may attend to: band (-w_left <= j - i <= w_right) and 0 <= j < len
-      const int e_lo = max(max(128 + r - p.w_left - 32 * m, -jlo), 0);
-      const int e_hi = row_ok ? min(min(128 + r + p.w_right - 32 * m, len - 1 - jlo), 31) : -1;
-      const unsigned live_e = e_hi >= e_lo ? ((0xffffffffu >> (31 - e_hi)) & (0xffffffffu << e_lo)) : 0u;   // bit e: column e attended
-      uint32_t v[32];
-      tmem_ld_32x32(t_row + m * 32, v);
-      tmem_ld_wait();
+    for (int kb = 0; kb < 2; ++kb) {
+      const uint64_t da = wgmma_desc_k_sw128(q_addr + kb * kSlab);
+      const uint64_t db = wgmma_desc_k_sw128(base + kOffKV + kb * pos_slab + ch * 4096);
 #pragma unroll
-      for (int e = 0; e < 32; e += 2) {
-        const uint32_t pair = __funnelshift_r(braw[e >> 1], braw[(e >> 1) + 1], sh);
-        const float2 bdv = __half22float2(*reinterpret_cast<const __half2*>(&pair));
+      for (int k = 0; k < 4; ++k) wgmma_bf16_ss_n32(acc, da + 2u * k, db + 2u * k, (kb | k) != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int col = ch * 32 + 8 * j + 2 * t;
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bd_bias + h * p.n_rel_pad + col));
+      *reinterpret_cast<__half2*>(s_bd + r0 * kBdPitch + col) = __floats2half2_rn((acc[4 * j] + bb.x) * scale2, (acc[4 * j + 1] + bb.y) * scale2);
+      *reinterpret_cast<__half2*>(s_bd + r1 * kBdPitch + col) = __floats2half2_rn((acc[4 * j + 2] + bb.x) * scale2, (acc[4 * j + 3] + bb.y) * scale2);
+    }
+  }
+  __syncwarp();                                        // a warp reads back only the BD rows it wrote
+  if (lane == 0) mbar_arrive(bar_drained);             // the ring may overwrite the positional table
+
+  // keys the warpgroup's in-range rows may attend to
+  const int wrow_lo = q0 + wg * 64;
+  const bool wg_valid = wrow_lo < len;
+  const int wkey_lo = max(0, wrow_lo - p.w_left), wkey_hi = min(len - 1, min(wrow_lo + 64, len) - 1 + p.w_right);
+
+  float o[64];
+#pragma unroll
+  for (int e = 0; e < 64; ++e) o[e] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;      // running maxima (log2 domain) and this lane's partial row sums
+  const __half* bd0 = s_bd + r0 * kBdPitch + p.w_left - i0;      // BD column of key j for row i: j - i + w_left
+  const __half* bd1 = s_bd + r1 * kBdPitch + p.w_left - i1;
+  int s = 0; uint32_t phase = 0;
+#pragma unroll 1
+  for (int blk = blk_lo; blk <= blk_hi; ++blk) {
+    mbar_wait(full_bar(s), phase);
+    const int jlo = j_base + blk * KB;
+    if (wg_valid && jlo + KB - 1 >= wkey_lo && jlo <= wkey_hi) {          // warpgroup-uniform
+      const uint32_t st = base + kOffKV + s * kKvStageBytes;
+      float sc[32];
+      wgmma_fence();
+#pragma unroll
+      for (int kb = 0; kb < 2; ++kb) {
+        const uint64_t da = wgmma_desc_k_sw128(q_addr + kb * kSlab);
+        const uint64_t db = wgmma_desc_k_sw128(st + kb * (KB * 128));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_bf16_ss_n64(sc, da + 2u * k, db + 2u * k, (kb | k) != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // t = S * scale2 + BD (pre-scaled), masked to the band (-w_left <= j - i <= w_right) and to 0 <= j < len
+      float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
-          const bool ok = (live_e >> (e + q)) & 1u;
-          const float t = ok ? fmaf(__uint_as_float(v[e + q]), scale2, q == 0 ? bdv.x : bdv.y) : -INFINITY;   // BD arrives pre-scaled
-          mx = fmaxf(mx, t);
-          v[e + q] = __float_as_uint(t);
+          const int ja = jlo + 8 * j + 2 * t + q;
+          const bool in = ja >= 0 && ja < len;
+          const bool a0 = in && ok0 && ja - i0 >= -p.w_left && ja - i0 <= p.w_right;
+          const bool a1 = in && ok1 && ja - i1 >= -p.w_left && ja - i1 <= p.w_right;
+          const float t0 = a0 ? fmaf(sc[4 * j + q], scale2, __half2float(bd0[ja])) : -INFINITY;
+          const float t1 = a1 ? fmaf(sc[4 * j + 2 + q], scale2, __half2float(bd1[ja])) : -INFINITY;
+          sc[4 * j + q] = t0; sc[4 * j + 2 + q] = t1;
+          mx0 = fmaxf(mx0, t0); mx1 = fmaxf(mx1, t1);
         }
       }
-      tmem_st_32x32(t_row + m * 32, v);
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      const float n0 = fmaxf(m0, mx0), n1 = fmaxf(m1, mx1);
+      const float c0 = m0 == -INFINITY ? 0.f : ex2f(m0 - n0), c1 = m1 == -INFINITY ? 0.f : ex2f(m1 - n1);
+      const float ref0 = n0 == -INFINITY ? 0.f : n0, ref1 = n1 == -INFINITY ? 0.f : n1;
+      m0 = n0; m1 = n1;
+      l0 *= c0; l1 *= c1;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) { o[4 * j] *= c0; o[4 * j + 1] *= c0; o[4 * j + 2] *= c1; o[4 * j + 3] *= c1; }
+      // p = exp2(t - m) as bf16 (row sums of the rounded values), handed to the P.V product as its A fragments
+      uint32_t pa[4][4];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t w0 = pack_bf16x2(ex2f(sc[4 * j] - ref0), ex2f(sc[4 * j + 1] - ref0));
+        const uint32_t w1 = pack_bf16x2(ex2f(sc[4 * j + 2] - ref1), ex2f(sc[4 * j + 3] - ref1));
+        const float2 b0 = unpack_bf16x2(w0), b1 = unpack_bf16x2(w1);
+        l0 += b0.x + b0.y; l1 += b1.x + b1.y;
+        pa[j >> 1][(j & 1) * 2] = w0; pa[j >> 1][(j & 1) * 2 + 1] = w1;
+      }
+      wgmma_fence();
+      const uint64_t dv = wgmma_desc_k_sw128(st + 2 * KB * 128);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_bf16_rs_n128(o, pa[kk], dv + 2u * kk, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-    tmem_st_wait();
-    ATC_STAMP(threadIdx.x == 32, 11);
-    s_max[hf * 128 + r] = mx;
-    fence_proxy_async();                                 // BD was written and read through the generic proxy; V^T arrives through the async proxy
-    mbar_arrive(bar_p1);                                 // the BD buffer is dead for this thread: V^T may land on it
-    softmax_bar();
-    float m_row = fmaxf(fmaxf(s_max[r], s_max[128 + r]), sg2);
-    if (m_row == -INFINITY) m_row = 0.f;
-    // ---- pass 2: p = exp2(t - m) as bf16 into the (dead) K tile, K-major swizzled; row sums of the rounded values
-    float sum = 0.f;
-#pragma unroll 1
-    for (int m = hf * 6; m < hf * 6 + 6; ++m) {
-      uint8_t* slab = gen + kOffK + (m >> 1) * kSlab;
-      const int cc0 = (m & 1) * 4;
-      if (!((live >> (m - hf * 6)) & 1u)) {
-        if ((m >> 2) >= rb_lo && (m >> 2) <= rb_hi) {      // the P.V product reads this slab: it must hold zeros
-#pragma unroll
-          for (int c = 0; c < 4; ++c) *reinterpret_cast<uint4*>(slab + sw128(r, cc0 + c)) = make_uint4(0, 0, 0, 0);
-        }
-        continue;
-      }
-      uint32_t v[32];
-      tmem_ld_32x32(t_row + m * 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t w[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float p0 = ex2f(__uint_as_float(v[c * 8 + 2 * e]) - m_row), p1 = ex2f(__uint_as_float(v[c * 8 + 2 * e + 1]) - m_row);
-          w[e] = pack_bf16x2(p0, p1);
-          const float2 back = unpack_bf16x2(w[e]);
-          sum += back.x + back.y;
-        }
-        *reinterpret_cast<uint4*>(slab + sw128(r, cc0 + c)) = make_uint4(w[0], w[1], w[2], w[3]);
-      }
-    }
-    ATC_STAMP(threadIdx.x == 32, 12);
-    s_sum[hf * 128 + r] = sum;
-    if (hf == 0) s_pg[r] = (p.n_global > 0 && row_ok) ? ex2f(sg2 - m_row) : 0.f;
-    fence_proxy_async();                                 // P was written through the generic proxy, UMMA reads it through the async proxy
-    tcgen05_fence_before();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty_bar(s));
+    if (++s == kKvStages) { s = 0; phase ^= 1u; }
   }
-  __syncthreads();
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ---- O = P V
-      constexpr uint32_t idesc = umma_idesc_bf16(128, 128);
-      ATC_STAMP(true, 4);
-      mbar_wait(bar_v, 0);
-      tcgen05_fence_after();
-      bool first = true;
-      for (int ks = 2 * rb_lo; ks <= 2 * rb_hi + 1; ++ks) {
-        const uint64_t da = umma_desc_k_sw128(base + kOffK + ks * kSlab);
-        const uint64_t db = umma_desc_k_sw128(base + kOffV + ks * kSlab);
+  // ---- epilogue: O + p_global * v_0, divided by the row sum -> bf16
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  float pg0 = 0.f, pg1 = 0.f;
+  if (p.n_global > 0) {
+    const float f0 = fmaxf(m0, sg0), f1 = fmaxf(m1, sg1);
+    const float c0 = m0 == -INFINITY ? 0.f : ex2f(m0 - f0), c1 = m1 == -INFINITY ? 0.f : ex2f(m1 - f1);
+    pg0 = ok0 ? ex2f(sg0 - f0) : 0.f; pg1 = ok1 ? ex2f(sg1 - f1) : 0.f;
+    l0 = l0 * c0 + pg0; l1 = l1 * c1 + pg1;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          umma_bf16_ss(tmem_base + TK, da + 2u * k, db + 2u * k, idesc, first ? 0u : 1u);
-          first = false;
-        }
-      }
-      umma_commit(bar_o);
-      ATC_STAMP(true, 5);
-    }
-    __syncwarp();
-  } else {
-    // ---- epilogue: warp (qd, hf) owns rows 32qd.. and output columns [64hf, 64hf + 64)
-    const int qd = warp & 3, hf = (warp - 1) >> 2;
-    const int r = qd * 32 + lane, i = q0 + r;
-    const float* s_sum = reinterpret_cast<const float*>(gen + kOffSum);
-    const float* s_pg = reinterpret_cast<const float*>(gen + kOffPg);
-    const float* s_v0 = reinterpret_cast<const float*>(gen + kOffV0);
-    const float pg = s_pg[r];
-    const float l = s_sum[r] + s_sum[128 + r] + pg;
-    const float inv = (i < len && l > 0.f) ? 1.0f / l : 0.f;
-    ATC_STAMP(threadIdx.x == 32, 13);
-    mbar_wait(bar_o, 0);
-    ATC_STAMP(threadIdx.x == 32, 14);
-    tcgen05_fence_after();
-    // staging: the P region is dead once bar_o has completed
-    __nv_bfloat16* stage = reinterpret_cast<__nv_bfloat16*>(gen + kOffK) + static_cast<size_t>(warp - 1) * 32 * kStagePitch;
-#pragma unroll
-    for (int half2 = 0; half2 < 2; ++half2) {
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(qd * 32) << 16) + TK + hf * 64 + half2 * 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t w[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int col = hf * 64 + half2 * 32 + c * 8 + 2 * e;
-          const float x = (__uint_as_float(v[c * 8 + 2 * e]) + pg * s_v0[col]) * inv;
-          const float y = (__uint_as_float(v[c * 8 + 2 * e + 1]) + pg * s_v0[col + 1]) * inv;
-          w[e] = pack_bf16x2(x, y);
-        }
-        *reinterpret_cast<uint4*>(stage + lane * kStagePitch + half2 * 32 + c * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-      }
-    }
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 8; ++it) {                      // 4 rows x 128 B per instruction
-      const int rr = it * 4 + (lane >> 3), cc = (lane & 7) * 8;
-      const int row = q0 + qd * 32 + rr;
-      const uint4 a = *reinterpret_cast<const uint4*>(stage + rr * kStagePitch + cc);
-      if (row < p.T_max) *reinterpret_cast<uint4*>(obase + static_cast<size_t>(row) * d + hf * 64 + cc) = a;
-    }
-    tcgen05_fence_before();
-    ATC_STAMP(threadIdx.x == 32, 15);
+    for (int j = 0; j < 16; ++j) { o[4 * j] *= c0; o[4 * j + 1] *= c0; o[4 * j + 2] *= c1; o[4 * j + 3] *= c1; }
   }
-  __syncthreads();
-  if (warp == 0) {
-    __syncwarp();
-    tcgen05_fence_after();
-    tmem_dealloc<512>(tmem_base);
-    ATC_STAMP(lane == 0, 6);
+  const float inv0 = (ok0 && l0 > 0.f) ? 1.0f / l0 : 0.f, inv1 = (ok1 && l1 > 0.f) ? 1.0f / l1 : 0.f;
+  __syncwarp();                                        // the warp's BD rows are dead: they stage its 16 output rows
+  __nv_bfloat16* stage = reinterpret_cast<__nv_bfloat16*>(s_bd + rbase * kBdPitch);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int col = 8 * j + 2 * t;
+    const float v0a = p.n_global > 0 ? s_v0[col] : 0.f, v0b = p.n_global > 0 ? s_v0[col + 1] : 0.f;
+    *reinterpret_cast<uint32_t*>(stage + g * kOutPitch + col) = pack_bf16x2((o[4 * j] + pg0 * v0a) * inv0, (o[4 * j + 1] + pg0 * v0b) * inv0);
+    *reinterpret_cast<uint32_t*>(stage + (g + 8) * kOutPitch + col) = pack_bf16x2((o[4 * j + 2] + pg1 * v0a) * inv1, (o[4 * j + 3] + pg1 * v0b) * inv1);
   }
+  __syncwarp();
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {                      // 2 rows x 256 B per instruction
+    const int rr = it * 2 + (lane >> 4), cc = (lane & 15) * 8;
+    const int row = q0 + rbase + rr;
+    const uint4 a = *reinterpret_cast<const uint4*>(stage + rr * kOutPitch + cc);
+    if (row < p.T_max) *reinterpret_cast<uint4*>(obase + static_cast<size_t>(row) * d + cc) = a;
+  }
+#ifdef RS_PROF
+  if (prof_cta) g_atc_prof[6] = clock64();
+#endif
 }
 
 // Row(s) of the global token(s): full attention softmax_j((q_g / sqrt(dk)) . k_j) v_j, no positional terms.
-// Same arithmetic as attention.cu::global_row_attention_kernel on the layouts of the tensor-core path: the query row
+// On the layouts of the tensor-core path: the query row
 // holds q + pos_bias_u (subtracted again here) and V is read from its transposed copy (keys contiguous).
 // grid (H, B), 256 threads.
 __global__ void __launch_bounds__(256)
@@ -527,7 +387,7 @@ global_row_attention_tc_kernel(const AtcDev p) {
   const float inv = 1.0f / (((red[0] + red[1]) + (red[2] + red[3])) + ((red[4] + red[5]) + (red[6] + red[7])));
   // out[dim] = sum_j p_j V^T[dim][j]: thread = (dim, one of two key segments); it walks its V^T row eight keys (16 bytes)
   // at a time with four loads in flight (the last, partial group of eight goes key by key: what follows the utterance in
-  // V^T is not this kernel's to read).  A warp-per-dim version with shuffle reductions took 40 us per launch.
+  // V^T is not this kernel's to read).
   __syncthreads();
   const __nv_bfloat16* vt = p.vt + static_cast<size_t>(h * TDK) * p.ld_vt + row0;
   const int len8 = ((row0 & 7) == 0) ? (len & ~7) : 0;
@@ -606,10 +466,11 @@ cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t stream) {
   p.bd_bias = a.bd_bias; p.bias_u = a.bias_u; p.out = static_cast<__nv_bfloat16*>(a.out);
   p.enc_len = a.enc_len; p.T_max = a.T_max; p.H = a.H; p.w_left = a.w_left; p.w_right = a.w_right;
   p.n_global = a.n_global; p.n_rel_pad = a.n_rel_pad; p.ld_qk = 3 * d; p.ld_vt = a.ld_vt;
-  CUtensorMap tm_qk, tm_vt, tm_pos;
+  CUtensorMap tm_q, tm_k, tm_vt, tm_pos;
   // positional table [H * n_rel_pad, 128] bf16, fetched in boxes of n_rel_pad / 2 rows (<= 144; a TMA box holds at most 256)
   if (!make_map(&tm_pos, a.pos, static_cast<uint64_t>(a.H) * a.n_rel_pad, TDK, TDK, static_cast<uint32_t>(a.n_rel_pad / 2))) return cudaErrorInvalidValue;
-  if (!make_map(&tm_qk, p.qk, static_cast<uint64_t>(M), static_cast<uint64_t>(2 * d), static_cast<uint64_t>(p.ld_qk))) return cudaErrorInvalidValue;
+  if (!make_map(&tm_q, p.qk, static_cast<uint64_t>(M), static_cast<uint64_t>(2 * d), static_cast<uint64_t>(p.ld_qk))) return cudaErrorInvalidValue;
+  if (!make_map(&tm_k, p.qk, static_cast<uint64_t>(M), static_cast<uint64_t>(2 * d), static_cast<uint64_t>(p.ld_qk), KB)) return cudaErrorInvalidValue;
   if (!make_map(&tm_vt, p.vt, static_cast<uint64_t>(d), static_cast<uint64_t>(M), static_cast<uint64_t>(p.ld_vt))) return cudaErrorInvalidValue;
   static DeviceOnce attr_once;
   if (attr_once.pending()) {
@@ -620,7 +481,7 @@ cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t stream) {
     attr_once.set();
   }
   const dim3 grid((a.T_max + TQ - 1) / TQ, a.H, a.B);
-  local_attention_tc_kernel<<<grid, kAtcThreads, kAtcSmem, stream>>>(tm_qk, tm_vt, tm_pos, p);
+  local_attention_tc_kernel<<<grid, kAtcThreads, kAtcSmem, stream>>>(tm_q, tm_k, tm_vt, tm_pos, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   if (a.n_global > 0) {

@@ -4,8 +4,8 @@
 // info", :38-40 the leading blank of y_sequence, :48 step - idx - 1).  Semantics restated in oracle/alsd_restated.py.
 //
 // One step = one anti-diagonal i = t + u of the (frame, token) lattice for every utterance at once.  The three matrix products
-// of a step (joint logits of the live hypotheses, LSTM gates and joint.pred of the newly extended ones) go through the tcgen05
-// GEMM of gemm_tcgen05.cu with their fp32 activations split into three bf16 terms (24 mantissa bits against bf16-exact
+// of a step (joint logits of the live hypotheses, LSTM gates and joint.pred of the newly extended ones) go through the wgmma
+// GEMM of gemm_wgmma.cu with their fp32 activations split into three bf16 terms (24 mantissa bits against bf16-exact
 // weights: fp32-accurate log-probabilities, so that beam decisions move only with the encoder's rounding, not the decoder's);
 // this file holds the kernels in between:
 //

@@ -11,13 +11,13 @@
 //  2. With kFrames x B rows per iteration the joint is a real (small) GEMM.  The CTAs form a 2-D grid,
 //     kGroups utterance groups x S vocabulary slices: a CTA keeps its ~82 rows of W_out in shared memory
 //     for the whole decode and multiplies them with the relu(enc_proj + pred_proj) rows of its group
-//     (32 rows per pass) on tcgen05 (see the kernel's comment).  Activations keep 22 mantissa bits: every fp32 value is
+//     (32 rows per pass) on wgmma (see the kernel's comment).  Activations keep 22 mantissa bits: every fp32 value is
 //     split into two IEEE-half terms (hi + lo), the bf16 weights are exact in half, accumulation is fp32.
 //     The LSTM step and joint.pred of the utterances that emitted are the same kind of GEMM (rows =
 //     utterances, K split over the warps, A fragments loaded straight from L2) on mma.sync m16n8k16.
 //  3. The input half of the LSTM gates depends on the emitted token only: W_ih . embed[k] + b_ih + b_hh is a table
 //     [V+1, 4*Hp] built once at load time (pred.gate_tab), so a step multiplies just the recurrent half W_hh . h -- half the
-//     shared memory, half the MMAs, and half of what every CTA pulls through L2 per step (all 148 CTAs read every
+//     shared memory, half the MMAs, and half of what every CTA pulls through L2 per step (all CTAs read every
 //     emitting utterance's full input vector: that traffic, not the arithmetic, is what the phase costs).
 //
 //   phase J  kGroups x S CTAs: window logits of the CTA's vocabulary slice -> per (utterance, frame) a grid-wide
@@ -54,9 +54,8 @@ struct SpecDev {
 };
 
 // Grid barrier over kBarCounters arrival counters, each in its own 128-byte line: CTA i arrives on counter i % kBarCounters,
-// threads 0..kBarCounters-1 each poll one counter.  All 148 arrivals on ONE address are serialised by the L2 slice that
-// owns it (the barrier then costs ~1.5 us, three times per decode iteration); spread over several lines they proceed in
-// parallel.  `round` counts the barriers passed; counter c has seen round * (number of CTAs with i % kBarCounters == c) arrivals.
+// threads 0..kBarCounters-1 each poll one counter.  Arrivals of every CTA on ONE address are serialised by the L2 slice that
+// owns it, three times per decode iteration; spread over several lines they proceed in parallel.  `round` counts the barriers passed; counter c has seen round * (number of CTAs with i % kBarCounters == c) arrivals.
 constexpr int kBarCounters = 8;
 constexpr int kBarStride = 32;            // unsigned ints between counters
 __device__ __forceinline__ void sp_grid_barrier(unsigned int* counters, unsigned int& round, unsigned int nblocks) {
@@ -89,8 +88,7 @@ __device__ __forceinline__ void mma_f16_16816(float (&d)[4], const uint32_t (&a)
 }
 
 // fp32 pair -> two IEEE-half pairs with hi + lo == x to 22 mantissa bits (11 + 11): the residual x - hi is exact in
-// fp32 and is itself rounded to half.  The legacy tensor path issues one m16n8k16 per ~19 cycles and scheduler on
-// sm_100, so the number of terms is what the joint costs; three bf16 terms (24 bits) were 1.5x slower.
+// fp32 and is itself rounded to half.  The number of terms is what the joint costs: two half terms, not three bf16 ones.
 // Magnitudes are clamped to the largest finite half before each conversion, which extends the exactly covered
 // range to |x| <= 2 * 65504; a transducer joint / LSTM input beyond that is outside what NeMo itself runs in fp16 AMP.
 __device__ __forceinline__ void split2(float2 x, uint32_t& hi, uint32_t& lo) {
@@ -118,26 +116,19 @@ __device__ __forceinline__ unsigned long long pack_best(float v, int row) {
   return (static_cast<unsigned long long>(fb) << 32) | (0xffffffffu - static_cast<unsigned int>(row));   // ties -> lower row
 }
 
-// The joint window runs on tcgen05.  A = the CTA's W_out rows as IEEE half in
-// 128B-swizzled K-major slabs of 64 columns (88 rows stored per slab; the M = 128 instruction reads on into the next slab /
-// region, whose rows land in accumulator lanes nobody looks at), B = the 32 (utterance, frame) activation rows as two half
-// planes (hi, lo) staged one k-half at a time, D = [128 vocabulary rows x (32 hi | 32 lo)] fp32 in tensor memory.  40 UMMAs
-// of 128x64x16 per pass replace 1760 mma.sync per CTA, which were issue-bound on the legacy path (~19 cycles each).
+// The joint window runs on wgmma.  A = the CTA's W_out rows as IEEE half in 128B-swizzled K-major slabs of 64 columns
+// (88 rows stored per slab; the two warpgroups' m64 instructions cover 128 rows and read on into the next slab / region,
+// whose rows land in accumulator rows nobody looks at), B = the 32 (utterance, frame) activation rows as two half planes
+// (hi, lo) staged one k-half at a time, D = [128 vocabulary rows x (32 hi | 32 lo)] fp32 in registers.
 // The hi and lo planes of the activations sit side by side as ONE B tile of 64 rows (rows 0-31 hi, 32-63 lo), so a k16 step
-// is one 128x64x16 UMMA and the two halves of D are added in the epilogue: small-N UMMAs cost about the same per
-// instruction as wider ones, so 80 instructions of N=32 took twice as long as 40 of N=64.
-constexpr uint32_t kIdescF16_128x64 = (1u << 4) | ((64u >> 3) << 17) | ((128u >> 4) << 24);   // D=f32, A=B=f16, K-major
-
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  umma_bf16_ss(tmem_d, desc_a, desc_b, idesc, accumulate);      // same instruction (kind::f16); the operand formats live in idesc
-}
+// is one m64n64k16 per warpgroup and the two halves of D are added in the epilogue.
+static_assert(kSpThreads == 256, "the joint is issued by two warpgroups");
 
 template <int HJ, int HP>
 __global__ void __launch_bounds__(kSpThreads, 1)
 rnnt_greedy_spec_kernel(const SpecDev p) {
   constexpr int KH = HJ / 2;                 // joint k-half staged in shared memory at a time
   constexpr int LS = HP + 8;                 // W_hh row stride in halves
-  constexpr int KS_H = KH / 16;              // k16 steps per joint half
   constexpr int KSW_L = (HP / 16) / kSpWarps;       // k16 steps per warp, LSTM (recurrent half only)
   constexpr int KSW_P = (HP / 16) / kSpWarps;       // k16 steps per warp, joint.pred
   constexpr int V4_ROW = KH / 4;             // float4 per staged row
@@ -182,15 +173,12 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   float* s_bout = reinterpret_cast<float*>(gB + kBRegion);                            // -inf beyond nj
   constexpr int n_bout = 128;
   float* s_c = s_bout + n_bout;                                                      // [B][units]
-  unsigned long long* s_best = reinterpret_cast<unsigned long long*>(s_c + ((static_cast<size_t>(B) * p.units + 1) & ~static_cast<size_t>(1)));   // [32][4]
-  int* s_t = reinterpret_cast<int*>(s_best + kPassRows * 4);
+  unsigned long long* s_best = reinterpret_cast<unsigned long long*>(s_c + ((static_cast<size_t>(B) * p.units + 1) & ~static_cast<size_t>(1)));   // [32][kSpWarps]
+  int* s_t = reinterpret_cast<int*>(s_best + kPassRows * kSpWarps);
   int* s_sym = s_t + B; int* s_n = s_sym + B; int* s_par = s_n + B; int* s_tok = s_par + B;
   int* s_emit = s_tok + B; int* s_len = s_emit + B;
   int* s_act = s_len + B;                                                            // ordered list of the utterances with frames left
   int* s_cnt = s_act + B;                                                            // [0] n_emit, [1] n_active, [2..2+8) warp counts x2
-  // one mbarrier (MMA completion) + the tensor-memory slot, 8-byte aligned after s_cnt
-  const uint32_t tc_bar = (smem_u32(s_cnt + 2 + 2 * kSpWarps) + 7u) & ~7u;
-  const uint32_t tc_slot = tc_bar + 8;
 
   {
     const uint32_t zero = 0;
@@ -202,7 +190,6 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
         if (r < nj) v = bf16x8_to_f16x8(reinterpret_cast<const uint4*>(p.w_out + static_cast<size_t>(j0 + r) * HJ)[c]);
         *reinterpret_cast<uint4*>(gA + (c >> 3) * a_slab + (r >> 3) * 1024 + (r & 7) * 128 + (((c & 7) ^ (r & 7)) << 4)) = v;
       }
-      if (tid == 0) { mbar_init(tc_bar, 1); fence_barrier_init(); }
     }
     for (int i = tid; i < 4 * p.units * (HP / 8); i += kSpThreads) {      // the W_hh half of [W_ih | W_hh]
       const int r = i / (HP / 8), c = i % (HP / 8);
@@ -224,19 +211,12 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     }
     if (tid == 0) { s_cnt[0] = B; s_cnt[1] = 0; }
   }
-  uint32_t tmem_d = 0, mma_phase = 0;
-  if (warp == 0) tmem_alloc<64>(tc_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_d) : "r"(tc_slot));
 
   unsigned int target = 0;
   int iter = 0;
   long long prof[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  // per-phase cycle counters of CTA 0 (rs_debug_decode_cycles).  They stay in the shipped kernel: on the same box, three alternating
-  // runs each, the kernel compiled WITH them decodes the bench batch in 5.30-5.35 ms and the one without in 5.62-5.70 ms (238 against
-  // 231 registers: the counters change the schedule ptxas picks, not the work; profiles/r02_ab.md).  -DRS_NO_DECODE_COUNTERS drops them.
+  // per-phase cycle counters of CTA 0 (rs_debug_decode_cycles); -DRS_NO_DECODE_COUNTERS drops them.
 #ifndef RS_NO_DECODE_COUNTERS
   auto tick = [&](int slot, long long& t0) { if (cta == 0 && tid == 0) { const long long t1 = clock64(); prof[slot] += t1 - t0; t0 = t1; } };
   long long tk = clock64();
@@ -445,7 +425,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
         const unsigned mask = __ballot_sync(0xffffffffu, row_b >= 0);
         if (mask == 0u) continue;                             // identical in every warp of the CTA
         // loader item = (utterance of the pass, float4 column): pred_proj is fetched once for the four frames of a window
-        // and the item order is rotated by the vocabulary-slice index so the 37 CTAs of a group, which all need the same
+        // and the item order is rotated by the vocabulary-slice index so the CTAs of a group, which all need the same
         // rows, do not ask L2 for the same lines at the same instant
         float4 gv[PERU][kFrames];
         auto load_half = [&](int h) {
@@ -483,7 +463,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
         auto jtick = [&](int) {};
 #endif
         {
-          // ---- tcgen05 joint: D[vocabulary row, (utterance, frame) row] in tensor memory
+          // ---- wgmma joint: D[vocabulary row, (utterance, frame) row]; warpgroup wgi holds vocabulary rows [64 wgi, +64)
           auto write_planes = [&]() {                         // gv -> two IEEE-half planes, 128B-swizzled K-major, 32 rows per slab
 #pragma unroll
             for (int i = 0; i < PERU; ++i) {
@@ -506,68 +486,60 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
               }
             }
           };
-          auto issue_half = [&](int h) {                      // one thread: NSLAB_H slabs x 4 k16 steps, N = 64 (hi | lo)
-            tcgen05_fence_after();
+          float dj[32];
+          const uint32_t a_rows = static_cast<uint32_t>(warp >> 2) * (64u * 128u);
+          auto issue_half = [&](int h) {                      // both warpgroups: NSLAB_H slabs x 4 k16 steps, N = 64 (hi | lo)
+            wgmma_fence();
 #pragma unroll 1
             for (int sl = 0; sl < NSLAB_H; ++sl) {
-              const uint64_t da = umma_desc_k_sw128(tc_base + static_cast<uint32_t>(h * NSLAB_H + sl) * a_slab);
-              const uint64_t db = umma_desc_k_sw128(tc_base + b_off + sl * kBSlab);
+              const uint64_t da = wgmma_desc_k_sw128(tc_base + static_cast<uint32_t>(h * NSLAB_H + sl) * a_slab + a_rows);
+              const uint64_t db = wgmma_desc_k_sw128(tc_base + b_off + sl * kBSlab);
 #pragma unroll
               for (int k = 0; k < 4; ++k)
-                umma_f16_ss(tmem_d, da + 2u * k, db + 2u * k, kIdescF16_128x64, (h | sl | k) != 0 ? 1u : 0u);
+                wgmma_f16_ss_n64(dj, da + 2u * k, db + 2u * k, (h | sl | k) != 0 ? 1u : 0u);
             }
-            umma_commit(tc_bar);
+            wgmma_commit();
           };
           load_half(0);
           write_planes();
           fence_proxy_async();
-          tcgen05_fence_before();
           __syncthreads();
           jtick(8);
-          if (tid == 0) issue_half(0);
-          __syncwarp();
+          issue_half(0);
           load_half(1);                                       // in flight under the MMAs of half 0
-          mbar_wait(tc_bar, mma_phase); mma_phase ^= 1u;      // half 0 consumed: the planes may be rewritten
+          wgmma_wait<0>();
+          __syncthreads();                                    // half 0 consumed by both warpgroups: the planes may be rewritten
           write_planes();
           fence_proxy_async();
-          tcgen05_fence_before();
           __syncthreads();
-          if (tid == 0) issue_half(1);
-          __syncwarp();
-          mbar_wait(tc_bar, mma_phase); mma_phase ^= 1u;
-          tcgen05_fence_after();
+          issue_half(1);
+          wgmma_wait<0>();
           jtick(9);
-          // ---- argmax over the vocabulary rows (= TMEM lanes) per (utterance, frame) column: warp w holds rows 32w..32w+31
-          if (warp < 4) {
-            uint32_t v[32], vlo[32];
-            tmem_ld_32x32(tmem_d + (static_cast<uint32_t>(warp * 32) << 16), v);          // A . hi
-            tmem_ld_32x32(tmem_d + (static_cast<uint32_t>(warp * 32) << 16) + 32, vlo);   // A . lo
-            tmem_ld_wait();
-            const int rr = warp * 32 + lane;
-            const bool rvalid = rr < nj;
-            const float bias = s_bout[rr];
-            unsigned my_key = 0; int my_row = 0x7fffffff;
+          // ---- argmax over the vocabulary rows per (utterance, frame) column.  A lane holds rows rr and rr + 8 of its warp's
+          // 16 and columns 8j + 2t, +1 (j < 4: A . hi, j + 4: A . lo); the eight lanes with the same t cover the warp's rows.
+          {
+            const int rr = (warp >> 2) * 64 + (warp & 3) * 16 + gid;
+            const bool v0 = rr < nj, v1 = rr + 8 < nj;
+            const float bias0 = s_bout[rr], bias1 = s_bout[rr + 8];
 #pragma unroll
-            for (int c = 0; c < 32; ++c) {
-              unsigned fb = __float_as_uint((__uint_as_float(v[c]) + __uint_as_float(vlo[c])) + bias);
-              fb = (fb & 0x80000000u) ? ~fb : (fb | 0x80000000u);               // order-preserving
-              const unsigned key = rvalid ? fb : 0u;
-              const unsigned mk = __reduce_max_sync(0xffffffffu, key);
-              const unsigned cand = (key == mk && rvalid) ? static_cast<unsigned>(rr) : 0x7fffffffu;
-              const unsigned mr = __reduce_min_sync(0xffffffffu, cand);         // ties -> lower row
-              if (lane == c) { my_key = mk; my_row = static_cast<int>(mr); }
+            for (int j = 0; j < 4; ++j) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                unsigned long long k0 = v0 ? pack_best((dj[4 * j + e] + dj[4 * (j + 4) + e]) + bias0, j0 + rr) : 0ull;
+                const unsigned long long k1 = v1 ? pack_best((dj[4 * j + 2 + e] + dj[4 * (j + 4) + 2 + e]) + bias1, j0 + rr + 8) : 0ull;
+                k0 = k1 > k0 ? k1 : k0;                       // higher logit first, ties -> lower row
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1) { const unsigned long long ot = __shfl_xor_sync(0xffffffffu, k0, o); k0 = ot > k0 ? ot : k0; }
+                if (gid == 0) s_best[(8 * j + 2 * tig + e) * kSpWarps + warp] = k0;
+              }
             }
-            s_best[lane * 4 + warp] = (my_row != 0x7fffffff && my_key != 0u)
-                                          ? ((static_cast<unsigned long long>(my_key) << 32) | (0xffffffffu - static_cast<unsigned>(j0 + my_row)))
-                                          : 0ull;
           }
-          tcgen05_fence_before();
         }
         __syncthreads();
         if (warp == 0 && row_b >= 0) {
-          unsigned long long m = s_best[lane * 4];
+          unsigned long long m = s_best[lane * kSpWarps];
 #pragma unroll
-          for (int q = 1; q < 4; ++q) { const unsigned long long o = s_best[lane * 4 + q]; m = o > m ? o : m; }
+          for (int q = 1; q < kSpWarps; ++q) { const unsigned long long o = s_best[lane * kSpWarps + q]; m = o > m ? o : m; }
           asm volatile("red.relaxed.gpu.global.max.u64 [%0], %1;" ::"l"(p.best + (static_cast<size_t>(iter % 3) * B + row_b) * kFrames + (lane % kFrames)), "l"(m) : "memory");
         }
         jtick(10);
@@ -624,9 +596,6 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   }
   if (cta == 0) for (int b = tid; b < B; b += kSpThreads) p.n_tok[b] = s_n[b];
   if (cta == 0 && tid == 0) for (int i = 0; i < 12; ++i) p.prof[i] = prof[i];
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) { tcgen05_fence_after(); tmem_dealloc<64>(tmem_d); }
 }
 
 // workspace: hbuf | ppbuf | pad to 128 | barrier counters (kBarCounters lines) | prof (128 B) | best
@@ -674,7 +643,7 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   if (4 * p.units > 24 || p.rows_p > 8 || 32 * p.units > kSpThreads || 32 * p.rows_p > kSpThreads || a.gate_tab == nullptr) return cudaErrorInvalidValue;
   cudaError_t e = cudaMemsetAsync(workspace, 0, rnnt_spec_workspace_bytes(a.B, a.Hj, a.Hp, num_sms), stream);
   if (e != cudaSuccess) return e;
-  const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + kPassRows * 4 * 8 + static_cast<size_t>(a.B) * 8 * 4 +
+  const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + kPassRows * kSpWarps * 8 + static_cast<size_t>(a.B) * 8 * 4 +
                        (2 + 2 * kSpWarps) * 4 + 64;
   const size_t w_lp = (static_cast<size_t>(4 * p.units) * (a.Hp + 8) + static_cast<size_t>(p.rows_p) * (a.Hp + 8)) * 2;
   if (p.rows_j > 128) return cudaErrorInvalidValue;

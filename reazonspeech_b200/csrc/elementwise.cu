@@ -84,7 +84,7 @@ cudaError_t launch_layernorm(const float* x, const float* gamma, const float* be
   const int wpb = 8;
   int num_sms = 0, dev = 0;                                    // per call: engines on different devices share this code
   cudaGetDevice(&dev);
-  if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
+  if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
   const int need = (rows + wpb - 1) / wpb;
   const int cap = num_sms * 2;                                 // 2 resident CTAs per SM (16 warps x 2 rows in flight)
   auto* ob = static_cast<__nv_bfloat16*>(out_bf16);

@@ -1,6 +1,6 @@
 // C ABI of the engine (include/rs_engine.h): weight table lookup, workspace planning and the
 // launch sequence of the FastConformer-RNNT path.  Host-side orchestration only; every device
-// operation is one of the sm_100a kernels declared in kernels.h.
+// operation is one of the sm_90a kernels declared in kernels.h.
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>
 
@@ -63,7 +63,7 @@ inline int enc_capacity(int mel_frames) { return (conv_len(conv_len(conv_len(mel
 struct rs_engine {
   rs_model_config cfg;
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   std::map<std::string, Tensor> w;
   rs::LmTables fe{};          // tables of the fused log-mel kernel (logmel_tables.py)
   // ALSD beam search (decode_alsd.cu): fp32-accurate tripled weights (optional: present when the engine was created with them),
@@ -402,7 +402,7 @@ int do_encode(rs_engine* e, const Plan& p, const float* mel, const int32_t* mel_
     RS_TRY(gemm(e, xn, L.ff1_w1, L.ff1_b1, nullptr, hb, M, c.d_ff, d, RS_EPI_BIAS_SWISH_BF16, 1.f, s));
     RS_TRY(resid_gemm(hb, L.ff1_w2, L.ff1_b2, c.d_ff, 0.5f));
     RS_K(e, rs::launch_layernorm(x, L.ln_att_g, L.ln_att_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s), 1);
-    // the relative-position term (q + pos_bias_v) . p[c] is a UMMA inside the attention kernel (attention_tc.cu): no score tensor in HBM
+    // the relative-position term (q + pos_bias_v) . p[c] is a wgmma product inside the attention kernel (attention_tc.cu): no score tensor in HBM
     rs::AttnArgs aa{hb, L.att_pos, L.att_bdbias, p.n_rel_pad, L.att_u, ab, enc_len, B, p.T3, c.n_heads, d / c.n_heads, c.att_left, c.att_right, c.global_tokens};
     aa.vt = at<void>(e, p.vt); aa.ld_vt = p.ld_vt;
     {   // q | k row-major, V transposed (keys contiguous) for the attention's P.V product
@@ -444,7 +444,7 @@ int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_
   rs::DecodeArgs da{at<float>(e, p.encp), enc_len, e->dec.out_w, e->dec.out_b, e->dec.embed, e->dec.lstm_w, e->dec.lstm_b, e->dec.gate_tab,
                     e->dec.pred_w, e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden,
                     c.vocab_size, U_max, c.max_symbols};
-  // One decode kernel for every batch size (windowed, weights-stationary, joint on tcgen05: decode_spec.cu): an utterance's
+  // One decode kernel for every batch size (windowed, weights-stationary, joint on wgmma: decode_spec.cu): an utterance's
   // logits are accumulated in the same order whether it is decoded alone or inside a batch, so results do not depend on
   // batch composition.
   RS_K(e, rs::launch_rnnt_greedy_spec(da, at<void>(e, p.dec_ws), e->num_sms, s), 2);
@@ -477,7 +477,7 @@ int rs_engine_create(const rs_model_config* cfg, const rs_tensor* weights, int n
   if (ce != cudaSuccess) return fail(nullptr, RS_ERR_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(ce));
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
-  if (prop.major != 10) return fail(nullptr, RS_ERR_UNSUPPORTED, "device %d is sm_%d%d; kernels are built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9) return fail(nullptr, RS_ERR_UNSUPPORTED, "device %d is sm_%d%d; kernels are built for sm_90a only", device, prop.major, prop.minor);
   rs_engine* e = new rs_engine();
   e->cfg = *cfg; e->device = device; e->num_sms = prop.multiProcessorCount;
   for (int i = 0; i < n_weights; ++i) e->w[weights[i].name] = Tensor{weights[i].dev_ptr, weights[i].dtype, weights[i].numel};

@@ -1,4 +1,4 @@
-// Host-side launch interface of the sm_100a kernels (internal to librs_engine.so).
+// Host-side launch interface of the sm_90a kernels (internal to librs_engine.so).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -76,7 +76,7 @@ struct DecodeArgs {
   int32_t* tokens; int32_t* frames; int32_t* n_tok;
   int B, T_max, Hj, Hp, V, U_max, max_symbols;
 };
-// windowed (kFrames per iteration) persistent decode, joint on tcgen05 (decode_spec.cu); workspace from rnnt_spec_workspace_bytes()
+// windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace from rnnt_spec_workspace_bytes()
 size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp, int num_sms);
 size_t rnnt_spec_prof_offset(int B, int Hj, int Hp);        // where the kernel's 12 cycle counters sit inside that workspace
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream);

@@ -1,7 +1,7 @@
 // ConvSubsampling (dw_striding, x8) direct-convolution parts (N2).  NeMo reference module:
 // parts/submodules/subsampling.py ConvSubsampling (reached via model.transcribe,
 // pkg/nemo-asr/src/transcribe.py:48-53).  The 1x1 convs and the output Linear run on the
-// tcgen05 GEMM over channels-last activations; this file holds the HBM-bound 3x3 convs.
+// wgmma GEMM over channels-last activations; this file holds the HBM-bound 3x3 convs.
 //
 // Kernel A fuses the per-feature normalisation of the log-mel features (statistics from logmel.cu), conv.0
 // (1->C, 3x3, s2, p1) + ReLU + conv.2 (depthwise 3x3, s2, p1): the

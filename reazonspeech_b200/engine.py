@@ -1,8 +1,8 @@
 """ctypes binding of librs_engine.so (include/rs_engine.h) + weight packing.
 
 PyTorch is used for device memory, streams and the one-time weight repack only; every
-operation on the inference path is a hand-written sm_100a kernel behind the C ABI.  There
-is deliberately no CPU or eager-PyTorch fallback: if the library or a B200 is missing the
+operation on the inference path is a hand-written sm_90a kernel behind the C ABI.  There
+is deliberately no CPU or eager-PyTorch fallback: if the library or an H100 is missing the
 constructors raise.
 """
 from __future__ import annotations
@@ -249,12 +249,12 @@ class Engine:
         """``packed``: the result of ``pack_weights(state_dict, cfg)`` when several engines share one checkpoint (one replica
         per device): the repack is done once, every engine uploads its own copy."""
         if not torch.cuda.is_available():
-            raise RuntimeError("reazonspeech_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("reazonspeech_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = load_library()
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError(f"device {device!r}: the B200 engine has no CPU path")
+            raise RuntimeError(f"device {device!r}: the engine has no CPU path")
         self.dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self.device = torch.device("cuda", self.dev_index)
         if packed is None:
@@ -466,26 +466,14 @@ class Engine:
         self.lib.rs_debug_attention_cycles.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
         self._check(self.lib.rs_debug_attention_cycles(self.h, out), "rs_debug_attention_cycles")
         v = list(out)
-        names = ["start", "tma_issue", "qk_landed", "s_issued", "pv_wait", "pv_issued", "dealloc", "_",
-                 "sm_start", "sm_gscore_done", "sm_s_ready", "sm_pass1", "sm_pass2", "sm_o_wait", "sm_o_ready", "sm_end"]
-        return {n: int(x - v[0]) for n, x in zip(names, v) if n != "_"}
+        return {"start": 0, "end": int(v[6] - v[0])}          # entry and exit of thread 0 of CTA (1, 0, 0); zeros without -DRS_PROF
 
     def gemm_cycles(self):
-        """Timeline (SM clocks relative to kernel entry) of the last 2-CTA GEMM launch, for its first and its last cluster.
-        Only a library built with RS_BUILD_FLAGS=-DRS_PROF writes the stamps (scripts/diag_gemm_timeline.py); the shipped one
-        returns whatever the buffer held (zeros)."""
+        """SM clocks from entry to exit of CTA 0 of the last GEMM launch.  Only a library built with
+        RS_BUILD_FLAGS=-DRS_PROF writes the stamps; the shipped one returns whatever the buffer held (zeros)."""
         out = (C.c_int64 * 64)()
         self._check(self.lib.rs_debug_gemm_cycles(self.h, out), "rs_debug_gemm_cycles")
-        res = {}
-        for c, tag in enumerate(("first_cluster", "last_cluster")):
-            v = list(out)[32 * c: 32 * c + 32]
-            d = {"roles_start": v[0] - v[30], "end": v[31] - v[30]}
-            for i in range(3):
-                if v[3 + 4 * i] > v[30]:
-                    d[f"tile{i}"] = {"acc_free": v[1 + 4 * i] - v[30], "operands": v[2 + 4 * i] - v[30], "mma_issued": v[3 + 4 * i] - v[30],
-                                     "acc_full": v[4 + 4 * i] - v[30], "epilogue_done": v[16 + 2 * i] - v[30]}
-            res[tag] = d
-        return res
+        return {"end": int(out[31] - out[30])}
 
     def decode_cycles(self, B: int, L_max: int, U_max: int):
         out = (C.c_int64 * 12)()
@@ -496,7 +484,7 @@ class Engine:
         self._check(self.lib.rs_enable_gemm_timing(self.h, int(on)), "rs_enable_gemm_timing")
 
     def gemm_timing(self):
-        """(summed device ms, summed algorithmic FLOPs, launches) of the tcgen05 GEMM since enabled / last read."""
+        """(summed device ms, summed algorithmic FLOPs, launches) of the wgmma GEMM since enabled / last read."""
         ms, fl, n = C.c_double(), C.c_double(), C.c_int64()
         self._check(self.lib.rs_gemm_timing(self.h, C.byref(ms), C.byref(fl), C.byref(n)), "rs_gemm_timing")
         return ms.value, fl.value, n.value

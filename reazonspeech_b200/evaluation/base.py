@@ -182,7 +182,7 @@ def _predict_multi_gpu(evaluator: "BaseEvaluator", rows: List[dict], batch_size,
 
 
 class NemoB200Evaluator(BaseEvaluator):
-    """The reference's RSNemoEvaluator (examples/rs-nemo/eval.py:15-32) on the B200 engine, with the batch hook
+    """The reference's RSNemoEvaluator (examples/rs-nemo/eval.py:15-32) on the H100 engine, with the batch hook
     implemented.  Rows carry ``{"audio": {"path": ...}}`` (datasets' undecoded Audio feature, eval.py:29) or
     ``{"audio": {"array": ..., "sampling_rate": ...}}``.
 

@@ -1,5 +1,5 @@
 """``load_model`` / ``transcribe`` with the reference's signatures (pkg/nemo-asr/src/transcribe.py:9-60)
-on top of the B200 engine, plus the batched ``transcribe_batch`` the reference lacks
+on top of the H100 engine, plus the batched ``transcribe_batch`` the reference lacks
 (its evaluators leave ``_evaluate_batch`` unimplemented, pkg/evaluation/examples/rs-nemo/eval.py:31-32).
 
 The object returned by ``load_model`` is a duck-typed stand-in for NeMo's EncDecRNNTBPEModel at
@@ -251,7 +251,7 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     if device is None:
         device = "cuda"
     if str(device).startswith("cpu"):
-        raise RuntimeError("reazonspeech_b200: device='cpu' is not supported (hand-written sm_100a kernels only)")
+        raise RuntimeError("reazonspeech_b200: device='cpu' is not supported (hand-written sm_90a kernels only)")
     if synthetic is None:
         synthetic = os.environ.get(ENV_SYNTHETIC, "") not in ("", "0")
     path = checkpoint or (None if synthetic else _find_checkpoint())

@@ -162,7 +162,7 @@ def _structure_predictor(sd: StateDict, cfg: ModelConfig, suppress: float = 16.0
 
     The RECURRENT random term is kept small enough (row norm 0.1) for the state map to be a contraction.  With row norm 0.5
     (round 1) the predictor was weakly chaotic: the fp32 and fp64 evaluations of the SAME token sequence drifted apart
-    exponentially (1e-7 after one step, 2.5e-3 after 800, /tmp experiment recorded in profiles/r02_parity_noise.md), so on a
+    exponentially (1e-7 after one step, 2.5e-3 after 800), so on a
     clip that bursts to a thousand tokens not even the oracle agreed with itself across precisions, let alone with the
     engine.  A trained prediction network forgets its distant past; this one now does too."""
     hp, hj = cfg.pred_hidden, cfg.joint_hidden

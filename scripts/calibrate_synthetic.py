@@ -5,8 +5,8 @@ the time-varying part of enc_proj to about unit standard deviation, (3) the blan
 a greedy emission rate of about one token per three encoder frames.  A deterministic function of the
 seeded weights; it shapes the decode load of the benchmark only and is not part of the engine.
 
-    python scripts/calibrate_synthetic.py --config tiny     # on a B200, through the engine (a few short clips)
-    python scripts/calibrate_synthetic.py --config full     # on a B200, through the engine (the benchmark's clip set)
+    python scripts/calibrate_synthetic.py --config tiny     # on an H100, through the engine (a few short clips)
+    python scripts/calibrate_synthetic.py --config full     # on an H100, through the engine (the benchmark's clip set)
 
 Both go through the product path (the engine); the oracle is test infrastructure and is not used here.
 """

@@ -1,6 +1,6 @@
 """Where the one-process multi-GPU API (load_model(devices=[...]) + transcribe_batch) spends its wall time.
 
-    python scripts/diag_multi_gpu_api.py [n_devices]        # on a box with that many B200s
+    python scripts/diag_multi_gpu_api.py [n_devices]        # on a box with that many H100s
 
 Wraps the staging call, the engine call and decode_hypothesis with timers (per thread), runs the same clip list three times,
 prints one JSON line per run.

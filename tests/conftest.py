@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100")
     from oracle.cpu_threads import tune_threads
     tune_threads(16)
 

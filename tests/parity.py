@@ -7,7 +7,7 @@ put on the engine's path and the walk goes on to the last frame.
 
 What may differ.  The engine stores activations in bf16 at the points the oracle's ``emulate`` mode rounds at, but
 accumulates in another order, so its roundings fall differently: the two encoders differ by the same ~2.7e-3 relative L2
-per frame by which the oracle's OWN fp32 and bf16-emulated evaluations differ (measured, profiles/r02_parity_noise.md).
+per frame by which the oracle's OWN fp32 and bf16-emulated evaluations differ.
 With the synthetic (untrained) checkpoint that moves a logit gap by sigma ~ 1e-2 .. 3e-2, and untrained logits have many
 competitive classes, so ~2 % of the emissions flip -- in the oracle itself when its encoder is swapped between fp32 and
 bf16 emulation, and in the engine.  Two bars therefore:

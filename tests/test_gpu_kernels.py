@@ -1,4 +1,4 @@
-"""Kernel-level parity tests (run on a B200 through the C ABI).
+"""Kernel-level parity tests (run on an H100 through the C ABI).
 
 GEMM / LayerNorm are floating-point kernels, so their reference is a plain fp32 torch
 evaluation of the same op on the same bf16-rounded inputs; every model stage is compared with
@@ -174,7 +174,7 @@ def test_encoder_vs_oracle(tiny_engine, tiny_cfg, tiny_sd, n_layers):
 
 # ------------------------------------------------------------------------------------ decode
 def test_greedy_teacher_forced(tiny_engine, tiny_cfg, tiny_sd):
-    """The decode kernel alone (windowed, weights stationary, joint on tcgen05): fed the ORACLE's encoder output, tokens and
+    """The decode kernel alone (windowed, weights stationary, joint on wgmma): fed the ORACLE's encoder output, tokens and
     frames must be identical."""
     from oracle import nemo_restated as O
     eng = tiny_engine

@@ -1,4 +1,4 @@
-"""The sm_100a engine against the third-party Parakeet vectors (tests/golden/parakeet_cases.npz):
+"""The sm_90a engine against the third-party Parakeet vectors (tests/golden/parakeet_cases.npz):
 log-mel frontend and FastConformer encoder, through the C ABI, no oracle in between.
 
 Tolerances: normalised log-mel max-abs 2e-3 (fp32 FFT in a different order; log of near-silent bins);

@@ -77,7 +77,7 @@ def test_two_engines_on_one_device_and_second_device_are_independent(tiny_cfg, t
     assert n > 0 and int(n1[0]) == n and torch.equal(t0[0, :n].cpu(), t1[0, :n].cpu()) and torch.equal(f0[0, :n].cpu(), f1[0, :n].cpu())
 
 
-@pytest.mark.skipif(torch.cuda.is_available() and torch.cuda.device_count() < 2, reason="needs two GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.is_available() and torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_one_process_multi_gpu_equals_single_gpu(model, tiny_cfg):
     """load_model(devices=[0, 1]): one replica, worker thread and staging pair per device in ONE process; the merged result
     equals the one-GPU result token for token and arrives in input order (SURVEY.md section 8e; the reference's
