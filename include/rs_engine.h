@@ -69,9 +69,8 @@ typedef enum rs_epilogue {
   RS_EPI_BIAS_RELU_BF16 = 1,  /* out_bf16[M,N]   = relu(acc + bias)                            */
   RS_EPI_BIAS_SWISH_BF16 = 2, /* out_bf16[M,N]   = swish(acc + bias)                           */
   RS_EPI_BIAS_GLU_BF16 = 3,   /* out_bf16[M,N/2] = a * sigmoid(g); W rows interleaved 16/16    */
-  RS_EPI_RESID_F32 = 4,       /* out_f32[M,N]    = resid + alpha * (acc + bias)  (may alias: with out == resid and
-                                 N % 256 == 0 the add is a TMA reduce-add performed by the memory system -- the residual is never
-                                 read into the SM; same fp32 sum, bit-identical to the two-buffer form)   */
+  RS_EPI_RESID_F32 = 4,       /* out_f32[M,N]    = resid + alpha * (acc + bias)  (out may alias resid: each element is
+                                 read and written by one lane)                                                        */
   RS_EPI_BIAS_F32 = 5,        /* out_f32[M,N]    = alpha * (acc + bias)                        */
   RS_EPI_BIAS_F16 = 6,        /* out_f16[M,N]    = acc + bias  (IEEE half)                          */
   RS_EPI_QKV_VT = 7           /* fused QKV projection: columns [0, split) -> out_bf16[M, ldo] as RS_EPI_BIAS_BF16,
@@ -178,13 +177,11 @@ int64_t rs_launch_count(const rs_engine* e);
 /* Per-stage device time of the last rs_transcribe_* call when timing was enabled. */
 int rs_enable_stage_timing(rs_engine* e, int on);
 int rs_stage_times_ms(const rs_engine* e, float* ms /*[8]*/);
+int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* out8);   /* profiling aid, see engine.cu */
 /* Per-launch CUDA-event timing of the wgmma GEMM (the dominant kernel): while enabled every GEMM
  * launch is bracketed by two events on its stream.  rs_gemm_timing() synchronises, returns the summed
  * device time, the summed algorithmic FLOPs (2*M*N*K) and the launch count since it was enabled or
- * last read, and resets the accumulators. */
-int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* out8);   /* profiling aid, see engine.cu */
-int rs_debug_attention_cycles(rs_engine* e, int64_t* out16);   /* clock64 stamps of one CTA of the last attention launch */
-int rs_debug_gemm_cycles(rs_engine* e, int64_t* out64);        /* clock64 stamps of CTA 0 of the last GEMM launch: [30] entry, [31] exit, only with -DRS_PROF (gemm_wgmma.cu) */
+ * last read, and resets the log. */
 int rs_enable_gemm_timing(rs_engine* e, int on);
 int rs_gemm_timing(rs_engine* e, double* ms, double* flops, int64_t* launches);
 /* Per-kernel CUDA-event timing of EVERY launch inside the real pipeline (warm caches, back-to-back launches, unlike

@@ -61,9 +61,6 @@ struct AtcDev {
   int T_max, H, w_left, w_right, n_global, n_rel_pad, ld_qk, ld_vt;
 };
 
-// cycle stamps of thread 0 of CTA (1, 0, 0): [0] kernel entry, [6] exit (profiling aid, rs_debug_attention_cycles; only with -DRS_PROF)
-__device__ long long g_atc_prof[16];
-
 __device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 // byte offset of the 16-byte chunk `chunk` (0..7) of row `row` inside a [rows x 64 bf16] 128B-swizzled slab
@@ -92,10 +89,6 @@ local_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid
   const size_t row0 = static_cast<size_t>(b) * p.T_max;
   __nv_bfloat16* obase = p.out + row0 * d + h * TDK;
 
-#ifdef RS_PROF
-  const bool prof_cta = blockIdx.x == 1 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0;
-  if (prof_cta) g_atc_prof[0] = clock64();
-#endif
   if (q0 >= len) {                                   // fully padded tile: defined zeros
     for (int id = threadIdx.x; id < TQ * 16; id += blockDim.x) {
       const int r = id >> 4, c = (id & 15) * 8;
@@ -329,9 +322,6 @@ local_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid
     const uint4 a = *reinterpret_cast<const uint4*>(stage + rr * kOutPitch + cc);
     if (row < p.T_max) *reinterpret_cast<uint4*>(obase + static_cast<size_t>(row) * d + cc) = a;
   }
-#ifdef RS_PROF
-  if (prof_cta) g_atc_prof[6] = clock64();
-#endif
 }
 
 // Row(s) of the global token(s): full attention softmax_j((q_g / sqrt(dk)) . k_j) v_j, no positional terms.
@@ -418,38 +408,7 @@ global_row_attention_tc_kernel(const AtcDev p) {
   if (seg == 0) p.out[row0 * d + h * TDK + dim] = __float2bfloat16_rn((part + gs[dim]) * inv);
 }
 
-typedef CUresult (*EncodeTiledFnA)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFnA encode_fn() {
-  static EncodeTiledFnA fn = nullptr;
-  if (fn == nullptr) {
-    void* sym = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFnA>(sym);
-  }
-  return fn;
-}
-
-// bf16 row-major [rows, cols] (row pitch ld elements) -> 2-D map, box 64 columns x box_rows rows, 128B swizzle, zero fill
-bool make_map(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows = 128) {
-  EncodeTiledFnA fn = encode_fn();
-  if (fn == nullptr) return false;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {64, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 }  // namespace
-
-cudaError_t attention_tc_debug_cycles(long long* out16) {
-  return cudaMemcpyFromSymbol(out16, g_atc_prof, sizeof(long long) * 16);
-}
 
 bool attention_tc_supported(const AttnArgs& a) {
   return a.dk == TDK && a.w_left >= 0 && a.w_right >= 0 && a.w_left <= 128 && a.w_right <= 128 && (a.w_left & 7) == 0 && a.n_global >= 0 &&
@@ -467,11 +426,12 @@ cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t stream) {
   p.enc_len = a.enc_len; p.T_max = a.T_max; p.H = a.H; p.w_left = a.w_left; p.w_right = a.w_right;
   p.n_global = a.n_global; p.n_rel_pad = a.n_rel_pad; p.ld_qk = 3 * d; p.ld_vt = a.ld_vt;
   CUtensorMap tm_q, tm_k, tm_vt, tm_pos;
+  char err[256];
   // positional table [H * n_rel_pad, 128] bf16, fetched in boxes of n_rel_pad / 2 rows (<= 144; a TMA box holds at most 256)
-  if (!make_map(&tm_pos, a.pos, static_cast<uint64_t>(a.H) * a.n_rel_pad, TDK, TDK, static_cast<uint32_t>(a.n_rel_pad / 2))) return cudaErrorInvalidValue;
-  if (!make_map(&tm_q, p.qk, static_cast<uint64_t>(M), static_cast<uint64_t>(2 * d), static_cast<uint64_t>(p.ld_qk))) return cudaErrorInvalidValue;
-  if (!make_map(&tm_k, p.qk, static_cast<uint64_t>(M), static_cast<uint64_t>(2 * d), static_cast<uint64_t>(p.ld_qk), KB)) return cudaErrorInvalidValue;
-  if (!make_map(&tm_vt, p.vt, static_cast<uint64_t>(d), static_cast<uint64_t>(M), static_cast<uint64_t>(p.ld_vt))) return cudaErrorInvalidValue;
+  if (!make_tmap_bf16(&tm_pos, a.pos, static_cast<uint64_t>(a.H) * a.n_rel_pad, TDK, TDK, static_cast<uint32_t>(a.n_rel_pad / 2), err)) return cudaErrorInvalidValue;
+  if (!make_tmap_bf16(&tm_q, p.qk, static_cast<uint64_t>(M), static_cast<uint64_t>(2 * d), static_cast<uint64_t>(p.ld_qk), 128, err)) return cudaErrorInvalidValue;
+  if (!make_tmap_bf16(&tm_k, p.qk, static_cast<uint64_t>(M), static_cast<uint64_t>(2 * d), static_cast<uint64_t>(p.ld_qk), KB, err)) return cudaErrorInvalidValue;
+  if (!make_tmap_bf16(&tm_vt, p.vt, static_cast<uint64_t>(d), static_cast<uint64_t>(M), static_cast<uint64_t>(p.ld_vt), 128, err)) return cudaErrorInvalidValue;
   static DeviceOnce attr_once;
   if (attr_once.pending()) {
     cudaError_t e = cudaFuncSetAttribute(local_attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kAtcSmem));

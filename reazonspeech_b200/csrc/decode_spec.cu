@@ -41,7 +41,7 @@ constexpr int kPassUtts = kPassRows / kFrames;
 
 struct SpecDev {
   const float* enc_proj; const int32_t* enc_len;
-  const __nv_bfloat16* w_out; const float* b_out; const float* embed;
+  const __nv_bfloat16* w_out; const float* b_out;
   const __nv_bfloat16* w_lstm; const float* gate_tab; const __nv_bfloat16* w_pred; const float* b_pred;
   int32_t* tokens; int32_t* frames; int32_t* n_tok;
   unsigned long long* best;   // [3][B][kFrames] packed (ordered logit bits << 32 | ~row), 3-deep ring
@@ -216,14 +216,9 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   unsigned int target = 0;
   int iter = 0;
   long long prof[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  // per-phase cycle counters of CTA 0 (rs_debug_decode_cycles); -DRS_NO_DECODE_COUNTERS drops them.
-#ifndef RS_NO_DECODE_COUNTERS
+  // per-phase cycle counters of CTA 0 (rs_debug_decode_cycles)
   auto tick = [&](int slot, long long& t0) { if (cta == 0 && tid == 0) { const long long t1 = clock64(); prof[slot] += t1 - t0; t0 = t1; } };
   long long tk = clock64();
-#else
-  auto tick = [&](int, long long&) {};
-  long long tk = 0;
-#endif
 
   // ------------------------------------------------------------------------------------------------
   // LSTM step + joint.pred for the utterances listed in s_emit[0..n_emit): token s_tok[b], state parity s_par[b]
@@ -455,13 +450,9 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
             }
           }
         };
-#ifndef RS_NO_DECODE_COUNTERS
         long long tj = 0;
         if (cta == 0 && tid == 0) tj = clock64();
         auto jtick = [&](int slot) { if (cta == 0 && tid == 0) { const long long t1 = clock64(); prof[slot] += t1 - tj; tj = t1; } };
-#else
-        auto jtick = [&](int) {};
-#endif
         {
           // ---- wgmma joint: D[vocabulary row, (utterance, frame) row]; warpgroup wgi holds vocabulary rows [64 wgi, +64)
           auto write_planes = [&]() {                         // gv -> two IEEE-half planes, 128B-swizzled K-major, 32 rows per slab
@@ -603,7 +594,7 @@ static size_t spec_counter_offset(int B, int Hj, int Hp) {
   return (static_cast<size_t>(2) * B * Hp * 4 + static_cast<size_t>(B) * Hj * 4 + 127) & ~static_cast<size_t>(127);
 }
 size_t rnnt_spec_prof_offset(int B, int Hj, int Hp) { return spec_counter_offset(B, Hj, Hp) + static_cast<size_t>(kBarCounters) * kBarStride * 4; }
-size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp, int /*num_sms*/) {
+size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp) {
   return rnnt_spec_prof_offset(B, Hj, Hp) + 128 + static_cast<size_t>(3) * B * kFrames * 8 + 128 /*base alignment slack*/;
 }
 
@@ -624,7 +615,7 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   const int G = num_sms;
   SpecDev p;
   p.enc_proj = a.enc_proj; p.enc_len = a.enc_len;
-  p.w_out = static_cast<const __nv_bfloat16*>(a.w_out); p.b_out = a.b_out; p.embed = a.embed;
+  p.w_out = static_cast<const __nv_bfloat16*>(a.w_out); p.b_out = a.b_out;
   p.w_lstm = static_cast<const __nv_bfloat16*>(a.w_lstm); p.gate_tab = a.gate_tab;
   p.w_pred = static_cast<const __nv_bfloat16*>(a.w_pred); p.b_pred = a.b_pred;
   p.tokens = a.tokens; p.frames = a.frames; p.n_tok = a.n_tok;
@@ -641,7 +632,7 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   p.units = (a.Hp + G - 1) / G;
   p.rows_p = (a.Hj + G - 1) / G;
   if (4 * p.units > 24 || p.rows_p > 8 || 32 * p.units > kSpThreads || 32 * p.rows_p > kSpThreads || a.gate_tab == nullptr) return cudaErrorInvalidValue;
-  cudaError_t e = cudaMemsetAsync(workspace, 0, rnnt_spec_workspace_bytes(a.B, a.Hj, a.Hp, num_sms), stream);
+  cudaError_t e = cudaMemsetAsync(workspace, 0, rnnt_spec_workspace_bytes(a.B, a.Hj, a.Hp), stream);
   if (e != cudaSuccess) return e;
   const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + kPassRows * kSpWarps * 8 + static_cast<size_t>(a.B) * 8 * 4 +
                        (2 + 2 * kSpWarps) * 4 + 64;

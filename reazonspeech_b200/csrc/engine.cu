@@ -79,28 +79,20 @@ struct rs_engine {
   struct { const void *enc_w, *out_w, *lstm_w, *pred_w; const float *enc_b, *out_b, *embed, *lstm_b, *pred_b, *gate_tab; } dec;
   void* ws = nullptr;
   size_t ws_bytes = 0;
-  int U_cap = 0;
   mutable char err[512] = "";
   int64_t launches = 0;
-  bool timing = false;
-  cudaEvent_t ev[9] = {};
-  bool ev_ok = false;
-  float stage_ms[8] = {};
-  bool gemm_timing = false;
-  std::vector<cudaEvent_t> gemm_ev;     // pairs
-  size_t gemm_ev_used = 0;
-  double gemm_flops = 0.0;
-  // per-kernel timing inside the real pipeline (warm caches, back-to-back launches): event pair around every launch
-  bool ktiming = false;
-  cudaStream_t cur_stream = nullptr;
-  std::vector<cudaEvent_t> k_ev;
-  std::vector<std::string> k_tag;       // one per event pair
+  bool timing = false;                  // stage marks (mark)
+  cudaEvent_t ev[6] = {};
+  // launch log (launch): one {tag, flops} entry per timed launch, timed by the event pair log_ev[2i], log_ev[2i + 1]
+  struct Timed { std::string tag; double flops; };
+  bool ktiming = false, gemm_timing = false;
+  std::vector<Timed> log;
+  std::vector<cudaEvent_t> log_ev;
   // rs_transcribe_batch: host->device copies run on their own stream in utterance chunks so the frontend of
   // chunk i overlaps the copy of chunk i+1
   static constexpr int kCopyChunks = 8;
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t copy_ev[kCopyChunks + 1] = {};
-  bool copy_ok = false;
 };
 
 namespace {
@@ -119,10 +111,70 @@ int fail(const rs_engine* e, int code, const char* fmt, ...) {
     if (_c != cudaSuccess) return fail((e), RS_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_c)); \
   } while (0)
 
+#define RS_TRY(x) do { int _r = (x); if (_r != RS_OK) return _r; } while (0)
+
+// Every device enqueue of the engine goes through launch(): `enqueue()` issues `n` launches (a memset counts as one) on
+// stream `s` and returns the first error.  The launches are counted (rs_launch_count).  While kernel timing is on, or GEMM
+// timing is on and the call is a GEMM (flops = 2*M*N*K > 0), the call is bracketed by an event pair on `s` and logged as
+// {tag, flops}.  `what` is the call's source text, quoted by the error message; the tag is its name without the rs::
+// namespace and the arguments.
+template <typename F>
+int launch(rs_engine* e, cudaStream_t s, const char* what, int n, double flops, F&& enqueue) {
+  const bool timed = e->ktiming || (e->gemm_timing && flops > 0.0);
+  const size_t i = 2 * e->log.size();
+  if (timed) {
+    while (e->log_ev.size() < i + 2) {
+      cudaEvent_t ev;
+      RS_CUDA(e, cudaEventCreate(&ev));
+      e->log_ev.push_back(ev);
+    }
+    RS_CUDA(e, cudaEventRecord(e->log_ev[i], s));
+  }
+  const cudaError_t c = enqueue();
+  if (c != cudaSuccess) return fail(e, RS_ERR_CUDA, "%s: %s", what, cudaGetErrorString(c));
+  if (timed) {
+    RS_CUDA(e, cudaEventRecord(e->log_ev[i + 1], s));
+    std::string tag(what);
+    if (tag.rfind("rs::", 0) == 0) tag = tag.substr(4);
+    e->log.push_back({tag.substr(0, tag.find('(')), flops});
+  }
+  e->launches += n;
+  return RS_OK;
+}
+#define RS_LAUNCH(e, s, n, call) RS_TRY(launch((e), (s), #call, (n), 0.0, [&] { return (call); }))
+
+int gemm(rs_engine* e, const rs::GemmArgs& g, cudaStream_t s) {
+  char what[64], msg[256] = "";
+  snprintf(what, sizeof what, "gemm N=%d K=%d epi=%d", g.N, g.K, g.epilogue);
+  const int r = launch(e, s, what, 1, 2.0 * g.M * static_cast<double>(g.N) * g.K, [&] { return rs::launch_gemm(g, e->num_sms, s, msg); });
+  if (r != RS_OK && msg[0] != '\0') return fail(e, r, "gemm: %s", msg);
+  return r;
+}
+
+// Synchronises the engine's device, passes every logged launch with its device time to visit(entry, ms), clears the log.
+template <typename F>
+int drain_log(rs_engine* e, F&& visit) {
+  RS_CUDA(e, cudaSetDevice(e->device));
+  RS_CUDA(e, cudaDeviceSynchronize());
+  for (size_t i = 0; i < e->log.size(); ++i) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e->log_ev[2 * i], e->log_ev[2 * i + 1]);
+    visit(e->log[i], ms);
+  }
+  e->log.clear();
+  return RS_OK;
+}
+
 size_t align_up(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 
+// Workspace layout: regions taken one after another, each starting 256-byte aligned.
+struct Arena {
+  size_t off = 0;
+  size_t take(size_t bytes) { const size_t o = off; off = align_up(off + bytes); return o; }
+};
+
 inline size_t dec_ws_bytes(const rs_engine* e, int B) {
-  return rs::rnnt_spec_workspace_bytes(B, e->cfg.joint_hidden, e->cfg.pred_hidden, e->num_sms);
+  return rs::rnnt_spec_workspace_bytes(B, e->cfg.joint_hidden, e->cfg.pred_hidden);
 }
 
 Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
@@ -136,34 +188,33 @@ Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
   p.M = B * p.T3;
   const size_t C = c.sub_channels, d = c.d_model;
   const size_t wide = static_cast<size_t>(c.d_ff) > 3 * d ? c.d_ff : 3 * d;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes); return o; };
-  p.wav = take(static_cast<size_t>(B) * L_max * 4);
-  p.len = take(static_cast<size_t>(B) * 4);
-  p.mel = take(static_cast<size_t>(B) * p.F_max * c.n_mels * 4);
-  p.mel_len = take(static_cast<size_t>(B) * 4);
-  p.mel_part = take(static_cast<size_t>(B) * rs::logmel_tiles(L_max, c.n_window_stride) * c.n_mels * 2 * 4);   // per-CTA (sum, sum of squares)
-  p.mel_stats = take(static_cast<size_t>(B) * c.n_mels * 2 * 4);                                               // (mean, 1 / (std + eps))
-  p.enc_len = take(static_cast<size_t>(B) * 4);
-  p.sub1 = take(static_cast<size_t>(B) * p.T2 * p.F2 * C * 2);
-  p.sub2 = take(static_cast<size_t>(B) * p.T2 * p.F2 * C * 2);
-  p.sub3 = take(static_cast<size_t>(B) * p.T3 * p.F3 * C * 2);
-  p.sub4 = take(static_cast<size_t>(B) * p.T3 * p.F3 * C * 2);
-  p.x = take(static_cast<size_t>(p.M) * d * 4);
-  p.xn = take(static_cast<size_t>(p.M) * d * 2);
-  p.hbuf = take(static_cast<size_t>(p.M) * wide * 2);
-  p.abuf = take(static_cast<size_t>(p.M) * d * 2);
-  p.cbuf = take(static_cast<size_t>(p.M) * d * 2);
+  Arena a;
+  p.wav = a.take(static_cast<size_t>(B) * L_max * 4);
+  p.len = a.take(static_cast<size_t>(B) * 4);
+  p.mel = a.take(static_cast<size_t>(B) * p.F_max * c.n_mels * 4);
+  p.mel_len = a.take(static_cast<size_t>(B) * 4);
+  p.mel_part = a.take(static_cast<size_t>(B) * rs::logmel_tiles(L_max, c.n_window_stride) * c.n_mels * 2 * 4);   // per-CTA (sum, sum of squares)
+  p.mel_stats = a.take(static_cast<size_t>(B) * c.n_mels * 2 * 4);                                               // (mean, 1 / (std + eps))
+  p.enc_len = a.take(static_cast<size_t>(B) * 4);
+  p.sub1 = a.take(static_cast<size_t>(B) * p.T2 * p.F2 * C * 2);
+  p.sub2 = a.take(static_cast<size_t>(B) * p.T2 * p.F2 * C * 2);
+  p.sub3 = a.take(static_cast<size_t>(B) * p.T3 * p.F3 * C * 2);
+  p.sub4 = a.take(static_cast<size_t>(B) * p.T3 * p.F3 * C * 2);
+  p.x = a.take(static_cast<size_t>(p.M) * d * 4);
+  p.xn = a.take(static_cast<size_t>(p.M) * d * 2);
+  p.hbuf = a.take(static_cast<size_t>(p.M) * wide * 2);
+  p.abuf = a.take(static_cast<size_t>(p.M) * d * 2);
+  p.cbuf = a.take(static_cast<size_t>(p.M) * d * 2);
   p.n_rel_pad = ((c.att_left + c.att_right + 1 + 31) / 32) * 32;
   p.ld_vt = ((p.M + 255) / 256) * 256 + 64;                               // V^T row pitch: covers the GEMM's 256-row tile overhang
-  p.vt = take(static_cast<size_t>(d) * p.ld_vt * 2);
-  p.enc = take(static_cast<size_t>(p.M) * d * 4);
-  p.encp = take(static_cast<size_t>(p.M) * c.joint_hidden * 4);
-  p.tokens = take(static_cast<size_t>(B) * U_max * 4);
-  p.frames = take(static_cast<size_t>(B) * U_max * 4);
-  p.ntok = take(static_cast<size_t>(B) * 4);
-  p.dec_ws = take(dec_ws_bytes(e, B));
-  p.total = off;
+  p.vt = a.take(static_cast<size_t>(d) * p.ld_vt * 2);
+  p.enc = a.take(static_cast<size_t>(p.M) * d * 4);
+  p.encp = a.take(static_cast<size_t>(p.M) * c.joint_hidden * 4);
+  p.tokens = a.take(static_cast<size_t>(B) * U_max * 4);
+  p.frames = a.take(static_cast<size_t>(B) * U_max * 4);
+  p.ntok = a.take(static_cast<size_t>(B) * 4);
+  p.dec_ws = a.take(dec_ws_bytes(e, B));
+  p.total = a.off;
   return p;
 }
 
@@ -256,71 +307,6 @@ __global__ void enc_len_kernel(const int32_t* __restrict__ mel_len, int32_t* __r
   enc_len[b] = n;
 }
 
-int gemm_args(rs_engine* e, const rs::GemmArgs& g, cudaStream_t s);
-
-int gemm(rs_engine* e, const void* a, const void* w, const float* bias, const float* resid, void* out, int M, int N,
-         int K, int epi, float alpha, cudaStream_t s) {
-  rs::GemmArgs g{a, w, bias, resid, out, M, N, K, epi, alpha};
-  return gemm_args(e, g, s);
-}
-
-void ktime_begin(rs_engine* e, const char* tag) {
-  if (!e->ktiming) return;
-  const size_t i = 2 * e->k_tag.size();
-  while (e->k_ev.size() < i + 2) { cudaEvent_t ev; cudaEventCreate(&ev); e->k_ev.push_back(ev); }
-  std::string t(tag);
-  if (t.rfind("rs::", 0) == 0) t = t.substr(4);
-  const size_t par = t.find('(');
-  e->k_tag.push_back(par == std::string::npos ? t : t.substr(0, par));
-  cudaEventRecord(e->k_ev[i], e->cur_stream);
-}
-void ktime_end(rs_engine* e) {
-  if (!e->ktiming) return;
-  cudaEventRecord(e->k_ev[2 * e->k_tag.size() - 1], e->cur_stream);
-}
-
-int gemm_args(rs_engine* e, const rs::GemmArgs& g_in, cudaStream_t s) {
-  const rs::GemmArgs& g = g_in;
-  const int M = g.M, N = g.N, K = g.K;
-  char msg[256] = "";
-  bool timed = false;
-  if (e->gemm_timing) {
-    if (e->gemm_ev_used + 2 > e->gemm_ev.size()) {
-      const size_t old = e->gemm_ev.size();
-      e->gemm_ev.resize(old + 512);
-      for (size_t i = old; i < e->gemm_ev.size(); ++i) cudaEventCreate(&e->gemm_ev[i]);
-    }
-    cudaEventRecord(e->gemm_ev[e->gemm_ev_used], s);
-    timed = true;
-  }
-  if (e->ktiming) {
-    char tag[64];
-    snprintf(tag, sizeof tag, "gemm N=%d K=%d epi=%d%s", N, K, g.epilogue, g.n_batch > 1 ? " batched" : "");
-    e->cur_stream = s;
-    ktime_begin(e, tag);
-  }
-  cudaError_t c = rs::launch_gemm(g, e->num_sms, s, msg);
-  ktime_end(e);
-  if (c != cudaSuccess) return fail(e, RS_ERR_CUDA, "gemm: %s", msg);
-  if (timed) {
-    cudaEventRecord(e->gemm_ev[e->gemm_ev_used + 1], s);
-    e->gemm_ev_used += 2;
-    e->gemm_flops += 2.0 * M * static_cast<double>(N) * K * (g.n_batch > 0 ? g.n_batch : 1);
-  }
-  e->launches++;
-  return RS_OK;
-}
-
-#define RS_TRY(x) do { int _r = (x); if (_r != RS_OK) return _r; } while (0)
-#define RS_K(e, call, n)                                                                       \
-  do {                                                                                         \
-    ktime_begin((e), #call);                                                                   \
-    cudaError_t _c = (call);                                                                   \
-    ktime_end((e));                                                                            \
-    if (_c != cudaSuccess) return fail((e), RS_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(_c)); \
-    (e)->launches += (n);                                                                      \
-  } while (0)
-
 int check_ws(rs_engine* e, const Plan& p) {
   if (e->ws == nullptr) return fail(e, RS_ERR_WORKSPACE, "no workspace set (rs_set_workspace)");
   if (p.total > e->ws_bytes)
@@ -329,7 +315,7 @@ int check_ws(rs_engine* e, const Plan& p) {
 }
 
 void mark(rs_engine* e, int i, cudaStream_t s) {
-  if (e->timing && e->ev_ok) cudaEventRecord(e->ev[i], s);
+  if (e->timing) cudaEventRecord(e->ev[i], s);
 }
 
 // Log-mel of utterances [b0, b0 + nb) of a batch whose statistics live at plan offsets (absolute utterance index).
@@ -337,7 +323,6 @@ void mark(rs_engine* e, int i, cudaStream_t s) {
 int do_logmel(rs_engine* e, const void* wav, bool i16, const int32_t* len, int nb, int L_max, float* mel, int32_t* mel_len,
               float* partials, float* stats, int b0, bool normalise, cudaStream_t s) {
   Nvtx range("rs::logmel");
-  e->cur_stream = s;
   const rs_model_config& c = e->cfg;
   if (b0 + nb > rs_engine::kMaxBatch) return fail(e, RS_ERR_INVALID_ARG, "batch of %d utterances exceeds the engine limit of %d", b0 + nb, rs_engine::kMaxBatch);
   rs::LogmelArgs a{};
@@ -347,107 +332,98 @@ int do_logmel(rs_engine* e, const void* wav, bool i16, const int32_t* len, int n
   a.tickets = e->lm_tickets + b0;
   a.tb = e->fe; a.n_mels = c.n_mels; a.hop = c.n_window_stride; a.n_fft = c.n_fft; a.win = c.n_window_size;
   a.preemph = c.preemph; a.guard = c.log_zero_guard; a.eps = c.norm_eps; a.normalise_in_place = normalise;
-  RS_K(e, rs::launch_logmel_fused(a, s), normalise ? 2 : 1);
+  RS_LAUNCH(e, s, normalise ? 2 : 1, rs::launch_logmel_fused(a, s));
   return RS_OK;
 }
 
 // mel_stats == nullptr: `mel` is already normalised (rs_encode takes rs_logmel's output)
 int do_sub_conv0(rs_engine* e, const Plan& p, const float* mel, const int32_t* mel_len, const float* mel_stats, int b0, int nb, cudaStream_t s) {
   Nvtx range("rs::subsampling.conv0_dw1");
-  e->cur_stream = s;
   const rs_model_config& c = e->cfg;
   const int C = c.sub_channels;
   rs::SubsampleArgs sa{mel + static_cast<size_t>(b0) * p.F_max * c.n_mels, mel_len + b0,
                        mel_stats ? mel_stats + static_cast<size_t>(b0) * c.n_mels * 2 : nullptr, nb, p.F_max, c.n_mels, C,
                        e->sub.c0w, e->sub.c0b, e->sub.d1w, e->sub.d1b,
                        at<uint16_t>(e, p.sub1) + static_cast<size_t>(b0) * p.T2 * p.F2 * C, p.T1, p.F1, p.T2, p.F2};
-  RS_K(e, rs::launch_sub_conv0_dw1(sa, s), 1);
+  RS_LAUNCH(e, s, 1, rs::launch_sub_conv0_dw1(sa, s));
   return RS_OK;
 }
 
-int do_encode(rs_engine* e, const Plan& p, const float* mel, const int32_t* mel_len, const float* mel_stats, float* enc, int32_t* enc_len,
-              int n_layers, cudaStream_t s, bool conv0_done = false) {
-  e->cur_stream = s;
+// The encoder after the first (fused) subsampling conv, which do_sub_conv0 has enqueued on `s`.
+int do_encode(rs_engine* e, const Plan& p, const int32_t* mel_len, float* enc, int32_t* enc_len, int n_layers, cudaStream_t s) {
   const rs_model_config& c = e->cfg;
   const int d = c.d_model, C = c.sub_channels, M = p.M, B = p.B;
   if (n_layers < 0 || n_layers > c.n_layers) n_layers = c.n_layers;
-  enc_len_kernel<<<(B + 127) / 128, 128, 0, s>>>(mel_len, enc_len, B);
-  RS_K(e, cudaGetLastError(), 1);
+  RS_TRY(launch(e, s, "enc_len_kernel", 1, 0.0, [&] {
+    enc_len_kernel<<<(B + 127) / 128, 128, 0, s>>>(mel_len, enc_len, B);
+    return cudaGetLastError();
+  }));
   // ---- ConvSubsampling
-  if (!conv0_done) RS_TRY(do_sub_conv0(e, p, mel, mel_len, mel_stats, 0, B, s));
-  RS_TRY(gemm(e, at<void>(e, p.sub1), e->sub.p1w, e->sub.p1b, nullptr, at<void>(e, p.sub2), B * p.T2 * p.F2, C, C,
-              RS_EPI_BIAS_RELU_BF16, 1.f, s));
-  RS_K(e, rs::launch_sub_dw(at<void>(e, p.sub2), at<void>(e, p.sub3), e->sub.d2w, e->sub.d2b, mel_len, 2, B, p.T2, p.F2,
-                            p.T3, p.F3, C, s), 1);
-  RS_TRY(gemm(e, at<void>(e, p.sub3), e->sub.p2w, e->sub.p2b, nullptr, at<void>(e, p.sub4), B * p.T3 * p.F3, C, C,
-              RS_EPI_BIAS_RELU_BF16, 1.f, s));
+  RS_TRY(gemm(e, {at<void>(e, p.sub1), e->sub.p1w, e->sub.p1b, nullptr, at<void>(e, p.sub2), B * p.T2 * p.F2, C, C, RS_EPI_BIAS_RELU_BF16, 1.f}, s));
+  RS_LAUNCH(e, s, 1, rs::launch_sub_dw(at<void>(e, p.sub2), at<void>(e, p.sub3), e->sub.d2w, e->sub.d2b, mel_len, 2, B, p.T2, p.F2,
+                                       p.T3, p.F3, C, s));
+  RS_TRY(gemm(e, {at<void>(e, p.sub3), e->sub.p2w, e->sub.p2b, nullptr, at<void>(e, p.sub4), B * p.T3 * p.F3, C, C, RS_EPI_BIAS_RELU_BF16, 1.f}, s));
   float* x = at<float>(e, p.x);
   Nvtx layers_range("rs::conformer_layers");
-  RS_TRY(gemm(e, at<void>(e, p.sub4), e->sub.ow, e->sub.ob, nullptr, x, M, d, p.F3 * C, RS_EPI_BIAS_F32, c.xscale, s));
+  RS_TRY(gemm(e, {at<void>(e, p.sub4), e->sub.ow, e->sub.ob, nullptr, x, M, d, p.F3 * C, RS_EPI_BIAS_F32, c.xscale}, s));
   mark(e, 2, s);
   // ---- Conformer layers
   void* xn = at<void>(e, p.xn); void* hb = at<void>(e, p.hbuf); void* ab = at<void>(e, p.abuf); void* cb = at<void>(e, p.cbuf);
   if (n_layers > 0) {
     const LayerW& L0 = e->layers[0];
-    RS_K(e, rs::launch_layernorm(x, L0.ln_ff1_g, L0.ln_ff1_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s), 1);
+    RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, L0.ln_ff1_g, L0.ln_ff1_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s));
   }
   auto resid_gemm = [&](const void* a, const void* w, const float* bias, int K, float alpha) -> int {
-    return gemm(e, a, w, bias, x, x, M, d, K, RS_EPI_RESID_F32, alpha, s);
+    return gemm(e, {a, w, bias, x, x, M, d, K, RS_EPI_RESID_F32, alpha}, s);
   };
   for (int i = 0; i < n_layers; ++i) {
     const LayerW& L = e->layers[i];
     char layer_name[32];
     snprintf(layer_name, sizeof layer_name, "rs::conformer_layer[%d]", i);
     Nvtx layer_range(layer_name);
-    RS_TRY(gemm(e, xn, L.ff1_w1, L.ff1_b1, nullptr, hb, M, c.d_ff, d, RS_EPI_BIAS_SWISH_BF16, 1.f, s));
+    RS_TRY(gemm(e, {xn, L.ff1_w1, L.ff1_b1, nullptr, hb, M, c.d_ff, d, RS_EPI_BIAS_SWISH_BF16, 1.f}, s));
     RS_TRY(resid_gemm(hb, L.ff1_w2, L.ff1_b2, c.d_ff, 0.5f));
-    RS_K(e, rs::launch_layernorm(x, L.ln_att_g, L.ln_att_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s), 1);
+    RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, L.ln_att_g, L.ln_att_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s));
     // the relative-position term (q + pos_bias_v) . p[c] is a wgmma product inside the attention kernel (attention_tc.cu): no score tensor in HBM
     rs::AttnArgs aa{hb, L.att_pos, L.att_bdbias, p.n_rel_pad, L.att_u, ab, enc_len, B, p.T3, c.n_heads, d / c.n_heads, c.att_left, c.att_right, c.global_tokens};
     aa.vt = at<void>(e, p.vt); aa.ld_vt = p.ld_vt;
-    {   // q | k row-major, V transposed (keys contiguous) for the attention's P.V product
-      rs::GemmArgs g{xn, L.wqkv, L.bqkv, nullptr, hb, M, 3 * d, d, RS_EPI_QKV_VT, 1.f};
-      g.out2 = at<void>(e, p.vt); g.split = 2 * d; g.ld2 = p.ld_vt;
-      RS_TRY(gemm_args(e, g, s));
-    }
-    RS_K(e, rs::launch_attention_tc(aa, s), c.global_tokens > 0 ? 2 : 1);
+    // q | k row-major, V transposed (keys contiguous) for the attention's P.V product
+    RS_TRY(gemm(e, {xn, L.wqkv, L.bqkv, nullptr, hb, M, 3 * d, d, RS_EPI_QKV_VT, 1.f, at<void>(e, p.vt), 2 * d, p.ld_vt}, s));
+    RS_LAUNCH(e, s, c.global_tokens > 0 ? 2 : 1, rs::launch_attention_tc(aa, s));
     RS_TRY(resid_gemm(ab, L.wo, L.bo, d, 1.f));
-    RS_K(e, rs::launch_layernorm(x, L.ln_conv_g, L.ln_conv_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s), 1);
-    RS_TRY(gemm(e, xn, L.pw1_w, L.pw1_b, nullptr, ab, M, 2 * d, d, RS_EPI_BIAS_GLU_BF16, 1.f, s));
-    RS_K(e, rs::launch_conv_dw(ab, cb, L.dw_w, L.dw_shift, enc_len, B, p.T3, d, c.conv_kernel, s), 1);
+    RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, L.ln_conv_g, L.ln_conv_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s));
+    RS_TRY(gemm(e, {xn, L.pw1_w, L.pw1_b, nullptr, ab, M, 2 * d, d, RS_EPI_BIAS_GLU_BF16, 1.f}, s));
+    RS_LAUNCH(e, s, 1, rs::launch_conv_dw(ab, cb, L.dw_w, L.dw_shift, enc_len, B, p.T3, d, c.conv_kernel, s));
     RS_TRY(resid_gemm(cb, L.pw2_w, L.pw2_b, d, 1.f));
-    RS_K(e, rs::launch_layernorm(x, L.ln_ff2_g, L.ln_ff2_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s), 1);
-    RS_TRY(gemm(e, xn, L.ff2_w1, L.ff2_b1, nullptr, hb, M, c.d_ff, d, RS_EPI_BIAS_SWISH_BF16, 1.f, s));
+    RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, L.ln_ff2_g, L.ln_ff2_b, nullptr, xn, nullptr, nullptr, M, d, c.ln_eps, s));
+    RS_TRY(gemm(e, {xn, L.ff2_w1, L.ff2_b1, nullptr, hb, M, c.d_ff, d, RS_EPI_BIAS_SWISH_BF16, 1.f}, s));
     RS_TRY(resid_gemm(hb, L.ff2_w2, L.ff2_b2, c.d_ff, 0.5f));
     if (i + 1 < n_layers) {   // norm_out chained with the next layer's norm_feed_forward1
       const LayerW& Ln = e->layers[i + 1];
-      RS_K(e, rs::launch_layernorm(x, L.ln_out_g, L.ln_out_b, x, xn, Ln.ln_ff1_g, Ln.ln_ff1_b, M, d, c.ln_eps, s), 1);
+      RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, L.ln_out_g, L.ln_out_b, x, xn, Ln.ln_ff1_g, Ln.ln_ff1_b, M, d, c.ln_eps, s));
     } else {
-      RS_K(e, rs::launch_layernorm(x, L.ln_out_g, L.ln_out_b, enc, nullptr, nullptr, nullptr, M, d, c.ln_eps, s), 1);
+      RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, L.ln_out_g, L.ln_out_b, enc, nullptr, nullptr, nullptr, M, d, c.ln_eps, s));
     }
   }
   if (n_layers == 0) RS_CUDA(e, cudaMemcpyAsync(enc, x, static_cast<size_t>(M) * d * 4, cudaMemcpyDeviceToDevice, s));
-  RS_K(e, rs::launch_zero_pad_rows(enc, enc_len, B, p.T3, d, s), 1);
+  RS_LAUNCH(e, s, 1, rs::launch_zero_pad_rows(enc, enc_len, B, p.T3, d, s));
   return RS_OK;
 }
 
 int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_len, int T_max, int32_t* tokens,
               int32_t* frames, int32_t* ntok, int U_max, cudaStream_t s) {
   Nvtx range("rs::rnnt_greedy (joint.enc projection + persistent decode)");
-  e->cur_stream = s;
   const rs_model_config& c = e->cfg;
   const int M = p.B * T_max;
-  RS_K(e, rs::launch_f32_to_bf16(enc, at<void>(e, p.xn), static_cast<int64_t>(M) * c.d_model, s), 1);
-  RS_TRY(gemm(e, at<void>(e, p.xn), e->dec.enc_w, e->dec.enc_b, nullptr, at<void>(e, p.encp), M, c.joint_hidden, c.d_model,
-              RS_EPI_BIAS_F32, 1.f, s));
+  RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, at<void>(e, p.xn), static_cast<int64_t>(M) * c.d_model, s));
+  RS_TRY(gemm(e, {at<void>(e, p.xn), e->dec.enc_w, e->dec.enc_b, nullptr, at<void>(e, p.encp), M, c.joint_hidden, c.d_model, RS_EPI_BIAS_F32, 1.f}, s));
   mark(e, 4, s);
-  rs::DecodeArgs da{at<float>(e, p.encp), enc_len, e->dec.out_w, e->dec.out_b, e->dec.embed, e->dec.lstm_w, e->dec.lstm_b, e->dec.gate_tab,
-                    e->dec.pred_w, e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden,
-                    c.vocab_size, U_max, c.max_symbols};
+  rs::DecodeArgs da{at<float>(e, p.encp), enc_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w, e->dec.gate_tab, e->dec.pred_w,
+                    e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, c.max_symbols};
   // One decode kernel for every batch size (windowed, weights-stationary, joint on wgmma: decode_spec.cu): an utterance's
   // logits are accumulated in the same order whether it is decoded alone or inside a batch, so results do not depend on
   // batch composition.
-  RS_K(e, rs::launch_rnnt_greedy_spec(da, at<void>(e, p.dec_ws), e->num_sms, s), 2);
+  RS_LAUNCH(e, s, 2, rs::launch_rnnt_greedy_spec(da, at<void>(e, p.dec_ws), e->num_sms, s));   // workspace memset + kernel
   return RS_OK;
 }
 
@@ -483,28 +459,26 @@ int rs_engine_create(const rs_model_config* cfg, const rs_tensor* weights, int n
   for (int i = 0; i < n_weights; ++i) e->w[weights[i].name] = Tensor{weights[i].dev_ptr, weights[i].dtype, weights[i].numel};
   int r = bind_weights(e);
   if (r != RS_OK) { snprintf(g_create_error, sizeof g_create_error, "%s", e->err); delete e; return r; }
-  if (cudaMalloc(&e->lm_tickets, rs_engine::kMaxBatch * sizeof(unsigned int)) != cudaSuccess ||
-      cudaMemset(e->lm_tickets, 0, rs_engine::kMaxBatch * sizeof(unsigned int)) != cudaSuccess) {
-    snprintf(g_create_error, sizeof g_create_error, "cannot allocate the log-mel ticket array (%s)", cudaGetErrorString(cudaGetLastError()));
-    cudaFree(e->lm_tickets);
-    delete e;
+  ce = cudaMalloc(&e->lm_tickets, rs_engine::kMaxBatch * sizeof(unsigned int));
+  if (ce == cudaSuccess) ce = cudaMemset(e->lm_tickets, 0, rs_engine::kMaxBatch * sizeof(unsigned int));
+  if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking);
+  for (auto& ev : e->ev) if (ce == cudaSuccess) ce = cudaEventCreate(&ev);
+  for (auto& ev : e->copy_ev) if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (ce != cudaSuccess) {
+    snprintf(g_create_error, sizeof g_create_error, "cannot create the log-mel ticket array, copy stream or events (%s)", cudaGetErrorString(ce));
+    rs_engine_destroy(e);
     return RS_ERR_CUDA;
   }
-  e->ev_ok = true;
-  for (auto& ev : e->ev) if (cudaEventCreate(&ev) != cudaSuccess) e->ev_ok = false;
-  e->copy_ok = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking) == cudaSuccess;
-  for (auto& ev : e->copy_ev) if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) e->copy_ok = false;
   *out = e;
   return RS_OK;
 }
 
 void rs_engine_destroy(rs_engine* e) {
   if (e == nullptr) return;
-  if (e->ev_ok) for (auto& ev : e->ev) cudaEventDestroy(ev);
+  for (auto& ev : e->ev) if (ev) cudaEventDestroy(ev);
   for (auto& ev : e->copy_ev) if (ev) cudaEventDestroy(ev);
   if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-  for (auto& ev : e->gemm_ev) cudaEventDestroy(ev);
-  for (auto& ev : e->k_ev) cudaEventDestroy(ev);
+  for (auto& ev : e->log_ev) cudaEventDestroy(ev);
   cudaFree(e->lm_tickets);
   cudaFree(e->alsd_ws);
   if (e->alsd_done_host) cudaFreeHost(e->alsd_done_host);
@@ -549,7 +523,9 @@ int rs_encode(rs_engine* e, const float* mel, const int32_t* mel_len, int B, int
   const int L_max = (F_max - 1) * e->cfg.n_window_stride;
   Plan p = make_plan(e, B, L_max, 1);
   RS_TRY(check_ws(e, p));
-  return do_encode(e, p, mel, mel_len, nullptr, enc, enc_len, n_layers, static_cast<cudaStream_t>(stream));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  RS_TRY(do_sub_conv0(e, p, mel, mel_len, nullptr, 0, B, s));
+  return do_encode(e, p, mel_len, enc, enc_len, n_layers, s);
 }
 
 int rs_rnnt_greedy(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int32_t* tokens,
@@ -558,13 +534,13 @@ int rs_rnnt_greedy(rs_engine* e, const float* enc, const int32_t* enc_len, int B
     return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_greedy: bad arguments");
   RS_CUDA(e, cudaSetDevice(e->device));
   Plan p{};
-  // only xn / encp are touched: size them for M = B*T_max rows
+  // only xn / encp / dec_ws are touched: size them for M = B*T_max rows
   p.B = B; p.M = B * T_max;
-  size_t off = 0;
-  p.xn = off; off = align_up(off + static_cast<size_t>(p.M) * e->cfg.d_model * 2);
-  p.encp = off; off = align_up(off + static_cast<size_t>(p.M) * e->cfg.joint_hidden * 4);
-  p.dec_ws = off; off = align_up(off + dec_ws_bytes(e, B));
-  p.total = off; p.L_max = 0;
+  Arena a;
+  p.xn = a.take(static_cast<size_t>(p.M) * e->cfg.d_model * 2);
+  p.encp = a.take(static_cast<size_t>(p.M) * e->cfg.joint_hidden * 4);
+  p.dec_ws = a.take(dec_ws_bytes(e, B));
+  p.total = a.off;
   RS_TRY(check_ws(e, p));
   return do_greedy(e, p, enc, enc_len, T_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
 }
@@ -573,39 +549,64 @@ int rs_rnnt_greedy(rs_engine* e, const float* enc, const int32_t* enc_len, int B
 
 namespace {
 
-// Device-resident whole path; `wav` holds f32 samples, or int16 PCM (scaled by 2^-15 inside the log-mel kernel) when i16.
-int transcribe_device(rs_engine* e, const void* wav, bool i16, const int32_t* len, int B, int L_max, int32_t* tokens,
-                      int32_t* frames, int32_t* n_tok, int U_max, cudaStream_t s) {
-  Plan p = make_plan(e, B, L_max, U_max);
-  RS_TRY(check_ws(e, p));
+int check_transcribe_args(rs_engine* e, const char* fn, const void* wav, const int32_t* len, int B, int L_max, const int32_t* tokens,
+                          const int32_t* frames, const int32_t* n_tok, int U_max) {
+  if (!e || !wav || !len || !tokens || !frames || !n_tok || B <= 0 || L_max <= 0 || U_max <= 0)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  return RS_OK;
+}
+
+// The whole path over plan `p`, the batch's utterances taken in n_chunks equal chunks (the last may be shorter): per chunk
+// log-mel and the fused first subsampling conv, then the rest of the encoder and the greedy decode over the whole batch.
+// landed[c] (when not null) is recorded once chunk c's samples have been copied in.  `wav` holds f32 samples, or int16 PCM
+// (scaled by 2^-15 inside the log-mel kernel) when i16.
+int run_pipeline(rs_engine* e, const Plan& p, const void* wav, bool i16, const int32_t* len, int n_chunks, const cudaEvent_t* landed,
+                 int32_t* tokens, int32_t* frames, int32_t* n_tok, int U_max, cudaStream_t s) {
+  const int B = p.B, per = (B + n_chunks - 1) / n_chunks;
+  const size_t row_bytes = static_cast<size_t>(p.L_max) * (i16 ? 2 : 4);
+  float* mel = at<float>(e, p.mel);
+  int32_t* mel_len = at<int32_t>(e, p.mel_len);
+  float* stats = at<float>(e, p.mel_stats);
   mark(e, 0, s);
-  RS_TRY(do_logmel(e, wav, i16, len, B, L_max, at<float>(e, p.mel), at<int32_t>(e, p.mel_len), at<float>(e, p.mel_part), at<float>(e, p.mel_stats), 0, false, s));
-  mark(e, 1, s);
-  RS_TRY(do_encode(e, p, at<float>(e, p.mel), at<int32_t>(e, p.mel_len), at<float>(e, p.mel_stats), at<float>(e, p.enc), at<int32_t>(e, p.enc_len), -1, s));
+  for (int c = 0, b0 = 0; b0 < B; ++c, b0 += per) {
+    const int nb = (B - b0 < per) ? B - b0 : per;
+    if (landed != nullptr) RS_CUDA(e, cudaStreamWaitEvent(s, landed[c], 0));
+    RS_TRY(do_logmel(e, static_cast<const char*>(wav) + b0 * row_bytes, i16, len + b0, nb, p.L_max,
+                     mel + static_cast<size_t>(b0) * p.F_max * e->cfg.n_mels, mel_len + b0, at<float>(e, p.mel_part), stats, b0, false, s));
+    mark(e, 1, s);                                      // of several chunks, the last one's record counts
+    RS_TRY(do_sub_conv0(e, p, mel, mel_len, stats, b0, nb, s));
+  }
+  RS_TRY(do_encode(e, p, mel_len, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), -1, s));
   mark(e, 3, s);
   RS_TRY(do_greedy(e, p, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), p.T3, tokens, frames, n_tok, U_max, s));
   mark(e, 5, s);
   return RS_OK;
 }
 
-// Host buffers in, host buffers out (the model.transcribe seam): H2D in utterance chunks on the copy stream, overlapped with
-// the frontend of the chunks that have landed; D2H of the tokens; synchronises before returning.
-int transcribe_batch(rs_engine* e, const void* wav_host, bool i16, const int32_t* len_host, int B, int L_max,
-                     int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, cudaStream_t s) {
+int transcribe_device(rs_engine* e, const char* fn, const void* wav, bool i16, const int32_t* len, int B, int L_max, int32_t* tokens,
+                      int32_t* frames, int32_t* n_tok, int U_max, cudaStream_t s) {
+  RS_TRY(check_transcribe_args(e, fn, wav, len, B, L_max, tokens, frames, n_tok, U_max));
   Plan p = make_plan(e, B, L_max, U_max);
   RS_TRY(check_ws(e, p));
-  const size_t esz = i16 ? 2 : 4;                       // the waveform region of the workspace is sized for f32
+  return run_pipeline(e, p, wav, i16, len, 1, nullptr, tokens, frames, n_tok, U_max, s);
+}
+
+// Host buffers in, host buffers out (the model.transcribe seam): H2D in utterance chunks on the copy stream, overlapped with
+// the frontend of the chunks that have landed; D2H of the tokens; synchronises before returning.
+int transcribe_batch(rs_engine* e, const char* fn, const void* wav_host, bool i16, const int32_t* len_host, int B, int L_max,
+                     int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, cudaStream_t s) {
+  RS_TRY(check_transcribe_args(e, fn, wav_host, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max));
+  Plan p = make_plan(e, B, L_max, U_max);
+  RS_TRY(check_ws(e, p));
+  const size_t row_bytes = static_cast<size_t>(L_max) * (i16 ? 2 : 4);   // the waveform region of the workspace is sized for f32
   char* wav = at<char>(e, p.wav);
   const char* wav_h = static_cast<const char*>(wav_host);
   int32_t* len = at<int32_t>(e, p.len);
-  float* mel = at<float>(e, p.mel);
-  int32_t* mel_len = at<int32_t>(e, p.mel_len);
-  const int n_chunks = (e->copy_ok && B >= 2 * rs_engine::kCopyChunks) ? rs_engine::kCopyChunks : 1;
+  const int n_chunks = B >= 2 * rs_engine::kCopyChunks ? rs_engine::kCopyChunks : 1;
   if (n_chunks == 1) {
-    RS_CUDA(e, cudaMemcpyAsync(wav, wav_h, static_cast<size_t>(B) * L_max * esz, cudaMemcpyHostToDevice, s));
+    RS_CUDA(e, cudaMemcpyAsync(wav, wav_h, B * row_bytes, cudaMemcpyHostToDevice, s));
     RS_CUDA(e, cudaMemcpyAsync(len, len_host, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, s));
-    RS_TRY(transcribe_device(e, wav, i16, len, B, L_max, at<int32_t>(e, p.tokens), at<int32_t>(e, p.frames),
-                             at<int32_t>(e, p.ntok), U_max, s));
   } else {
     // copies on the copy stream, chunk by chunk; log-mel and the first (fused) subsampling conv of a chunk start as
     // soon as its samples have landed.  The copy stream first waits for everything already queued on the caller's
@@ -616,21 +617,12 @@ int transcribe_batch(rs_engine* e, const void* wav_host, bool i16, const int32_t
     RS_CUDA(e, cudaMemcpyAsync(len, len_host, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, e->copy_stream));
     for (int c = 0, b0 = 0; b0 < B; ++c, b0 += per) {
       const int nb = (B - b0 < per) ? B - b0 : per;
-      RS_CUDA(e, cudaMemcpyAsync(wav + static_cast<size_t>(b0) * L_max * esz, wav_h + static_cast<size_t>(b0) * L_max * esz,
-                                 static_cast<size_t>(nb) * L_max * esz, cudaMemcpyHostToDevice, e->copy_stream));
+      RS_CUDA(e, cudaMemcpyAsync(wav + b0 * row_bytes, wav_h + b0 * row_bytes, nb * row_bytes, cudaMemcpyHostToDevice, e->copy_stream));
       RS_CUDA(e, cudaEventRecord(e->copy_ev[c], e->copy_stream));
     }
-    for (int c = 0, b0 = 0; b0 < B; ++c, b0 += per) {
-      const int nb = (B - b0 < per) ? B - b0 : per;
-      RS_CUDA(e, cudaStreamWaitEvent(s, e->copy_ev[c], 0));
-      RS_TRY(do_logmel(e, wav + static_cast<size_t>(b0) * L_max * esz, i16, len + b0, nb, L_max,
-                       mel + static_cast<size_t>(b0) * p.F_max * e->cfg.n_mels, mel_len + b0, at<float>(e, p.mel_part), at<float>(e, p.mel_stats), b0, false, s));
-      RS_TRY(do_sub_conv0(e, p, mel, mel_len, at<float>(e, p.mel_stats), b0, nb, s));
-    }
-    RS_TRY(do_encode(e, p, mel, mel_len, at<float>(e, p.mel_stats), at<float>(e, p.enc), at<int32_t>(e, p.enc_len), -1, s, true));
-    RS_TRY(do_greedy(e, p, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), p.T3, at<int32_t>(e, p.tokens),
-                     at<int32_t>(e, p.frames), at<int32_t>(e, p.ntok), U_max, s));
   }
+  RS_TRY(run_pipeline(e, p, wav, i16, len, n_chunks, n_chunks > 1 ? e->copy_ev : nullptr, at<int32_t>(e, p.tokens),
+                      at<int32_t>(e, p.frames), at<int32_t>(e, p.ntok), U_max, s));
   RS_CUDA(e, cudaMemcpyAsync(tokens_host, at<int32_t>(e, p.tokens), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(frames_host, at<int32_t>(e, p.frames), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(n_tok_host, at<int32_t>(e, p.ntok), static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
@@ -644,34 +636,24 @@ extern "C" {
 
 int rs_transcribe_device(rs_engine* e, const float* wav, const int32_t* len, int B, int L_max, int32_t* tokens,
                          int32_t* frames, int32_t* n_tok, int U_max, void* stream) {
-  if (!e || !wav || !len || !tokens || !frames || !n_tok || B <= 0 || L_max <= 0 || U_max <= 0)
-    return fail(e, RS_ERR_INVALID_ARG, "rs_transcribe_device: bad arguments");
-  RS_CUDA(e, cudaSetDevice(e->device));
-  return transcribe_device(e, wav, false, len, B, L_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
+  return transcribe_device(e, "rs_transcribe_device", wav, false, len, B, L_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
 }
 
 int rs_transcribe_device_pcm16(rs_engine* e, const int16_t* wav, const int32_t* len, int B, int L_max, int32_t* tokens,
                                int32_t* frames, int32_t* n_tok, int U_max, void* stream) {
-  if (!e || !wav || !len || !tokens || !frames || !n_tok || B <= 0 || L_max <= 0 || U_max <= 0)
-    return fail(e, RS_ERR_INVALID_ARG, "rs_transcribe_device_pcm16: bad arguments");
-  RS_CUDA(e, cudaSetDevice(e->device));
-  return transcribe_device(e, wav, true, len, B, L_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
+  return transcribe_device(e, "rs_transcribe_device_pcm16", wav, true, len, B, L_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
 }
 
 int rs_transcribe_batch(rs_engine* e, const float* wav_host, const int32_t* len_host, int B, int L_max,
                         int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, void* stream) {
-  if (!e || !wav_host || !len_host || !tokens_host || !frames_host || !n_tok_host || B <= 0 || L_max <= 0 || U_max <= 0)
-    return fail(e, RS_ERR_INVALID_ARG, "rs_transcribe_batch: bad arguments");
-  RS_CUDA(e, cudaSetDevice(e->device));
-  return transcribe_batch(e, wav_host, false, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max, static_cast<cudaStream_t>(stream));
+  return transcribe_batch(e, "rs_transcribe_batch", wav_host, false, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max,
+                          static_cast<cudaStream_t>(stream));
 }
 
 int rs_transcribe_batch_pcm16(rs_engine* e, const int16_t* wav_host, const int32_t* len_host, int B, int L_max,
                               int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, void* stream) {
-  if (!e || !wav_host || !len_host || !tokens_host || !frames_host || !n_tok_host || B <= 0 || L_max <= 0 || U_max <= 0)
-    return fail(e, RS_ERR_INVALID_ARG, "rs_transcribe_batch_pcm16: bad arguments");
-  RS_CUDA(e, cudaSetDevice(e->device));
-  return transcribe_batch(e, wav_host, true, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max, static_cast<cudaStream_t>(stream));
+  return transcribe_batch(e, "rs_transcribe_batch_pcm16", wav_host, true, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max,
+                          static_cast<cudaStream_t>(stream));
 }
 
 // ALSD beam search over encoder outputs (decode_alsd.cu; semantics: oracle/alsd_restated.py).  Synchronises: the host checks every
@@ -685,22 +667,20 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
   RS_CUDA(e, cudaSetDevice(e->device));
   Nvtx range("rs::rnnt_alsd");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  e->cur_stream = s;
   const rs_model_config& c = e->cfg;
   const int Hj = c.joint_hidden, Hp = c.pred_hidden, d = c.d_model, V = c.vocab_size, blank = c.vocab_size, n_pad = e->alsd.n_pad;
   const int M = B * T_max, R = B * beam;
   const int total_steps = T_max + static_cast<int>(u_max_ratio * static_cast<float>(T_max));
   const int max_nodes = 1 + beam * (total_steps + 1);
   // ---- workspace
-  size_t off = 0;
-  auto take = [&](size_t bytes) { off = align_up(off); size_t o = off; off += bytes; return o; };
-  const size_t o_xn = take(static_cast<size_t>(M) * d * 2), o_encp = take(static_cast<size_t>(M) * Hj * 4);
+  Arena a;
+  const size_t o_xn = a.take(static_cast<size_t>(M) * d * 2), o_encp = a.take(static_cast<size_t>(M) * Hj * 4);
   const size_t plane_cols = static_cast<size_t>(3 * Hj > 6 * Hp ? 3 * Hj : 6 * Hp);
-  const size_t o_planes = take(static_cast<size_t>(R) * plane_cols * 2), o_logits = take(static_cast<size_t>(R) * n_pad * 4);
-  const size_t o_gates = take(static_cast<size_t>(R) * 4 * Hp * 4), o_pp = take(static_cast<size_t>(R) * Hj * 4);
+  const size_t o_planes = a.take(static_cast<size_t>(R) * plane_cols * 2), o_logits = a.take(static_cast<size_t>(R) * n_pad * 4);
+  const size_t o_gates = a.take(static_cast<size_t>(R) * 4 * Hp * 4), o_pp = a.take(static_cast<size_t>(R) * Hj * 4);
   const size_t state_bytes = rs::alsd_state_bytes(B, beam, Hp, Hj, max_nodes);
-  const size_t o_state = take(state_bytes);
-  const size_t need_bytes = align_up(off);
+  const size_t o_state = a.take(state_bytes);
+  const size_t need_bytes = a.off;
   if (need_bytes > e->alsd_ws_bytes) {
     RS_CUDA(e, cudaStreamSynchronize(s));
     cudaFree(e->alsd_ws); e->alsd_ws = nullptr; e->alsd_ws_bytes = 0;
@@ -715,24 +695,24 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
   rs::AlsdState st{};
   rs::alsd_bind_state(st, ws + o_state, B, beam, Hp, Hj, max_nodes, score_norm != 0);
   // ---- joint.enc over every frame (as in the greedy path)
-  RS_K(e, rs::launch_f32_to_bf16(enc, xn, static_cast<int64_t>(M) * d, s), 1);
-  RS_TRY(gemm(e, xn, e->dec.enc_w, e->dec.enc_b, nullptr, encp, M, Hj, d, RS_EPI_BIAS_F32, 1.f, s));
+  RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, xn, static_cast<int64_t>(M) * d, s));
+  RS_TRY(gemm(e, {xn, e->dec.enc_w, e->dec.enc_b, nullptr, encp, M, Hj, d, RS_EPI_BIAS_F32, 1.f}, s));
   // predictor of the extended hypotheses of the beam being built (also the start: [blank] from the zero state)
   auto predictor = [&]() -> int {
-    RS_K(e, rs::alsd_launch_lstm_in(st, B, e->dec.embed, Hp, planes, s), 1);
-    RS_TRY(gemm(e, planes, e->alsd.lstm_w3, e->dec.lstm_b, nullptr, gates, R, 4 * Hp, 6 * Hp, RS_EPI_BIAS_F32, 1.f, s));
-    RS_K(e, rs::alsd_launch_cell(st, B, gates, Hp, planes, s), 1);
-    RS_TRY(gemm(e, planes, e->alsd.pred_w3, e->dec.pred_b, nullptr, ppn, R, Hj, 3 * Hp, RS_EPI_BIAS_F32, 1.f, s));
-    RS_K(e, rs::alsd_launch_commit(st, B, ppn, Hp, Hj, s), 2);
+    RS_LAUNCH(e, s, 1, rs::alsd_launch_lstm_in(st, B, e->dec.embed, Hp, planes, s));
+    RS_TRY(gemm(e, {planes, e->alsd.lstm_w3, e->dec.lstm_b, nullptr, gates, R, 4 * Hp, 6 * Hp, RS_EPI_BIAS_F32, 1.f}, s));
+    RS_LAUNCH(e, s, 1, rs::alsd_launch_cell(st, B, gates, Hp, planes, s));
+    RS_TRY(gemm(e, {planes, e->alsd.pred_w3, e->dec.pred_b, nullptr, ppn, R, Hj, 3 * Hp, RS_EPI_BIAS_F32, 1.f}, s));
+    RS_LAUNCH(e, s, 2, rs::alsd_launch_commit(st, B, ppn, Hp, Hj, s));
     return RS_OK;
   };
-  RS_K(e, rs::alsd_launch_init(st, B, blank, s), 1);
+  RS_LAUNCH(e, s, 1, rs::alsd_launch_init(st, B, blank, s));
   RS_TRY(predictor());
   for (int step = 0; step <= total_steps; ++step) {
-    RS_K(e, rs::alsd_launch_rows(st, B, encp, enc_len, T_max, Hj, step, planes, s), 1);
-    RS_TRY(gemm(e, planes, e->alsd.out_w3, e->alsd.out_b, nullptr, logits, R, n_pad, 3 * Hj, RS_EPI_BIAS_F32, 1.f, s));
-    RS_K(e, rs::alsd_launch_reduce(st, B, logits, n_pad, V, s), 1);
-    RS_K(e, rs::alsd_launch_select(st, B, enc_len, step, blank, u_max_ratio, recombine_returns_input != 0, s), 1);
+    RS_LAUNCH(e, s, 1, rs::alsd_launch_rows(st, B, encp, enc_len, T_max, Hj, step, planes, s));
+    RS_TRY(gemm(e, {planes, e->alsd.out_w3, e->alsd.out_b, nullptr, logits, R, n_pad, 3 * Hj, RS_EPI_BIAS_F32, 1.f}, s));
+    RS_LAUNCH(e, s, 1, rs::alsd_launch_reduce(st, B, logits, n_pad, V, s));
+    RS_LAUNCH(e, s, 1, rs::alsd_launch_select(st, B, enc_len, step, blank, u_max_ratio, recombine_returns_input != 0, s));
     RS_TRY(predictor());
     if ((step & 31) == 31) {
       RS_CUDA(e, cudaMemcpyAsync(e->alsd_done_host, st.n_done, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -740,7 +720,7 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
       if (*e->alsd_done_host >= B) break;
     }
   }
-  RS_K(e, rs::alsd_launch_output(st, B, blank, y_dev, step_dev, n_dev, score_dev, U_cap, s), 1);
+  RS_LAUNCH(e, s, 1, rs::alsd_launch_output(st, B, blank, y_dev, step_dev, n_dev, score_dev, U_cap, s));
   RS_CUDA(e, cudaStreamSynchronize(s));
   return RS_OK;
 }
@@ -751,10 +731,10 @@ int rs_resample_mono(rs_engine* e, const void* in_dev, int in_is_pcm16, const in
   if (!e || !in_dev || !len_in_dev || !taps_dev || !out_dev || !len_out_dev) return fail(e, RS_ERR_INVALID_ARG, "rs_resample_mono: bad arguments");
   RS_CUDA(e, cudaSetDevice(e->device));
   Nvtx range("rs::resample_mono");
-  e->cur_stream = static_cast<cudaStream_t>(stream);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
   rs::ResampleArgs a{in_dev, in_is_pcm16 != 0, len_in_dev, B, channels, L_in_max, taps_dev, taps_per_phase, up, down, n_pre_remove, pad,
                      out_dev, L_out_row, len_out_dev};
-  RS_K(e, rs::launch_resample_mono(a, static_cast<cudaStream_t>(stream)), 1);
+  RS_LAUNCH(e, s, 1, rs::launch_resample_mono(a, s));
   return RS_OK;
 }
 
@@ -762,15 +742,15 @@ int rs_gemm_bf16(rs_engine* e, const void* a, const void* w, const float* bias, 
                  int N, int K, int epilogue, float alpha, void* stream) {
   if (!e || !a || !w || !out) return fail(e, RS_ERR_INVALID_ARG, "rs_gemm_bf16: bad arguments");
   RS_CUDA(e, cudaSetDevice(e->device));
-  return gemm(e, a, w, bias, resid, out, M, N, K, epilogue, alpha, static_cast<cudaStream_t>(stream));
+  return gemm(e, {a, w, bias, resid, out, M, N, K, epilogue, alpha}, static_cast<cudaStream_t>(stream));
 }
 
 int rs_layernorm(rs_engine* e, const float* x, const float* gamma, const float* beta, float* out_f32, void* out_bf16,
                  int rows, int d, void* stream) {
   if (!e || !x || !gamma || !beta) return fail(e, RS_ERR_INVALID_ARG, "rs_layernorm: bad arguments");
   RS_CUDA(e, cudaSetDevice(e->device));
-  RS_K(e, rs::launch_layernorm(x, gamma, beta, out_f32, out_bf16, nullptr, nullptr, rows, d, e->cfg.ln_eps,
-                               static_cast<cudaStream_t>(stream)), 1);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, gamma, beta, out_f32, out_bf16, nullptr, nullptr, rows, d, e->cfg.ln_eps, s));
   return RS_OK;
 }
 
@@ -784,7 +764,7 @@ int rs_enable_stage_timing(rs_engine* e, int on) {
 
 // Stages: [0] log-mel, [1] subsampling, [2] conformer layers, [3] f32->bf16 + joint.enc GEMM, [4] greedy decode.
 int rs_stage_times_ms(const rs_engine* e, float* ms) {
-  if (!e || !ms || !e->ev_ok) return RS_ERR_INVALID_ARG;
+  if (!e || !ms) return RS_ERR_INVALID_ARG;
   for (int i = 0; i < 8; ++i) ms[i] = 0.f;
   if (cudaEventSynchronize(e->ev[5]) != cudaSuccess) return RS_ERR_CUDA;
   for (int i = 0; i < 5; ++i) cudaEventElapsedTime(&ms[i], e->ev[i], e->ev[i + 1]);
@@ -805,21 +785,18 @@ int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* o
 int rs_enable_kernel_timing(rs_engine* e, int on) {
   if (!e) return RS_ERR_INVALID_ARG;
   e->ktiming = on != 0;
-  e->k_tag.clear();
+  e->log.clear();
   return RS_OK;
 }
 
-// Text summary "name\tcount\ttotal_ms\n..." of every launch since rs_enable_kernel_timing(e, 1); resets the log.
+// Text summary "name\tcount\ttotal_ms\n..." of every launch logged since rs_enable_kernel_timing(e, 1); clears the log.
 int rs_kernel_timing(rs_engine* e, char* buf, int buf_bytes) {
   if (!e || !buf || buf_bytes <= 0) return RS_ERR_INVALID_ARG;
-  RS_CUDA(e, cudaDeviceSynchronize());
   std::map<std::string, std::pair<int, double>> agg;
-  for (size_t i = 0; i < e->k_tag.size(); ++i) {
-    float t = 0.f;
-    cudaEventElapsedTime(&t, e->k_ev[2 * i], e->k_ev[2 * i + 1]);
-    auto& a = agg[e->k_tag[i]];
-    a.first += 1; a.second += t;
-  }
+  RS_TRY(drain_log(e, [&](const rs_engine::Timed& t, float ms) {
+    auto& a = agg[t.tag];
+    a.first += 1; a.second += ms;
+  }));
   std::string out;
   char line[160];
   for (const auto& kv : agg) {
@@ -827,45 +804,25 @@ int rs_kernel_timing(rs_engine* e, char* buf, int buf_bytes) {
     out += line;
   }
   snprintf(buf, static_cast<size_t>(buf_bytes), "%s", out.c_str());
-  e->k_tag.clear();
-  return RS_OK;
-}
-
-int rs_debug_attention_cycles(rs_engine* e, int64_t* out16) {
-  if (!e || !out16) return RS_ERR_INVALID_ARG;
-  RS_CUDA(e, cudaDeviceSynchronize());
-  RS_CUDA(e, rs::attention_tc_debug_cycles(reinterpret_cast<long long*>(out16)));
-  return RS_OK;
-}
-
-int rs_debug_gemm_cycles(rs_engine* e, int64_t* out64) {
-  if (!e || !out64) return RS_ERR_INVALID_ARG;
-  RS_CUDA(e, cudaDeviceSynchronize());
-  RS_CUDA(e, rs::gemm_debug_cycles(reinterpret_cast<long long*>(out64)));
   return RS_OK;
 }
 
 int rs_enable_gemm_timing(rs_engine* e, int on) {
   if (!e) return RS_ERR_INVALID_ARG;
   e->gemm_timing = on != 0;
-  e->gemm_ev_used = 0;
-  e->gemm_flops = 0.0;
+  e->log.clear();
   return RS_OK;
 }
 
+// The GEMM entries of the launch log: summed device time, summed 2*M*N*K, count; clears the log.
 int rs_gemm_timing(rs_engine* e, double* ms, double* flops, int64_t* launches) {
   if (!e || !ms || !flops || !launches) return RS_ERR_INVALID_ARG;
-  double total = 0.0;
-  if (e->gemm_ev_used > 0) {
-    RS_CUDA(e, cudaEventSynchronize(e->gemm_ev[e->gemm_ev_used - 1]));
-    for (size_t i = 0; i + 1 < e->gemm_ev_used; i += 2) {
-      float t = 0.f;
-      cudaEventElapsedTime(&t, e->gemm_ev[i], e->gemm_ev[i + 1]);
-      total += t;
-    }
-  }
-  *ms = total; *flops = e->gemm_flops; *launches = static_cast<int64_t>(e->gemm_ev_used / 2);
-  e->gemm_ev_used = 0; e->gemm_flops = 0.0;
+  double total = 0.0, fl = 0.0;
+  int64_t n = 0;
+  RS_TRY(drain_log(e, [&](const rs_engine::Timed& t, float t_ms) {
+    if (t.flops > 0.0) { total += t_ms; fl += t.flops; ++n; }
+  }));
+  *ms = total; *flops = fl; *launches = n;
   return RS_OK;
 }
 

@@ -37,9 +37,6 @@ struct GemmDev {
   int epilogue;
   float alpha;
   int ldo;              // output (and residual) row stride in elements
-  // optional batching along columns (one launch for several independent products): batch b reads A columns
-  // [b*a_col_stride, +K), W rows [b*w_row_stride, +N), bias + b*bias_stride, writes columns + b*out_col_stride
-  int n_batch, a_col_stride, w_row_stride, bias_stride, out_col_stride;
   void* out2; int split, ld2;    // RS_EPI_QKV_VT
 };
 template <int BN>
@@ -57,8 +54,7 @@ struct GemmCfg {
 // from the staging buffer in an ownership where one instruction covers whole rows of the chunk.
 // EG: epilogue group compiled into a kernel instance -- 0: the common epilogues, 1: RS_EPI_QKV_VT.
 template <int EG>
-__device__ __forceinline__ void epilogue_store(const GemmDev& p, const float* stage, int tile_row0, int lane, int col0, int bt) {
-  const size_t col_off = static_cast<size_t>(bt) * p.out_col_stride;
+__device__ __forceinline__ void epilogue_store(const GemmDev& p, const float* stage, int tile_row0, int lane, int col0) {
   int epi = p.epilogue;
   if constexpr (EG == 1) {
     if (col0 < p.split) {
@@ -97,7 +93,7 @@ __device__ __forceinline__ void epilogue_store(const GemmDev& p, const float* st
                             ? make_uint4(pack_f16x2(v[0], v[1]), pack_f16x2(v[2], v[3]), pack_f16x2(v[4], v[5]), pack_f16x2(v[6], v[7]))
                             : make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
         if (row < p.M)       // __half and __nv_bfloat16 are both two bytes: one address computation
-          *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(row) * p.ldo + col_off + col0 + c8) = o;
+          *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(row) * p.ldo + col0 + c8) = o;
       }
       break;
     }
@@ -109,7 +105,7 @@ __device__ __forceinline__ void epilogue_store(const GemmDev& p, const float* st
 #pragma unroll
       for (int j = 0; j < 8; ++j) g[j] = stage[rl * kStageLd + c8 + j] * sigmoidf_fast(stage[rl * kStageLd + 16 + c8 + j]);
       if (row < p.M)
-        *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out) + static_cast<size_t>(row) * p.ldo + col_off + col0 / 2 + c8) =
+        *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out) + static_cast<size_t>(row) * p.ldo + col0 / 2 + c8) =
             make_uint4(pack_bf16x2(g[0], g[1]), pack_bf16x2(g[2], g[3]), pack_bf16x2(g[4], g[5]), pack_bf16x2(g[6], g[7]));
       break;
     }
@@ -120,7 +116,7 @@ __device__ __forceinline__ void epilogue_store(const GemmDev& p, const float* st
         const int rl = i * 4 + (lane >> 3), cw = (lane & 7) * 4;
         const int row = tile_row0 + rl;
         if (row < p.M) {
-          const size_t off = static_cast<size_t>(row) * p.ldo + col_off + col0 + cw;
+          const size_t off = static_cast<size_t>(row) * p.ldo + col0 + cw;
           float4 a = *reinterpret_cast<const float4*>(stage + rl * kStageLd + cw);
           a.x *= p.alpha; a.y *= p.alpha; a.z *= p.alpha; a.w *= p.alpha;
           if (add) {                                           // out may be resid (in place): each element is read and written by this lane only
@@ -134,9 +130,6 @@ __device__ __forceinline__ void epilogue_store(const GemmDev& p, const float* st
     }
   }
 }
-
-// Cycle stamps of CTA 0 (SM clock): [30] kernel entry, [31] kernel exit of the last launch.  Compiled in only with -DRS_PROF.
-__device__ long long g_gemm_prof[2][32];
 
 template <int BN, int EG>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -156,12 +149,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
   const int lane = lane_id();
   const int num_m = (p.M + BM - 1) / BM;
   const int num_n = (p.N + BN - 1) / BN;
-  const int tiles_per_batch = num_m * num_n;
-  const int num_tiles = tiles_per_batch * p.n_batch;
+  const int num_tiles = num_m * num_n;
   const int num_k = p.K / BK;
-#ifdef RS_PROF
-  if (blockIdx.x == 0 && threadIdx.x == 0) g_gemm_prof[0][30] = clock64();
-#endif
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a);
@@ -176,13 +165,12 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
     if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int bt = tile / tiles_per_batch, tl = tile % tiles_per_batch;
-        const int m0 = (tl / num_n) * BM, n0 = (tl % num_n) * BN;
+        const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1u);
           mbar_arrive_expect_tx(full_bar(stage), Cfg::kStageBytes);
-          tma_load_2d(smem_a(stage), &tm_a, bt * p.a_col_stride + kb * BK, m0, full_bar(stage));
-          tma_load_2d(smem_b(stage), &tm_b, kb * BK, bt * p.w_row_stride + n0, full_bar(stage));
+          tma_load_2d(smem_a(stage), &tm_a, kb * BK, m0, full_bar(stage));
+          tma_load_2d(smem_b(stage), &tm_b, kb * BK, n0, full_bar(stage));
           if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
         }
       }
@@ -195,8 +183,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
     const int g = lane >> 2, t = lane & 3;
     int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int bt = tile / tiles_per_batch, tl = tile % tiles_per_batch;
-      const int m0 = (tl / num_n) * BM, n0 = (tl % num_n) * BN;
+      const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
       float d[BN / 2];
       int prev = -1;
       for (int kb = 0; kb < num_k; ++kb) {
@@ -226,21 +213,17 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const int col = 8 * j + 2 * t;
-            const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + bt * p.bias_stride + col0 + col)) : make_float2(0.f, 0.f);
+            const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + col0 + col)) : make_float2(0.f, 0.f);
             *reinterpret_cast<float2*>(stage_f + g * kStageLd + col) = make_float2(d[c * 16 + j * 4] + b.x, d[c * 16 + j * 4 + 1] + b.y);
             *reinterpret_cast<float2*>(stage_f + (g + 8) * kStageLd + col) = make_float2(d[c * 16 + j * 4 + 2] + b.x, d[c * 16 + j * 4 + 3] + b.y);
           }
           __syncwarp();
-          epilogue_store<EG>(p, stage_f, tile_row0, lane, col0, bt);
+          epilogue_store<EG>(p, stage_f, tile_row0, lane, col0);
           __syncwarp();                                        // staging buffer reusable
         }
       }
     }
   }
-#ifdef RS_PROF
-  __syncthreads();
-  if (blockIdx.x == 0 && threadIdx.x == 0) g_gemm_prof[0][31] = clock64();
-#endif
 }
 
 // ---------------------------------------------------------------------------- host side
@@ -260,8 +243,7 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// bf16 row-major [rows, cols] -> 2-D map with a (box_rows x 64) box and 128B swizzle.
-static bool make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, char* err) {
+bool make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, char* err) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) { snprintf(err, 256, "cuTensorMapEncodeTiled entry point unavailable"); return false; }
   cuuint64_t dims[2] = {cols, rows};
@@ -275,8 +257,6 @@ static bool make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t rows, uint6
   return true;
 }
 
-cudaError_t gemm_debug_cycles(long long* out64) { return cudaMemcpyFromSymbol(out64, g_gemm_prof, sizeof(long long) * 64); }
-
 inline int epilogue_group(int epilogue) { return epilogue == RS_EPI_QKV_VT ? 1 : 0; }
 
 template <int BN, int EG>
@@ -289,15 +269,11 @@ static cudaError_t launch_bn_eg(const GemmArgs& g, int num_sms, cudaStream_t str
     attr_once.set();
   }
   CUtensorMap tm_a, tm_b;
-  const int nb = g.n_batch > 0 ? g.n_batch : 1;
-  const int lda = g.lda > 0 ? g.lda : g.K;
-  const int a_cols = nb > 1 ? (nb - 1) * g.a_col_stride + g.K : g.K;
-  const int w_rows = nb > 1 ? (nb - 1) * g.w_row_stride + g.N : g.N;
-  const int ldo = g.ldo > 0 ? g.ldo : (g.epilogue == RS_EPI_BIAS_GLU_BF16 ? g.N / 2 : g.N);
-  if (!make_tmap_bf16(&tm_a, g.a, g.M, a_cols, lda, BM, err)) return cudaErrorInvalidValue;
-  if (!make_tmap_bf16(&tm_b, g.w, w_rows, g.K, g.K, BN, err)) return cudaErrorInvalidValue;
-  GemmDev p{g.bias, g.resid, g.out, g.M, g.N, g.K, g.epilogue, g.alpha, ldo, nb, g.a_col_stride, g.w_row_stride, g.bias_stride, g.out_col_stride, g.out2, g.split, g.ld2};
-  const int tiles = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN) * nb;
+  const int ldo = g.epilogue == RS_EPI_BIAS_GLU_BF16 ? g.N / 2 : g.N;
+  if (!make_tmap_bf16(&tm_a, g.a, g.M, g.K, g.K, BM, err)) return cudaErrorInvalidValue;
+  if (!make_tmap_bf16(&tm_b, g.w, g.N, g.K, g.K, BN, err)) return cudaErrorInvalidValue;
+  GemmDev p{g.bias, g.resid, g.out, g.M, g.N, g.K, g.epilogue, g.alpha, ldo, g.out2, g.split, g.ld2};
+  const int tiles = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN);
   const int grid = tiles < num_sms ? tiles : num_sms;
   gemm_bf16_tn_kernel<BN, EG><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(tm_a, tm_b, p);
   cudaError_t e = cudaGetLastError();
@@ -323,7 +299,7 @@ cudaError_t launch_gemm(const GemmArgs& g, int num_sms, cudaStream_t stream, cha
     return cudaErrorInvalidValue;
   }
   if (g.epilogue == RS_EPI_RESID_F32 && g.resid == nullptr) { snprintf(err, 256, "gemm: residual epilogue without resid"); return cudaErrorInvalidValue; }
-  if (g.epilogue == RS_EPI_QKV_VT && (g.out2 == nullptr || g.split % 32 || g.ld2 % 8 || g.M % 8 || g.ld2 < g.M || g.n_batch > 1)) {
+  if (g.epilogue == RS_EPI_QKV_VT && (g.out2 == nullptr || g.split % 32 || g.ld2 % 8 || g.M % 8 || g.ld2 < g.M)) {
     snprintf(err, 256, "gemm: RS_EPI_QKV_VT needs out2, split %% 32 == 0, ld2 %% 8 == 0, M %% 8 == 0, ld2 >= M");
     return cudaErrorInvalidValue;
   }

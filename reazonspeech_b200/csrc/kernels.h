@@ -1,29 +1,31 @@
 // Host-side launch interface of the sm_90a kernels (internal to librs_engine.so).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace rs {
 
+// out = epi(A[M,K] * W[N,K]^T); the output row pitch is N (N / 2 for RS_EPI_BIAS_GLU_BF16)
 struct GemmArgs {
   const void* a;       // bf16 [M,K] row-major
   const void* w;       // bf16 [N,K] row-major (nn.Linear layout)
   const float* bias;   // f32 [N] or nullptr
-  const float* resid;  // f32 [M,N] for RS_EPI_RESID_F32
+  const float* resid;  // f32 [M,N] for RS_EPI_RESID_F32 (may be out)
   void* out;
   int M, N, K;
   int epilogue;        // rs_epilogue
   float alpha;
-  // optional: A row stride (elements, default K), output row stride (default N), column batching
-  int lda = 0, ldo = 0;
-  int n_batch = 1, a_col_stride = 0, w_row_stride = 0, bias_stride = 0, out_col_stride = 0;
   // RS_EPI_QKV_VT: columns >= split go, transposed, to out2 (bf16 [N - split, ld2]; ld2 >= M rounded up to 256)
   void* out2 = nullptr; int split = 0, ld2 = 0;
 };
 
 // Returns cudaSuccess or the failing CUDA error; err (>=256 B) receives a description.
 cudaError_t launch_gemm(const GemmArgs& g, int num_sms, cudaStream_t stream, char* err);
-cudaError_t gemm_debug_cycles(long long* out64);   // timeline of the last 2-CTA launch (see g_gemm_prof)
+
+// bf16 row-major [rows, cols] with a row pitch of ld elements -> 2-D TMA map with a (box_rows x 64) box and 128B swizzle,
+// out-of-bounds elements read as zero.  Returns false and writes a description into err (>=256 B) on failure.
+bool make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, char* err);
 
 cudaError_t launch_layernorm(const float* x, const float* gamma, const float* beta, float* out_f32,
                              void* out_bf16, const float* gamma2, const float* beta2, int rows, int d,
@@ -60,16 +62,13 @@ struct AttnArgs {
 };
 bool attention_tc_supported(const AttnArgs& a);
 cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t stream);
-cudaError_t attention_tc_debug_cycles(long long* out16);   // clock64 stamps of CTA (1,0,0) of the last launch
 
 struct DecodeArgs {
   const float* enc_proj;      // f32 [B*T_max, Hj]  (joint.enc applied to every frame)
   const int32_t* enc_len;
   const void* w_out;          // bf16 [V+1, Hj]
   const float* b_out;         // f32 [V+1]
-  const float* embed;         // f32 [V+1, Hp]
   const void* w_lstm;         // bf16 [4*Hp, 2*Hp]  (W_ih | W_hh, gate order i,f,g,o)
-  const float* b_lstm;        // f32 [4*Hp]  (b_ih + b_hh)
   const float* gate_tab;      // f32 [V+1, 4*Hp]: W_ih . embed[k] + b_ih + b_hh (the input half of the gates, per token)
   const void* w_pred;         // bf16 [Hj, Hp]
   const float* b_pred;        // f32 [Hj]
@@ -77,7 +76,7 @@ struct DecodeArgs {
   int B, T_max, Hj, Hp, V, U_max, max_symbols;
 };
 // windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace from rnnt_spec_workspace_bytes()
-size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp, int num_sms);
+size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp);
 size_t rnnt_spec_prof_offset(int B, int Hj, int Hp);        // where the kernel's 12 cycle counters sit inside that workspace
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream);
 

@@ -49,7 +49,7 @@ EXPORTS = [
     "rs_mel_frames", "rs_enc_frames", "rs_mel_valid", "rs_enc_valid", "rs_logmel", "rs_encode", "rs_rnnt_greedy", "rs_transcribe_device",
     "rs_transcribe_batch", "rs_transcribe_device_pcm16", "rs_transcribe_batch_pcm16", "rs_resample_mono", "rs_rnnt_alsd", "rs_gemm_bf16", "rs_layernorm", "rs_launch_count", "rs_enable_stage_timing",
     "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing", "rs_debug_decode_cycles",
-    "rs_enable_kernel_timing", "rs_kernel_timing", "rs_debug_attention_cycles", "rs_debug_gemm_cycles", "rs_stage_rows",
+    "rs_enable_kernel_timing", "rs_kernel_timing", "rs_stage_rows",
 ]
 
 
@@ -97,8 +97,6 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_stage_times_ms.argtypes = [vp, f32p]
     lib.rs_debug_decode_cycles.argtypes = [vp, ip, ip, ip, C.POINTER(C.c_int64)]
     lib.rs_debug_decode_cycles.restype = ip
-    lib.rs_debug_gemm_cycles.argtypes = [vp, C.POINTER(C.c_int64)]
-    lib.rs_debug_gemm_cycles.restype = ip
     lib.rs_stage_rows.argtypes = [vp, C.c_int64, C.POINTER(vp), C.POINTER(C.c_int64), i32p, ip, ip, C.c_int64, ip]
     lib.rs_stage_rows.restype = ip
     lib.rs_enable_kernel_timing.argtypes = [vp, ip]
@@ -461,19 +459,8 @@ class Engine:
         return out
 
     def attention_cycles(self):
-        """clock64 stamps of CTA (1,0,0) of the last tensor-core attention launch, relative to its first stamp."""
-        out = (C.c_int64 * 16)()
-        self.lib.rs_debug_attention_cycles.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
-        self._check(self.lib.rs_debug_attention_cycles(self.h, out), "rs_debug_attention_cycles")
-        v = list(out)
-        return {"start": 0, "end": int(v[6] - v[0])}          # entry and exit of thread 0 of CTA (1, 0, 0); zeros without -DRS_PROF
-
-    def gemm_cycles(self):
-        """SM clocks from entry to exit of CTA 0 of the last GEMM launch.  Only a library built with
-        RS_BUILD_FLAGS=-DRS_PROF writes the stamps; the shipped one returns whatever the buffer held (zeros)."""
-        out = (C.c_int64 * 64)()
-        self._check(self.lib.rs_debug_gemm_cycles(self.h, out), "rs_debug_gemm_cycles")
-        return {"end": int(out[31] - out[30])}
+        """Cycle stamps of the attention kernel: the kernel records none, so both are zero."""
+        return {"start": 0, "end": 0}
 
     def decode_cycles(self, B: int, L_max: int, U_max: int):
         out = (C.c_int64 * 12)()

@@ -83,8 +83,8 @@ def test_gemm_epilogues(tiny_engine, epi):
 
 @pytest.mark.parametrize("M,N,K,with_bias,alpha", [(640, 256, 1024, False, 1.0), (1000, 1024, 256, True, 0.5), (12416 // 8 + 3, 1024, 1024, True, 1.0)])
 def test_gemm_resid_in_place(tiny_engine, M, N, K, with_bias, alpha):
-    """x += alpha * (A W^T + b) with out == resid takes the TMA reduce-add epilogue (the memory system performs the add);
-    it must equal the register-path result (resid != out) bit for bit: same fp32 operations, each element reduced once."""
+    """x += alpha * (A W^T + b) in place (out == resid: each element is read and written by one lane) must equal the
+    two-buffer result (resid != out) bit for bit: same fp32 operations, each element reduced once."""
     eng = tiny_engine
     g = torch.Generator(device="cuda").manual_seed(5 + M)
     a = torch.randn(M, K, device="cuda", generator=g).to(torch.bfloat16)
