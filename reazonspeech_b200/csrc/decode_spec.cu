@@ -13,19 +13,21 @@
 //     for the whole decode and multiplies them with the relu(enc_proj + pred_proj) rows of its group
 //     (32 rows per pass) on wgmma (see the kernel's comment).  Activations keep 22 mantissa bits: every fp32 value is
 //     split into two IEEE-half terms (hi + lo), the bf16 weights are exact in half, accumulation is fp32.
-//     The LSTM step and joint.pred of the utterances that emitted are the same kind of GEMM (rows =
+//     joint.pred and the recurrent half of the LSTM of the utterances that emitted are the same kind of GEMM (rows =
 //     utterances, K split over the warps, A fragments loaded straight from L2) on mma.sync m16n8k16.
 //  3. The input half of the LSTM gates depends on the emitted token only: W_ih . embed[k] + b_ih + b_hh is a table
-//     [V+1, 4*Hp] built once at load time (pred.gate_tab), so a step multiplies just the recurrent half W_hh . h -- half the
-//     shared memory, half the MMAs, and half of what every CTA pulls through L2 per step (all CTAs read every
-//     emitting utterance's full input vector: that traffic, not the arithmetic, is what the phase costs).
+//     [V+1, 4*Hp] built once at load time (pred.gate_tab).  The recurrent half W_hh . h does not depend on the token at
+//     all, so it is computed as soon as h is known: phase P, which has to pull every emitting utterance's full new h
+//     through L2 for joint.pred anyway (that traffic, not the arithmetic, is what the phase costs), multiplies the same
+//     fragments by the CTA's W_hh rows too and keeps the result (rec) for the utterance's next step.  That step is then
+//     elementwise: gates = rec + gate_tab[token].
 //
 //   phase J  kGroups x S CTAs: window logits of the CTA's vocabulary slice -> per (utterance, frame) a grid-wide
 //            64-bit red.max of (ordered logit bits | ~row)
-//   barrier  -> every CTA reads the window's tokens, advances (t, symbols), emits
-//   phase L  utterances that emitted: LSTM gates of the CTA's units -> new h slice
+//   barrier  -> every CTA reads the window's tokens, advances (t, symbols), emits; requests the next window's enc_proj rows
+//   phase L  utterances that emitted: gates = rec + gate_tab[token] of the CTA's units -> new h slice
 //   barrier
-//   phase P  utterances that emitted: pred_proj rows of the CTA from the new h
+//   phase P  utterances that emitted: pred_proj rows and rec = W_hh . h of the CTA from the new h
 //   barrier
 #include "common.cuh"
 #include "kernels.h"
@@ -45,7 +47,8 @@ struct SpecDev {
   const __nv_bfloat16* w_lstm; const float* gate_tab; const __nv_bfloat16* w_pred; const float* b_pred;
   int32_t* tokens; int32_t* frames; int32_t* n_tok;
   unsigned long long* best;   // [3][B][kFrames] packed (ordered logit bits << 32 | ~row), 3-deep ring
-  float* hbuf;                // [2][B][Hp]
+  float* hbuf;                // [B][Hp]
+  float* rec;                 // [B][Hp][4 gates] W_hh . h, written and read only by the CTA that owns the unit
   float* ppbuf;               // [B][Hj]
   unsigned int* counter;      // grid barrier: kBarCounters arrival counters, one per 128-byte line
   long long* prof;            // [12] cycle counters of CTA 0
@@ -129,8 +132,7 @@ __global__ void __launch_bounds__(kSpThreads, 1)
 rnnt_greedy_spec_kernel(const SpecDev p) {
   constexpr int KH = HJ / 2;                 // joint k-half staged in shared memory at a time
   constexpr int LS = HP + 8;                 // W_hh row stride in halves
-  constexpr int KSW_L = (HP / 16) / kSpWarps;       // k16 steps per warp, LSTM (recurrent half only)
-  constexpr int KSW_P = (HP / 16) / kSpWarps;       // k16 steps per warp, joint.pred
+  constexpr int KSW = (HP / 16) / kSpWarps;  // k16 steps per warp of phase P
   constexpr int V4_ROW = KH / 4;             // float4 per staged row
   constexpr int ITEMS = kPassUtts * V4_ROW;  // loader items per k-half: (utterance, float4 column)
   constexpr int PERU = (ITEMS + kSpThreads - 1) / kSpThreads;
@@ -158,8 +160,8 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   const int rows_a8 = (p.rows_j + 7) & ~7;
   const uint32_t a_slab = static_cast<uint32_t>(rows_a8) * 128u;   // bytes per A slab
   constexpr uint32_t kBSlab = 8192u;                               // B slab: 64 rows x 128 B = hi plane (rows 0-31) | lo plane (rows 32-63)
-  constexpr uint32_t kBRegion = (NSLAB_H * kBSlab > 24576u) ? NSLAB_H * kBSlab : 24576u;   // >= what an M = 128 read of the last A slab overruns, and the LSTM reduction buffer
-  // Order: [A slabs | W_lstm | W_pred | pad to 1024 | B slabs (also the L / P reduction buffer) | bias, state ...].  The mma.sync B fragments of the LSTM /
+  constexpr uint32_t kBRegion = (NSLAB_H * kBSlab > 32768u) ? NSLAB_H * kBSlab : 32768u;   // >= what an M = 128 read of the last A slab overruns, and the P reduction buffer
+  // Order: [A slabs | W_lstm | W_pred | pad to 1024 | B slabs (also the P reduction buffer) | bias, state ...].  The mma.sync B fragments of the LSTM /
   // joint.pred phases read up to 8 rows past the end of their (5- or 20-row) arrays: those reads must land inside the
   // allocation, so the big B region follows the weight arrays (a 2-utterance batch otherwise read past the end of shared memory).
   const uint32_t wlp_bytes = static_cast<uint32_t>((static_cast<size_t>(4 * p.units) * LS + static_cast<size_t>(p.rows_p) * (HP + 8)) * 2);   // LS = HP + 8
@@ -169,13 +171,14 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   uint8_t* gB = gA + b_off;
   __nv_bfloat16* s_wlstm = reinterpret_cast<__nv_bfloat16*>(gA + KSLABS * a_slab);    // [4*units][LS] gate-major
   __nv_bfloat16* s_wpred = s_wlstm + static_cast<size_t>(4 * p.units) * LS;           // [rows_p][HP + 8]
-  float* s_g = reinterpret_cast<float*>(gB);                                          // B planes; also the L / P reduction buffer
+  float* s_g = reinterpret_cast<float*>(gB);                                          // B planes; also the P reduction buffer
   float* s_bout = reinterpret_cast<float*>(gB + kBRegion);                            // -inf beyond nj
   constexpr int n_bout = 128;
   float* s_c = s_bout + n_bout;                                                      // [B][units]
   unsigned long long* s_best = reinterpret_cast<unsigned long long*>(s_c + ((static_cast<size_t>(B) * p.units + 1) & ~static_cast<size_t>(1)));   // [32][kSpWarps]
-  int* s_t = reinterpret_cast<int*>(s_best + kPassRows * kSpWarps);
-  int* s_sym = s_t + B; int* s_n = s_sym + B; int* s_par = s_n + B; int* s_tok = s_par + B;
+  long long* s_prof = reinterpret_cast<long long*>(s_best + kPassRows * kSpWarps);    // [12] cycle counters of CTA 0 (rs_debug_decode_cycles)
+  int* s_t = reinterpret_cast<int*>(s_prof + 12);
+  int* s_sym = s_t + B; int* s_n = s_sym + B; int* s_tok = s_n + B;
   int* s_emit = s_tok + B; int* s_len = s_emit + B;
   int* s_act = s_len + B;                                                            // ordered list of the utterances with frames left
   int* s_cnt = s_act + B;                                                            // [0] n_emit, [1] n_active, [2..2+8) warp counts x2
@@ -207,67 +210,76 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     for (int i = tid; i < n_bout; i += kSpThreads) s_bout[i] = i < nj ? p.b_out[j0 + i] : -INFINITY;
     for (int i = tid; i < B * p.units; i += kSpThreads) s_c[i] = 0.f;
     for (int b = tid; b < B; b += kSpThreads) {
-      s_t[b] = 0; s_sym[b] = 0; s_n[b] = 0; s_par[b] = 0; s_tok[b] = blank; s_emit[b] = b; s_len[b] = p.enc_len[b];
+      s_t[b] = 0; s_sym[b] = 0; s_n[b] = 0; s_tok[b] = blank; s_len[b] = p.enc_len[b];
     }
-    if (tid == 0) { s_cnt[0] = B; s_cnt[1] = 0; }
+    if (tid < 12) s_prof[tid] = 0;
   }
   __syncthreads();
 
   unsigned int target = 0;
   int iter = 0;
-  long long prof[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  // per-phase cycle counters of CTA 0 (rs_debug_decode_cycles)
-  auto tick = [&](int slot, long long& t0) { if (cta == 0 && tid == 0) { const long long t1 = clock64(); prof[slot] += t1 - t0; t0 = t1; } };
+  // per-phase cycle counters, kept by thread 0 of CTA 0 in shared memory (in registers they would cost every thread 24)
+  auto tick = [&](int slot, long long& t0) { if (cta == 0 && tid == 0) { const long long t1 = clock64(); s_prof[slot] += t1 - t0; t0 = t1; } };
   long long tk = clock64();
 
   // ------------------------------------------------------------------------------------------------
-  // LSTM step + joint.pred for the utterances listed in s_emit[0..n_emit): token s_tok[b], state parity s_par[b]
+  // LSTM step + joint.pred for the utterances listed in s_emit[0..n_emit), which emitted token s_tok[b]
   // ------------------------------------------------------------------------------------------------
   auto lstm_and_pred = [&]() {
     const int n_emit = s_cnt[0];
-    float* red = s_g;                                  // [warps][32][24]: 24 KB of the B-plane region
-    // ---- phase L: gates[utterance][4*units] = gate_tab[token] + h . W_hh[slice]^T, K split over the warps.  Both 16-row
-    // tiles of a step (up to 32 emitting utterances) are loaded before the first MMA: one L2 round trip, one reduction.
+    // ---- phase L: gates = rec + gate_tab[token] per (utterance, unit of the CTA) -> cell -> h.  rec = W_hh . h of the
+    // utterance's previous step came from this CTA's phase P (zero before the first step, as h is).
     if (nu > 0) {
+      for (int i = tid; i < n_emit * nu; i += kSpThreads) {
+        const int b = s_emit[i / nu], u = i % nu, unit = u0 + u;
+        const float* tr = p.gate_tab + static_cast<size_t>(s_tok[b]) * 4 * HP + unit;
+        const float4 r = __ldcg(reinterpret_cast<const float4*>(p.rec + (static_cast<size_t>(b) * HP + unit) * 4));
+        float tab[4];
+#pragma unroll
+        for (int gate = 0; gate < 4; ++gate) tab[gate] = __ldg(tr + gate * HP);
+        const float ig = sigmoidf_accurate(r.x + tab[0]), fg = sigmoidf_accurate(r.y + tab[1]);
+        const float cg = tanhf(r.z + tab[2]), og = sigmoidf_accurate(r.w + tab[3]);
+        const float c2 = fg * s_c[b * p.units + u] + ig * cg;
+        s_c[b * p.units + u] = c2;
+        __stcg(p.hbuf + static_cast<size_t>(b) * HP + unit, og * tanhf(c2));
+      }
+    }
+    tick(3, tk);
+    sp_grid_barrier(p.counter, target, G);
+    tick(4, tk);
+    // ---- phase P: one load of the new h of every emitting utterance feeds both products of the CTA, K split over the
+    // warps: its rows_p rows of W_pred (-> ppbuf) and its 4 * units rows of W_hh (-> rec, the recurrent half of the
+    // utterance's next step).  Both 16-row tiles of a step (up to 32 emitting utterances) are loaded before the first MMA:
+    // one L2 round trip, one reduction.
+    if (nu + np > 0) {
+      float* red = s_g;                                // [warps][32 utterances][32]: columns 0-23 W_hh rows, 24-31 W_pred rows
       const int kw = (warp + cta) % kSpWarps;          // which k-range this warp takes (rotated per CTA against L2 hot-spotting)
       for (int m0 = 0; m0 < n_emit; m0 += 32) {
         const bool two = m0 + 16 < n_emit;             // block-uniform
-        float2 x[2][KSW_L][4];                         // [tile][k-step][row a lo, row b lo, row a hi, row b hi]
+        float2 x[2][KSW][4];                           // [tile][k-step][row a lo, row b lo, row a hi, row b hi]
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) {
           if (mt == 1 && !two) break;
           const int ea = m0 + 16 * mt + gid, eb = ea + 8;
           const bool va = ea < n_emit, vb = eb < n_emit;
-          const int ba = va ? s_emit[ea] : 0, bb = vb ? s_emit[eb] : 0;
-          const float* h_a = p.hbuf + (static_cast<size_t>(s_par[ba]) * B + ba) * HP;
-          const float* h_b = p.hbuf + (static_cast<size_t>(s_par[bb]) * B + bb) * HP;
+          const float* h_a = p.hbuf + static_cast<size_t>(va ? s_emit[ea] : 0) * HP;
+          const float* h_b = p.hbuf + static_cast<size_t>(vb ? s_emit[eb] : 0) * HP;
 #pragma unroll
-          for (int i = 0; i < KSW_L; ++i) {
-            const int off = (kw * KSW_L + i) * 16 + tig * 2;
+          for (int i = 0; i < KSW; ++i) {
+            const int off = (kw * KSW + i) * 16 + tig * 2;
             x[mt][i][0] = va ? ldcg2(h_a + off) : make_float2(0.f, 0.f); x[mt][i][2] = va ? ldcg2(h_a + off + 8) : make_float2(0.f, 0.f);
             x[mt][i][1] = vb ? ldcg2(h_b + off) : make_float2(0.f, 0.f); x[mt][i][3] = vb ? ldcg2(h_b + off + 8) : make_float2(0.f, 0.f);
           }
         }
-        // the table row of this thread's (utterance, unit) -- the reducer threads below -- is requested now as well
-        float tab[4] = {0.f, 0.f, 0.f, 0.f};
-        const int el_r = tid / nu, u_r = tid % nu, e_r = m0 + el_r;
-        const bool red_on = tid < 32 * nu && e_r < n_emit;
-        int b_r = 0;
-        if (red_on) {
-          b_r = s_emit[e_r];
-          const float* tr = p.gate_tab + static_cast<size_t>(s_tok[b_r]) * 4 * HP + u0 + u_r;
-#pragma unroll
-          for (int gate = 0; gate < 4; ++gate) tab[gate] = __ldg(tr + gate * HP);
-        }
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) {
           if (mt == 1 && !two) break;
-          float acc[3][4];
+          float acc[4][4];                               // n8 tiles 0-2: W_hh rows, 3: W_pred rows
 #pragma unroll
-          for (int n = 0; n < 3; ++n) { acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.f; }
+          for (int n = 0; n < 4; ++n) { acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.f; }
 #pragma unroll
-          for (int i = 0; i < KSW_L; ++i) {
-            const int ks = kw * KSW_L + i;
+          for (int i = 0; i < KSW; ++i) {
+            const int ks = kw * KSW + i;
             uint32_t ah[4], al[4];
             split2(x[mt][i][0], ah[0], al[0]); split2(x[mt][i][1], ah[1], al[1]);
             split2(x[mt][i][2], ah[2], al[2]); split2(x[mt][i][3], ah[3], al[3]);
@@ -281,84 +293,39 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
                 mma_f16_16816(acc[n], ah, b0, b1); mma_f16_16816(acc[n], al, b0, b1);
               }
             }
-          }
-#pragma unroll
-          for (int n = 0; n < 3; ++n) {                  // red: [warps][32 utterances][24]
-            float* r0 = red + ((warp * 32 + 16 * mt + gid) * 24) + n * 8 + tig * 2;
-            r0[0] = acc[n][0]; r0[1] = acc[n][1]; r0[8 * 24] = acc[n][2]; r0[8 * 24 + 1] = acc[n][3];
-          }
-        }
-        __syncthreads();
-        if (red_on) {
-          const int unit = u0 + u_r;
-          float gsum[4];
-#pragma unroll
-          for (int gate = 0; gate < 4; ++gate) {
-            float s = 0.f;
-#pragma unroll
-            for (int w = 0; w < kSpWarps; ++w) s += red[(w * 32 + el_r) * 24 + gate * p.units + u_r];
-            gsum[gate] = s + tab[gate];
-          }
-          const float ig = sigmoidf_accurate(gsum[0]), fg = sigmoidf_accurate(gsum[1]);
-          const float cg = tanhf(gsum[2]), og = sigmoidf_accurate(gsum[3]);
-          const float c2 = fg * s_c[b_r * p.units + u_r] + ig * cg;
-          s_c[b_r * p.units + u_r] = c2;
-          __stcg(p.hbuf + (static_cast<size_t>(s_par[b_r] ^ 1) * B + b_r) * HP + unit, og * tanhf(c2));
-        }
-        __syncthreads();
-      }
-    }
-    tick(3, tk);
-    sp_grid_barrier(p.counter, target, G);
-    tick(4, tk);
-    // ---- phase P (state parity flips for the utterances that stepped)
-    for (int e = tid; e < n_emit; e += kSpThreads) s_par[s_emit[e]] ^= 1;
-    __syncthreads();
-    if (np > 0) {
-      const int kw = (warp + cta) % kSpWarps;
-      for (int m0 = 0; m0 < n_emit; m0 += 32) {
-        const bool two = m0 + 16 < n_emit;
-        float2 x[2][KSW_P][4];
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          if (mt == 1 && !two) break;
-          const int ea = m0 + 16 * mt + gid, eb = ea + 8;
-          const bool va = ea < n_emit, vb = eb < n_emit;
-          const int ba = va ? s_emit[ea] : 0, bb = vb ? s_emit[eb] : 0;
-          const float* h_a = p.hbuf + (static_cast<size_t>(s_par[ba]) * B + ba) * HP;
-          const float* h_b = p.hbuf + (static_cast<size_t>(s_par[bb]) * B + bb) * HP;
-#pragma unroll
-          for (int i = 0; i < KSW_P; ++i) {
-            const int off = (kw * KSW_P + i) * 16 + tig * 2;
-            x[mt][i][0] = va ? ldcg2(h_a + off) : make_float2(0.f, 0.f); x[mt][i][2] = va ? ldcg2(h_a + off + 8) : make_float2(0.f, 0.f);
-            x[mt][i][1] = vb ? ldcg2(h_b + off) : make_float2(0.f, 0.f); x[mt][i][3] = vb ? ldcg2(h_b + off + 8) : make_float2(0.f, 0.f);
-          }
-        }
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          if (mt == 1 && !two) break;
-          float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int i = 0; i < KSW_P; ++i) {
-            const int ks = kw * KSW_P + i;
-            uint32_t ah[4], al[4];
-            split2(x[mt][i][0], ah[0], al[0]); split2(x[mt][i][1], ah[1], al[1]);
-            split2(x[mt][i][2], ah[2], al[2]); split2(x[mt][i][3], ah[3], al[3]);
             const __nv_bfloat16* wr = s_wpred + static_cast<size_t>(min(gid, p.rows_p - 1)) * (HP + 8) + ks * 16 + tig * 2;   // clamped like the LSTM rows
             const uint32_t b0 = *reinterpret_cast<const uint32_t*>(wr), b1 = *reinterpret_cast<const uint32_t*>(wr + 8);
-            mma_f16_16816(acc, ah, b0, b1); mma_f16_16816(acc, al, b0, b1);
+            mma_f16_16816(acc[3], ah, b0, b1); mma_f16_16816(acc[3], al, b0, b1);
           }
-          float* r0 = red + (warp * 32 + 16 * mt + gid) * 8 + tig * 2;
-          r0[0] = acc[0]; r0[1] = acc[1]; r0[8 * 8] = acc[2]; r0[8 * 8 + 1] = acc[3];
+#pragma unroll
+          for (int n = 0; n < 4; ++n) {
+            float* r0 = red + ((warp * 32 + 16 * mt + gid) * 32) + n * 8 + tig * 2;
+            r0[0] = acc[n][0]; r0[1] = acc[n][1]; r0[8 * 32] = acc[n][2]; r0[8 * 32 + 1] = acc[n][3];
+          }
         }
         __syncthreads();
-        if (tid < 32 * np) {
-          const int el = tid / np, r = tid % np, e = m0 + el;
-          if (e < n_emit) {
-            float s = 0.f;
+        // reducers: (utterance, unit) items write the unit's four gate sums, then (utterance, W_pred row) items
+        for (int i = tid; i < 32 * (nu + np); i += kSpThreads) {
+          if (i < 32 * nu) {
+            const int el = i / nu, u = i % nu, e = m0 + el;
+            if (e < n_emit) {
+              float s[4];
 #pragma unroll
-            for (int w = 0; w < kSpWarps; ++w) s += red[(w * 32 + el) * 8 + r];
-            __stcg(p.ppbuf + static_cast<size_t>(s_emit[e]) * HJ + p0 + r, s + __ldg(p.b_pred + p0 + r));
+              for (int gate = 0; gate < 4; ++gate) {
+                s[gate] = 0.f;
+#pragma unroll
+                for (int w = 0; w < kSpWarps; ++w) s[gate] += red[(w * 32 + el) * 32 + gate * p.units + u];
+              }
+              __stcg(reinterpret_cast<float4*>(p.rec + (static_cast<size_t>(s_emit[e]) * HP + u0 + u) * 4), make_float4(s[0], s[1], s[2], s[3]));
+            }
+          } else {
+            const int el = (i - 32 * nu) / np, r = (i - 32 * nu) % np, e = m0 + el;
+            if (e < n_emit) {
+              float s = 0.f;
+#pragma unroll
+              for (int w = 0; w < kSpWarps; ++w) s += red[(w * 32 + el) * 32 + 24 + r];
+              __stcg(p.ppbuf + static_cast<size_t>(s_emit[e]) * HJ + p0 + r, s + __ldg(p.b_pred + p0 + r));
+            }
           }
         }
         __syncthreads();
@@ -395,67 +362,103 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     __syncthreads();
   };
 
-  lstm_and_pred();                                // SOS: every utterance steps once on the blank (zero) embedding
-  for (int b = tid; b < B; b += kSpThreads) s_tok[b] = -1;
-  __syncthreads();
-  compact();
+  // ---- operand rows of a joint pass.  Row r = (utterance r / kFrames of the pass, frame r % kFrames of its window); lane r of
+  // every warp holds row r's utterance (-1: none) and frame.  Loader item = (utterance of the pass, float4 column):
+  // pred_proj is fetched once for the four frames of a window, and the item order is rotated by the vocabulary-slice
+  // index so the CTAs of a group, which all need the same rows, do not ask L2 for the same lines at the same instant.
+  int row_b = -1, row_t = 0;
+  float4 gv[2][PERU][kFrames];                     // [k-half][item][frame]: enc_proj, then relu(enc_proj + pred_proj)
+  auto item_rows = [&](int i, int& c4, int (&rb)[kFrames], int (&rt)[kFrames]) {
+    int it = tid + kSpThreads * i;
+    const bool in_range = it < ITEMS;
+    it = (it + slice * 29) % ITEMS;
+    const int ul = it / V4_ROW;
+    c4 = it % V4_ROW;
+#pragma unroll
+    for (int j = 0; j < kFrames; ++j) {
+      rb[j] = __shfl_sync(0xffffffffu, row_b, ul * kFrames + j);
+      rt[j] = __shfl_sync(0xffffffffu, row_t, ul * kFrames + j);
+    }
+    return in_range;
+  };
+  auto enc_row = [&](int h, int b, int t, int c4) {
+    return __ldg(reinterpret_cast<const float4*>(p.enc_proj + (static_cast<size_t>(b) * p.T_max + t) * HJ + h * KH) + c4);
+  };
+  // the rows of a pass and their enc_proj values of k-half 0.  They depend only on the consumed windows and the active
+  // list, and enc_proj is read-only during the decode, so pass 0 is requested right after compact(): those loads are in
+  // flight during phases L and P.  (Holding k-half 1 across phase P as well would need more than 255 registers.)
+  auto fetch_enc = [&](int pass) {
+    // the active utterances are dealt round-robin to the groups every iteration (any group can serve any utterance:
+    // all hold the full vocabulary), so the groups stay balanced while utterances finish at different times
+    const int n_act = s_cnt[1];
+    {
+      const int e = pass * kPassUtts + lane / kFrames, ai = grp + kGroups * e, j = lane % kFrames;
+      const int b = ai < n_act ? s_act[ai] : 0;
+      const bool ok = ai < n_act && s_t[b] + j < s_len[b];
+      row_b = ok ? b : -1; row_t = ok ? s_t[b] + j : 0;
+    }
+#pragma unroll
+    for (int i = 0; i < PERU; ++i) {
+      int c4, rb[kFrames], rt[kFrames];
+      const bool in_range = item_rows(i, c4, rb, rt);
+#pragma unroll
+      for (int j = 0; j < kFrames; ++j) gv[0][i][j] = in_range && rb[j] >= 0 ? enc_row(0, rb[j], rt[j], c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+  // pred_proj rows of both k-halves and the enc_proj values of k-half 1, all requested before the first is used
+  // -> relu(enc_proj + pred_proj); rows without a frame stay zero
+  auto add_pred = [&]() {
+    float4 q4[PERU][2];
+    unsigned ok[PERU];                             // bit j: the item's frame j is a row
+#pragma unroll
+    for (int i = 0; i < PERU; ++i) {
+      int c4, rb[kFrames], rt[kFrames];
+      const bool in_range = item_rows(i, c4, rb, rt);
+      ok[i] = 0u;
+#pragma unroll
+      for (int j = 0; j < kFrames; ++j) ok[i] |= (in_range && rb[j] >= 0 ? 1u : 0u) << j;
+      q4[i][0] = q4[i][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (ok[i] & 1u) {
+        const float* q = p.ppbuf + static_cast<size_t>(rb[0]) * HJ + 4 * c4;
+        q4[i][0] = ldcg4s(q); q4[i][1] = ldcg4s(q + KH);
+      }
+#pragma unroll
+      for (int j = 0; j < kFrames; ++j) gv[1][i][j] = (ok[i] >> j) & 1u ? enc_row(1, rb[j], rt[j], c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int i = 0; i < PERU; ++i) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int j = 0; j < kFrames; ++j) {
+          if ((ok[i] >> j) & 1u) {
+            const float4 e4 = gv[h][i][j], q = q4[i][h];
+            gv[h][i][j] = make_float4(fmaxf(e4.x + q.x, 0.f), fmaxf(e4.y + q.y, 0.f), fmaxf(e4.z + q.z, 0.f), fmaxf(e4.w + q.w, 0.f));
+          }
+        }
+      }
+    }
+  };
 
+  compact();                                      // SOS: every utterance steps once on the blank (zero) embedding
+  if (has_j) fetch_enc(0);
+  lstm_and_pred();
 
   for (;;) {
     // ---- phase J
     if (has_j) {
-      // the active utterances are dealt round-robin to the groups every iteration (any group can serve any utterance:
-      // all hold the full vocabulary), so the groups stay balanced while utterances finish at different times
       const int n_act = s_cnt[1];
       const int n_pass = ((n_act + kGroups - 1) / kGroups + kPassUtts - 1) / kPassUtts;
       for (int pass = 0; pass < n_pass; ++pass) {
-        // row r = (utterance ul of the pass, frame j of its window); lane r evaluates row r's validity for the ballot
-        int row_b, row_t;
-        {
-          const int e = pass * kPassUtts + lane / kFrames, ai = grp + kGroups * e, j = lane % kFrames;
-          const int b = ai < n_act ? s_act[ai] : 0;
-          const bool ok = ai < n_act && s_t[b] + j < s_len[b];
-          row_b = ok ? b : -1; row_t = ok ? s_t[b] + j : 0;
-        }
+        if (pass > 0) fetch_enc(pass);                        // pass 0 was requested when the window was consumed
         const unsigned mask = __ballot_sync(0xffffffffu, row_b >= 0);
         if (mask == 0u) continue;                             // identical in every warp of the CTA
-        // loader item = (utterance of the pass, float4 column): pred_proj is fetched once for the four frames of a window
-        // and the item order is rotated by the vocabulary-slice index so the CTAs of a group, which all need the same
-        // rows, do not ask L2 for the same lines at the same instant
-        float4 gv[PERU][kFrames];
-        auto load_half = [&](int h) {
-#pragma unroll
-          for (int i = 0; i < PERU; ++i) {
-            int it = tid + kSpThreads * i;
-            const bool in_range = it < ITEMS;
-            it = (it + slice * 29) % ITEMS;
-            const int ul = it / V4_ROW, c4 = it % V4_ROW;
-            int rb[kFrames], rt[kFrames];
-#pragma unroll
-            for (int j = 0; j < kFrames; ++j) {
-              rb[j] = __shfl_sync(0xffffffffu, row_b, ul * kFrames + j);     // every warp holds the row table, lane r = row r
-              rt[j] = __shfl_sync(0xffffffffu, row_t, ul * kFrames + j);
-            }
-#pragma unroll
-            for (int j = 0; j < kFrames; ++j) gv[i][j] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (in_range && rb[0] >= 0) {
-              const float4 q4 = ldcg4s(p.ppbuf + static_cast<size_t>(rb[0]) * HJ + h * KH + 4 * c4);
-#pragma unroll
-              for (int j = 0; j < kFrames; ++j) {
-                if (rb[j] >= 0) {
-                  const float4 e4 = __ldg(reinterpret_cast<const float4*>(p.enc_proj + (static_cast<size_t>(rb[j]) * p.T_max + rt[j]) * HJ + h * KH) + c4);
-                  gv[i][j] = make_float4(fmaxf(e4.x + q4.x, 0.f), fmaxf(e4.y + q4.y, 0.f), fmaxf(e4.z + q4.z, 0.f), fmaxf(e4.w + q4.w, 0.f));
-                }
-              }
-            }
-          }
-        };
         long long tj = 0;
         if (cta == 0 && tid == 0) tj = clock64();
-        auto jtick = [&](int slot) { if (cta == 0 && tid == 0) { const long long t1 = clock64(); prof[slot] += t1 - tj; tj = t1; } };
+        auto jtick = [&](int slot) { if (cta == 0 && tid == 0) { const long long t1 = clock64(); s_prof[slot] += t1 - tj; tj = t1; } };
         {
           // ---- wgmma joint: D[vocabulary row, (utterance, frame) row]; warpgroup wgi holds vocabulary rows [64 wgi, +64)
-          auto write_planes = [&]() {                         // gv -> two IEEE-half planes, 128B-swizzled K-major, 32 rows per slab
+          auto write_planes = [&](int h) {                    // gv[h] -> two IEEE-half planes, 128B-swizzled K-major, 32 rows per slab
 #pragma unroll
             for (int i = 0; i < PERU; ++i) {
               int it = tid + kSpThreads * i;
@@ -468,8 +471,8 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
                 for (int j = 0; j < kFrames; ++j) {
                   const int row = ul * kFrames + j;
                   uint32_t h0, l0, h1, l1;
-                  split2(make_float2(gv[i][j].x, gv[i][j].y), h0, l0);
-                  split2(make_float2(gv[i][j].z, gv[i][j].w), h1, l1);
+                  split2(make_float2(gv[h][i][j].x, gv[h][i][j].y), h0, l0);
+                  split2(make_float2(gv[h][i][j].z, gv[h][i][j].w), h1, l1);
                   uint8_t* dst = gB + off_k + (row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4) + sub;
                   *reinterpret_cast<uint2*>(dst) = make_uint2(h0, h1);
                   *reinterpret_cast<uint2*>(dst + 4096) = make_uint2(l0, l1);       // row + 32 of the same slab
@@ -491,16 +494,15 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
             }
             wgmma_commit();
           };
-          load_half(0);
-          write_planes();
+          add_pred();
+          write_planes(0);
           fence_proxy_async();
           __syncthreads();
           jtick(8);
           issue_half(0);
-          load_half(1);                                       // in flight under the MMAs of half 0
           wgmma_wait<0>();
           __syncthreads();                                    // half 0 consumed by both warpgroups: the planes may be rewritten
-          write_planes();
+          write_planes(1);
           fence_proxy_async();
           __syncthreads();
           issue_half(1);
@@ -581,17 +583,18 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     compact();
     const int n_active = s_cnt[1];
     tick(2, tk);
-    prof[7] += 1;
+    if (cta == 0 && tid == 0) s_prof[7] += 1;
+    if (has_j) fetch_enc(0);                      // the next window's enc_proj rows, in flight under phases L and P
     if (s_cnt[0] > 0) lstm_and_pred();
     if (n_active == 0) break;
   }
   if (cta == 0) for (int b = tid; b < B; b += kSpThreads) p.n_tok[b] = s_n[b];
-  if (cta == 0 && tid == 0) for (int i = 0; i < 12; ++i) p.prof[i] = prof[i];
+  if (cta == 0 && tid == 0) for (int i = 0; i < 12; ++i) p.prof[i] = s_prof[i];
 }
 
-// workspace: hbuf | ppbuf | pad to 128 | barrier counters (kBarCounters lines) | prof (128 B) | best
+// workspace: hbuf | rec | ppbuf | pad to 128 | barrier counters (kBarCounters lines) | prof (128 B) | best
 static size_t spec_counter_offset(int B, int Hj, int Hp) {
-  return (static_cast<size_t>(2) * B * Hp * 4 + static_cast<size_t>(B) * Hj * 4 + 127) & ~static_cast<size_t>(127);
+  return (static_cast<size_t>(5) * B * Hp * 4 + static_cast<size_t>(B) * Hj * 4 + 127) & ~static_cast<size_t>(127);
 }
 size_t rnnt_spec_prof_offset(int B, int Hj, int Hp) { return spec_counter_offset(B, Hj, Hp) + static_cast<size_t>(kBarCounters) * kBarStride * 4; }
 size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp) {
@@ -622,7 +625,8 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   if (reinterpret_cast<uintptr_t>(workspace) & 15u) return cudaErrorInvalidValue;   // the window is read with 16-byte loads
   char* ws = static_cast<char*>(workspace);
   p.hbuf = reinterpret_cast<float*>(ws);
-  p.ppbuf = reinterpret_cast<float*>(ws + static_cast<size_t>(2) * a.B * a.Hp * 4);
+  p.rec = reinterpret_cast<float*>(ws + static_cast<size_t>(a.B) * a.Hp * 4);
+  p.ppbuf = reinterpret_cast<float*>(ws + static_cast<size_t>(5) * a.B * a.Hp * 4);
   p.counter = reinterpret_cast<unsigned int*>(ws + spec_counter_offset(a.B, a.Hj, a.Hp));
   p.prof = reinterpret_cast<long long*>(ws + rnnt_spec_prof_offset(a.B, a.Hj, a.Hp));
   p.best = reinterpret_cast<unsigned long long*>(ws + rnnt_spec_prof_offset(a.B, a.Hj, a.Hp) + 128);
@@ -631,16 +635,16 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   p.rows_j = (a.V + 1 + p.S - 1) / p.S;
   p.units = (a.Hp + G - 1) / G;
   p.rows_p = (a.Hj + G - 1) / G;
-  if (4 * p.units > 24 || p.rows_p > 8 || 32 * p.units > kSpThreads || 32 * p.rows_p > kSpThreads || a.gate_tab == nullptr) return cudaErrorInvalidValue;
+  if (4 * p.units > 24 || p.rows_p > 8 || a.gate_tab == nullptr) return cudaErrorInvalidValue;   // the n8 tiles of phase P
   cudaError_t e = cudaMemsetAsync(workspace, 0, rnnt_spec_workspace_bytes(a.B, a.Hj, a.Hp), stream);
   if (e != cudaSuccess) return e;
-  const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + kPassRows * kSpWarps * 8 + static_cast<size_t>(a.B) * 8 * 4 +
+  const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + (kPassRows * kSpWarps + 12) * 8 + static_cast<size_t>(a.B) * 7 * 4 +
                        (2 + 2 * kSpWarps) * 4 + 64;
   const size_t w_lp = (static_cast<size_t>(4 * p.units) * (a.Hp + 8) + static_cast<size_t>(p.rows_p) * (a.Hp + 8)) * 2;
   if (p.rows_j > 128) return cudaErrorInvalidValue;
   const size_t rows_a8 = (p.rows_j + 7) & ~7;
   const size_t b_bytes = static_cast<size_t>(a.Hj / 2 / 64) * 8192;
-  const size_t b_region = b_bytes > 24576 ? b_bytes : 24576;     // also the [8 warps][32][24] fp32 reduction buffer of the LSTM phase
+  const size_t b_region = b_bytes > 32768 ? b_bytes : 32768;     // also the [8 warps][32][32] fp32 reduction buffer of phase P
   const size_t ab = ((static_cast<size_t>(a.Hj / 64) * rows_a8 * 128 + w_lp + 1023) & ~static_cast<size_t>(1023));   // A slabs, W_lstm, W_pred, pad
   const size_t smem = 1024 + ab + b_region + 128 * 4 + state + 16;
   if (smem > 227 * 1024) return cudaErrorInvalidValue;
