@@ -177,7 +177,7 @@ int64_t rs_launch_count(const rs_engine* e);
 /* Per-stage device time of the last rs_transcribe_* call when timing was enabled. */
 int rs_enable_stage_timing(rs_engine* e, int on);
 int rs_stage_times_ms(const rs_engine* e, float* ms /*[8]*/);
-int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* out8);   /* profiling aid, see engine.cu */
+int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* out12);  /* profiling aid, see engine.cu */
 /* Per-launch CUDA-event timing of the wgmma GEMM (the dominant kernel): while enabled every GEMM
  * launch is bracketed by two events on its stream.  rs_gemm_timing() synchronises, returns the summed
  * device time, the summed algorithmic FLOPs (2*M*N*K) and the launch count since it was enabled or

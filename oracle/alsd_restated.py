@@ -56,6 +56,7 @@ class AlsdResult:
     timestamp: List[int]               # pack_hypotheses: the leading -1 removed
     score: float
     nbest: List[BeamHyp] = field(default_factory=list)
+    from_final: bool = True            # False: no hypothesis finished, the winner is the best of the last beam
 
     @property
     def tokens(self) -> List[int]:
@@ -121,7 +122,7 @@ def alsd_beam(enc: torch.Tensor, sd: StateDict, cfg: ModelConfig, beam: int = 4,
         nbest = sorted(pool, key=key, reverse=True)
         best = nbest[0]
         return AlsdResult(best.y, best.timestamp[1:] if best.timestamp and best.timestamp[0] == -1 else best.timestamp,
-                          best.score, nbest)
+                          best.score, nbest, from_final=bool(final))
     finally:
         torch.set_num_threads(n_threads)
 

@@ -17,9 +17,12 @@
 //                        list (hypotheses that took the blank at the last frame), back-pointer nodes of the extensions
 //   alsd_lstm_in_kernel  extended hypotheses: [embed[token] | h_parent] -> three bf16 planes
 //   [GEMM]               gates = planes . [W_lstm x3]^T + b
-//   alsd_cell_kernel     LSTM cell, new (h, c); h -> three bf16 planes         (kept hypotheses: state copied from the parent)
-//   [GEMM]               pred_proj = planes . [W_pred x3]^T + b_pred
-//   alsd_commit_kernel   the new beam's state / pred_proj become current
+//   alsd_cell_kernel     LSTM cell, new (h, c) (kept hypotheses: copied from the parent); h -> three bf16 planes
+//   [GEMM]               pred_proj = planes . [W_pred x3]^T + b_pred, straight into the next beam
+//
+// The state holds two beams, the current one and the one the step builds; the host swaps them after every predictor pass.
+// A kept hypothesis's pred_proj is recomputed from the h it inherits rather than copied: a GEMM row does not depend on the
+// other rows or on its position, so the value is the parent's bit for bit.
 //
 // Scores are doubles (Python floats in NeMo), log-probabilities fp32 (torch.log_softmax of fp32 logits).
 #include <cfloat>
@@ -49,17 +52,17 @@ __global__ void __launch_bounds__(128)
 alsd_rows_kernel(const AlsdState st, const float* __restrict__ enc_proj, const int32_t* __restrict__ enc_len, int T_max, int Hj,
                  int step, __nv_bfloat16* __restrict__ planes) {
   const int r = blockIdx.x, b = r / st.beam, k = r % st.beam;
-  const int n_h = st.n_hyp[b];
+  const int n_h = st.cur.n_hyp[b];
   const int T = enc_len[b];
   int t = -1;
   if (!st.done[b] && k < n_h) {
-    t = step - st.u[r];
+    t = step - st.cur.u[r];
     if (t > T - 1) t = -1;
   }
   if (threadIdx.x == 0) st.row_t[r] = t;
   __nv_bfloat16* row = planes + static_cast<size_t>(r) * 3 * Hj;
   const float* ep = enc_proj + (static_cast<size_t>(b) * T_max + (t >= 0 ? t : 0)) * Hj;
-  const float* pp = st.pp + static_cast<size_t>(r) * Hj;
+  const float* pp = st.cur.pp + static_cast<size_t>(r) * Hj;
   for (int j = threadIdx.x; j < Hj; j += blockDim.x) {
     const float x = t >= 0 ? fmaxf(ep[j] + pp[j], 0.f) : 0.f;
     __nv_bfloat16 h, m, l;
@@ -140,33 +143,44 @@ __device__ __forceinline__ double logaddexp(double a, double b) {
 
 // grid (B), block 32 (lane 0 does the serial work: at most beam * (beam + 1) <= 72 candidates).
 __global__ void __launch_bounds__(32)
-alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int step, int blank, float u_max_ratio, int recombine_returns_input) {
+alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int step, float u_max_ratio, int recombine_returns_input) {
   const int b = blockIdx.x;
   if (threadIdx.x != 0 || st.done[b]) return;
   const int K = st.beam;
   const int T = enc_len[b];
   const int u_max = static_cast<int>(u_max_ratio * static_cast<float>(T));
-  if (step >= T + u_max) {                             // the loop of the reference ends here whether or not hypotheses remain
+  const AlsdBeam& cur = st.cur;
+  const int n_h = cur.n_hyp[b];
+  // the search of utterance b ends: no kernel writes its beam again, so the next beam becomes a copy of the current one and
+  // both halves hold it whichever way later swaps fall (alsd_output_kernel reads it when no hypothesis finished)
+  auto finish = [&]() {
+    st.nx.n_hyp[b] = n_h;
+    for (int k = 0; k < n_h; ++k) {
+      const int r = b * K + k;
+      st.nx.score[r] = cur.score[r]; st.nx.hash[r] = cur.hash[r]; st.nx.u[r] = cur.u[r]; st.nx.node[r] = cur.node[r];
+    }
     st.done[b] = 1;
     atomicAdd(st.n_done, 1);
+  };
+  if (step >= T + u_max) {                             // the loop of the reference ends here whether or not hypotheses remain
+    finish();
     return;
   }
   // A in the reference's order: for every live hypothesis of B: [stay, extension 0 .. K-1]
   double a_score[kMaxBeam * (kMaxBeam + 1)];
   int a_par[kMaxBeam * (kMaxBeam + 1)], a_tok[kMaxBeam * (kMaxBeam + 1)];
   int n_a = 0;
-  const int n_h = st.n_hyp[b];
   for (int k = 0; k < n_h; ++k) {
     const int r = b * K + k;
     const int t = st.row_t[r];
     if (t < 0) continue;                               // past the last frame: dropped (it entered `final` when it got there)
-    const double s0 = st.score[r];
+    const double s0 = cur.score[r];
     const double stay = s0 + static_cast<double>(st.cand_logp[r * (kMaxBeam + 1)]);
     a_score[n_a] = stay; a_par[n_a] = k; a_tok[n_a] = -1; ++n_a;
     if (t == T - 1) {                                  // finished hypothesis: keep the best by score / len(y) (score_norm), first one on ties
-      const double key = st.score_norm ? stay / static_cast<double>(st.u[r] + 1) : stay;
+      const double key = st.score_norm ? stay / static_cast<double>(cur.u[r] + 1) : stay;
       if (!st.has_final[b] || key > st.final_key[b]) {
-        st.has_final[b] = 1; st.final_key[b] = key; st.final_score[b] = stay; st.final_node[b] = st.node[r]; st.final_u[b] = st.u[r];
+        st.has_final[b] = 1; st.final_key[b] = key; st.final_score[b] = stay; st.final_node[b] = cur.node[r]; st.final_u[b] = cur.u[r];
       }
     }
     for (int c = 0; c < K; ++c) {
@@ -175,8 +189,7 @@ alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int 
     }
   }
   if (n_a == 0) {                                      // every hypothesis has left the lattice: the reference breaks out of its loop
-    st.done[b] = 1;
-    atomicAdd(st.n_done, 1);
+    finish();
     return;
   }
   // the K best of A by score, stable
@@ -191,15 +204,15 @@ alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int 
     used[best] = true;
     pick[j] = best;
   }
-  // new beam (written to the `next` half; the commit kernel swaps)
+  // new beam, written to the `nx` half
   double n_score[kMaxBeam];
   unsigned long long n_hash[kMaxBeam];
   int n_len[kMaxBeam];
   for (int j = 0; j < n_new; ++j) {
     const int a = pick[j], pk = a_par[a], pr = b * K + pk;
     n_score[j] = a_score[a];
-    n_hash[j] = a_tok[a] >= 0 ? st.hash[pr] * 1000003ull + static_cast<unsigned long long>(a_tok[a] + 1) : st.hash[pr];
-    n_len[j] = st.u[pr] + (a_tok[a] >= 0 ? 1 : 0);
+    n_hash[j] = a_tok[a] >= 0 ? cur.hash[pr] * 1000003ull + static_cast<unsigned long long>(a_tok[a] + 1) : cur.hash[pr];
+    n_len[j] = cur.u[pr] + (a_tok[a] >= 0 ? 1 : 0);
   }
   // NeMo's recombine_hypotheses: the score of a later duplicate is added (logaddexp) into the first occurrence; as recalled, the
   // reference then returns its INPUT list, duplicates included (oracle/alsd_restated.py `recombine_returns_input`)
@@ -216,37 +229,36 @@ alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int 
   for (int j = 0; j < n_new; ++j) {
     if (dropped[j]) continue;
     const int a = pick[j], pk = a_par[a], pr = b * K + pk, nr = b * K + w;
-    st.nx_score[nr] = n_score[j];
-    st.nx_hash[nr] = n_hash[j];
+    st.nx.score[nr] = n_score[j];
+    st.nx.hash[nr] = n_hash[j];
     st.nx_parent[nr] = pk;
     st.nx_tok[nr] = a_tok[a];
     if (a_tok[a] >= 0) {                               // extension: one more token, emitted at alignment step `step`
-      st.nx_u[nr] = st.u[pr] + 1;
+      st.nx.u[nr] = cur.u[pr] + 1;
       const int node = st.n_nodes[b]++;
-      st.node_parent[static_cast<size_t>(b) * st.max_nodes + node] = st.node[pr];
+      st.node_parent[static_cast<size_t>(b) * st.max_nodes + node] = cur.node[pr];
       st.node_tok[static_cast<size_t>(b) * st.max_nodes + node] = a_tok[a];
       st.node_step[static_cast<size_t>(b) * st.max_nodes + node] = step;
-      st.nx_node[nr] = node;
+      st.nx.node[nr] = node;
     } else {
-      st.nx_u[nr] = st.u[pr];
-      st.nx_node[nr] = st.node[pr];
+      st.nx.u[nr] = cur.u[pr];
+      st.nx.node[nr] = cur.node[pr];
     }
     ++w;
   }
-  st.nx_n_hyp[b] = w;
-  (void)blank;
+  st.nx.n_hyp[b] = w;
 }
 
 // ---------------------------------------------------------------------------------------------- predictor of the extensions
 // grid (B * beam), block 128: rows of the NEXT beam.  Extended hypotheses get [embed[token] | h_parent] as three bf16 planes
-// (K = 2 * Hp per plane); kept ones (and absent rows) get zeros and are skipped by the cell kernel.
+// (K = 2 * Hp per plane); kept ones (and absent rows) get zeros, and the cell kernel ignores their gates.
 __global__ void __launch_bounds__(128)
 alsd_lstm_in_kernel(const AlsdState st, const float* __restrict__ embed, int Hp, __nv_bfloat16* __restrict__ planes) {
   const int r = blockIdx.x, b = r / st.beam, k = r % st.beam;
-  const bool ext = !st.done[b] && k < st.nx_n_hyp[b] && st.nx_tok[r] >= 0;
+  const bool ext = !st.done[b] && k < st.nx.n_hyp[b] && st.nx_tok[r] >= 0;
   __nv_bfloat16* row = planes + static_cast<size_t>(r) * 6 * Hp;
   const float* e = embed + static_cast<size_t>(ext ? st.nx_tok[r] : 0) * Hp;
-  const float* h = st.h + (static_cast<size_t>(b) * st.beam + (ext ? st.nx_parent[r] : 0)) * Hp;
+  const float* h = st.cur.h + (static_cast<size_t>(b) * st.beam + (ext ? st.nx_parent[r] : 0)) * Hp;
   for (int j = threadIdx.x; j < 2 * Hp; j += blockDim.x) {
     const float x = ext ? (j < Hp ? e[j] : h[j - Hp]) : 0.f;
     __nv_bfloat16 hi, mid, lo;
@@ -255,12 +267,12 @@ alsd_lstm_in_kernel(const AlsdState st, const float* __restrict__ embed, int Hp,
   }
 }
 
-// grid (B * beam), block 128: LSTM cell (gate order i, f, g, o; biases already in `gates`), new state into the `next` half;
-// h as three bf16 planes for joint.pred.  Kept hypotheses copy (h, c) from their parent; their pred_proj is copied at commit.
+// grid (B * beam), block 128: LSTM cell (gate order i, f, g, o; biases already in `gates`), new state into the `nx` half;
+// h of every live row as three bf16 planes for joint.pred.  Kept hypotheses copy (h, c) from their parent.
 __global__ void __launch_bounds__(128)
 alsd_cell_kernel(const AlsdState st, const float* __restrict__ gates, int Hp, __nv_bfloat16* __restrict__ planes) {
   const int r = blockIdx.x, b = r / st.beam, k = r % st.beam;
-  const bool live = !st.done[b] && k < st.nx_n_hyp[b];
+  const bool live = !st.done[b] && k < st.nx.n_hyp[b];
   const bool ext = live && st.nx_tok[r] >= 0;
   const size_t pr = static_cast<size_t>(b) * st.beam + (live ? st.nx_parent[r] : 0);
   const float* g = gates + static_cast<size_t>(r) * 4 * Hp;
@@ -270,63 +282,32 @@ alsd_cell_kernel(const AlsdState st, const float* __restrict__ gates, int Hp, __
     if (ext) {
       const float ig = sigmoidf_accurate(g[j]), fg = sigmoidf_accurate(g[Hp + j]);
       const float cg = tanhf(g[2 * Hp + j]), og = sigmoidf_accurate(g[3 * Hp + j]);
-      c2 = fg * st.c[pr * Hp + j] + ig * cg;
+      c2 = fg * st.cur.c[pr * Hp + j] + ig * cg;
       h2 = og * tanhf(c2);
     } else if (live) {
-      h2 = st.h[pr * Hp + j]; c2 = st.c[pr * Hp + j];
+      h2 = st.cur.h[pr * Hp + j]; c2 = st.cur.c[pr * Hp + j];
     }
-    st.nx_h[static_cast<size_t>(r) * Hp + j] = h2;
-    st.nx_c[static_cast<size_t>(r) * Hp + j] = c2;
+    st.nx.h[static_cast<size_t>(r) * Hp + j] = h2;
+    st.nx.c[static_cast<size_t>(r) * Hp + j] = c2;
     __nv_bfloat16 hi, mid, lo;
-    split3(ext ? h2 : 0.f, hi, mid, lo);
+    split3(h2, hi, mid, lo);
     row[j] = hi; row[Hp + j] = mid; row[2 * Hp + j] = lo;
   }
 }
 
-// grid (B * beam), block 128: the next beam becomes current.  pred_proj: the GEMM's row for extended hypotheses, the parent's for
-// kept ones (read from the current half before it is overwritten: every CTA reads its parent row first, then all write after a
-// grid-wide ordering provided by running this in two launches: phase 0 stages into nx_pp, phase 1 copies nx_* over the current).
-__global__ void __launch_bounds__(128)
-alsd_commit_kernel(const AlsdState st, const float* __restrict__ pp_new, int Hp, int Hj, int phase) {
-  const int r = blockIdx.x, b = r / st.beam, k = r % st.beam;
-  if (st.done[b]) return;
-  const bool live = k < st.nx_n_hyp[b];
-  if (phase == 0) {
-    if (!live) return;
-    const bool ext = st.nx_tok[r] >= 0;
-    const float* src = ext ? pp_new + static_cast<size_t>(r) * Hj : st.pp + (static_cast<size_t>(b) * st.beam + st.nx_parent[r]) * Hj;
-    for (int j = threadIdx.x; j < Hj; j += blockDim.x) st.nx_pp[static_cast<size_t>(r) * Hj + j] = src[j];
-    return;
-  }
-  if (live) {
-    for (int j = threadIdx.x; j < Hj; j += blockDim.x) st.pp[static_cast<size_t>(r) * Hj + j] = st.nx_pp[static_cast<size_t>(r) * Hj + j];
-    for (int j = threadIdx.x; j < Hp; j += blockDim.x) {
-      st.h[static_cast<size_t>(r) * Hp + j] = st.nx_h[static_cast<size_t>(r) * Hp + j];
-      st.c[static_cast<size_t>(r) * Hp + j] = st.nx_c[static_cast<size_t>(r) * Hp + j];
-    }
-  }
-  if (threadIdx.x == 0) {
-    if (live) {
-      st.score[r] = st.nx_score[r]; st.hash[r] = st.nx_hash[r]; st.u[r] = st.nx_u[r]; st.node[r] = st.nx_node[r];
-    }
-    if (k == 0) st.n_hyp[b] = st.nx_n_hyp[b];
-  }
-}
-
-// grid (B), block 32: initial beam = one hypothesis [blank] with score 0 (its predictor state is computed by one pass of the
-// lstm_in / cell / commit kernels with nx_tok = blank -> the zero embedding)
+// grid (B), block 32, on the zeroed state: initial beam = one hypothesis [blank] with score 0 in the `nx` half (its predictor
+// state is computed by one predictor pass with nx_tok = blank -> the zero embedding, from the zero state of the `cur` half)
 __global__ void alsd_init_kernel(const AlsdState st, int blank) {
   const int b = blockIdx.x;
   if (threadIdx.x != 0) return;
   const int K = st.beam;
-  st.done[b] = 0; st.has_final[b] = 0; st.n_hyp[b] = 0; st.nx_n_hyp[b] = 1; st.n_nodes[b] = 1;
+  st.nx.n_hyp[b] = 1; st.n_nodes[b] = 1;
   st.node_parent[static_cast<size_t>(b) * st.max_nodes] = -1;
   st.node_tok[static_cast<size_t>(b) * st.max_nodes] = blank;
   st.node_step[static_cast<size_t>(b) * st.max_nodes] = -1;
-  for (int k = 0; k < K; ++k) { st.u[b * K + k] = 0; st.nx_tok[b * K + k] = -1; st.nx_parent[b * K + k] = 0; }
+  for (int k = 1; k < K; ++k) st.nx_tok[b * K + k] = -1;
   const int r = b * K;
-  st.nx_score[r] = 0.0; st.nx_hash[r] = 1469598103934665603ull; st.nx_u[r] = 0; st.nx_node[r] = 0; st.nx_tok[r] = blank; st.nx_parent[r] = 0;
-  if (b == 0) *st.n_done = 0;
+  st.nx.hash[r] = 1469598103934665603ull; st.nx_tok[r] = blank;
 }
 
 // grid (B), block 32: walk the back-pointers of the winning hypothesis (best finished one; with none, the best of the last
@@ -341,13 +322,14 @@ __global__ void alsd_output_kernel(const AlsdState st, int blank, int32_t* __res
   else {
     int best = 0;
     double bk = -DBL_MAX;
-    for (int k = 0; k < st.n_hyp[b]; ++k) {
+    const AlsdBeam& cur = st.cur;
+    for (int k = 0; k < cur.n_hyp[b]; ++k) {
       const int r = b * st.beam + k;
-      const double key = st.score_norm ? st.score[r] / static_cast<double>(st.u[r] + 1) : st.score[r];
+      const double key = st.score_norm ? cur.score[r] / static_cast<double>(cur.u[r] + 1) : cur.score[r];
       if (key > bk) { bk = key; best = k; }
     }
     const int r = b * st.beam + best;
-    node = st.node[r]; u = st.u[r]; score = st.score[r];
+    node = cur.node[r]; u = cur.u[r]; score = cur.score[r];
   }
   n_out[b] = u;
   score_out[b] = score;
@@ -366,43 +348,25 @@ __global__ void alsd_output_kernel(const AlsdState st, int blank, int32_t* __res
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ host side
-size_t alsd_state_bytes(int B, int beam, int Hp, int Hj, int max_nodes) {
+void alsd_layout_state(AlsdState& st, Arena& a, char* base, int B, int beam, int Hp, int Hj, int max_nodes, bool score_norm) {
   const size_t R = static_cast<size_t>(B) * beam;
-  size_t n = 0;
-  auto add = [&](size_t bytes) { n = (n + 255) & ~static_cast<size_t>(255); n += bytes; };
-  for (int i = 0; i < 2; ++i) { add(R * 8); add(R * 8); add(R * 4); add(R * 4); }          // score, hash, u, node (cur + next)
-  add(R * 4); add(R * 4); add(R * 4);                                                       // nx_parent, nx_tok, row_t
-  for (int i = 0; i < 2; ++i) { add(R * Hp * 4); add(R * Hp * 4); add(R * Hj * 4); }        // h, c, pp (cur + next)
-  add(R * (kMaxBeam + 1) * 4); add(R * kMaxBeam * 4);                                       // candidates
-  add(static_cast<size_t>(B) * 4 * 8);                                                      // n_hyp, nx_n_hyp, done, has_final, n_nodes, final_node, final_u (+pad)
-  add(static_cast<size_t>(B) * 8 * 2);                                                      // final_key, final_score
-  add(static_cast<size_t>(B) * max_nodes * 4 * 3);                                          // node tree
-  add(256);                                                                                 // n_done
-  return n + 256;
-}
-
-void alsd_bind_state(AlsdState& st, void* base, int B, int beam, int Hp, int Hj, int max_nodes, bool score_norm) {
-  const size_t R = static_cast<size_t>(B) * beam;
-  char* p = static_cast<char*>(base);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { off = (off + 255) & ~static_cast<size_t>(255); char* q = p + off; off += bytes; return q; };
+  auto take = [&](size_t bytes) { return reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(base) + a.take(bytes)); };
   st.beam = beam; st.max_nodes = max_nodes; st.score_norm = score_norm ? 1 : 0;
-  st.score = reinterpret_cast<double*>(take(R * 8)); st.hash = reinterpret_cast<unsigned long long*>(take(R * 8));
-  st.u = reinterpret_cast<int*>(take(R * 4)); st.node = reinterpret_cast<int*>(take(R * 4));
-  st.nx_score = reinterpret_cast<double*>(take(R * 8)); st.nx_hash = reinterpret_cast<unsigned long long*>(take(R * 8));
-  st.nx_u = reinterpret_cast<int*>(take(R * 4)); st.nx_node = reinterpret_cast<int*>(take(R * 4));
-  st.nx_parent = reinterpret_cast<int*>(take(R * 4)); st.nx_tok = reinterpret_cast<int*>(take(R * 4)); st.row_t = reinterpret_cast<int*>(take(R * 4));
-  st.h = reinterpret_cast<float*>(take(R * Hp * 4)); st.c = reinterpret_cast<float*>(take(R * Hp * 4)); st.pp = reinterpret_cast<float*>(take(R * Hj * 4));
-  st.nx_h = reinterpret_cast<float*>(take(R * Hp * 4)); st.nx_c = reinterpret_cast<float*>(take(R * Hp * 4)); st.nx_pp = reinterpret_cast<float*>(take(R * Hj * 4));
-  st.cand_logp = reinterpret_cast<float*>(take(R * (kMaxBeam + 1) * 4)); st.cand_tok = reinterpret_cast<int*>(take(R * kMaxBeam * 4));
-  int* ints = reinterpret_cast<int*>(take(static_cast<size_t>(B) * 4 * 8));
-  st.n_hyp = ints; st.nx_n_hyp = ints + B; st.done = ints + 2 * B; st.has_final = ints + 3 * B; st.n_nodes = ints + 4 * B;
-  st.final_node = ints + 5 * B; st.final_u = ints + 6 * B;
-  double* dbl = reinterpret_cast<double*>(take(static_cast<size_t>(B) * 8 * 2));
+  for (AlsdBeam* m : {&st.cur, &st.nx}) {
+    m->score = static_cast<double*>(take(R * 8)); m->hash = static_cast<unsigned long long*>(take(R * 8));
+    m->u = static_cast<int*>(take(R * 4)); m->node = static_cast<int*>(take(R * 4));
+    m->h = static_cast<float*>(take(R * Hp * 4)); m->c = static_cast<float*>(take(R * Hp * 4)); m->pp = static_cast<float*>(take(R * Hj * 4));
+    m->n_hyp = static_cast<int*>(take(static_cast<size_t>(B) * 4));
+  }
+  st.nx_parent = static_cast<int*>(take(R * 4)); st.nx_tok = static_cast<int*>(take(R * 4)); st.row_t = static_cast<int*>(take(R * 4));
+  st.cand_logp = static_cast<float*>(take(R * (kMaxBeam + 1) * 4)); st.cand_tok = static_cast<int*>(take(R * kMaxBeam * 4));
+  int* ints = static_cast<int*>(take(static_cast<size_t>(B) * 4 * 5));
+  st.done = ints; st.has_final = ints + B; st.n_nodes = ints + 2 * B; st.final_node = ints + 3 * B; st.final_u = ints + 4 * B;
+  double* dbl = static_cast<double*>(take(static_cast<size_t>(B) * 8 * 2));
   st.final_key = dbl; st.final_score = dbl + B;
-  int* tree = reinterpret_cast<int*>(take(static_cast<size_t>(B) * max_nodes * 4 * 3));
+  int* tree = static_cast<int*>(take(static_cast<size_t>(B) * max_nodes * 4 * 3));
   st.node_parent = tree; st.node_tok = tree + static_cast<size_t>(B) * max_nodes; st.node_step = tree + 2 * static_cast<size_t>(B) * max_nodes;
-  st.n_done = reinterpret_cast<int*>(take(256));
+  st.n_done = static_cast<int*>(take(4));
 }
 
 cudaError_t alsd_launch_init(const AlsdState& st, int B, int blank, cudaStream_t s) {
@@ -417,8 +381,8 @@ cudaError_t alsd_launch_reduce(const AlsdState& st, int B, const float* logits, 
   alsd_reduce_kernel<<<B * st.beam, 256, 0, s>>>(st, logits, ld, V);
   return cudaGetLastError();
 }
-cudaError_t alsd_launch_select(const AlsdState& st, int B, const int32_t* enc_len, int step, int blank, float u_max_ratio, bool recombine_returns_input, cudaStream_t s) {
-  alsd_select_kernel<<<B, 32, 0, s>>>(st, enc_len, step, blank, u_max_ratio, recombine_returns_input ? 1 : 0);
+cudaError_t alsd_launch_select(const AlsdState& st, int B, const int32_t* enc_len, int step, float u_max_ratio, bool recombine_returns_input, cudaStream_t s) {
+  alsd_select_kernel<<<B, 32, 0, s>>>(st, enc_len, step, u_max_ratio, recombine_returns_input ? 1 : 0);
   return cudaGetLastError();
 }
 cudaError_t alsd_launch_lstm_in(const AlsdState& st, int B, const float* embed, int Hp, void* planes, cudaStream_t s) {
@@ -427,11 +391,6 @@ cudaError_t alsd_launch_lstm_in(const AlsdState& st, int B, const float* embed, 
 }
 cudaError_t alsd_launch_cell(const AlsdState& st, int B, const float* gates, int Hp, void* planes, cudaStream_t s) {
   alsd_cell_kernel<<<B * st.beam, 128, 0, s>>>(st, gates, Hp, static_cast<__nv_bfloat16*>(planes));
-  return cudaGetLastError();
-}
-cudaError_t alsd_launch_commit(const AlsdState& st, int B, const float* pp_new, int Hp, int Hj, cudaStream_t s) {
-  alsd_commit_kernel<<<B * st.beam, 128, 0, s>>>(st, pp_new, Hp, Hj, 0);
-  alsd_commit_kernel<<<B * st.beam, 128, 0, s>>>(st, pp_new, Hp, Hj, 1);
   return cudaGetLastError();
 }
 cudaError_t alsd_launch_output(const AlsdState& st, int B, int blank, int32_t* y, int32_t* steps, int32_t* n, double* score, int U_cap, cudaStream_t s) {

@@ -592,13 +592,18 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   if (cta == 0 && tid == 0) for (int i = 0; i < 12; ++i) p.prof[i] = s_prof[i];
 }
 
-// workspace: hbuf | rec | ppbuf | pad to 128 | barrier counters (kBarCounters lines) | prof (128 B) | best
-static size_t spec_counter_offset(int B, int Hj, int Hp) {
-  return (static_cast<size_t>(5) * B * Hp * 4 + static_cast<size_t>(B) * Hj * 4 + 127) & ~static_cast<size_t>(127);
-}
-size_t rnnt_spec_prof_offset(int B, int Hj, int Hp) { return spec_counter_offset(B, Hj, Hp) + static_cast<size_t>(kBarCounters) * kBarStride * 4; }
-size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp) {
-  return rnnt_spec_prof_offset(B, Hj, Hp) + 128 + static_cast<size_t>(3) * B * kFrames * 8 + 128 /*base alignment slack*/;
+// workspace (SpecDev's global buffers): hbuf | rec | ppbuf | barrier counters (kBarCounters 128-byte lines) | prof | best
+SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp) {
+  Arena a;
+  SpecWorkspace w;
+  w.hbuf = a.take(static_cast<size_t>(B) * Hp * 4);
+  w.rec = a.take(static_cast<size_t>(B) * Hp * 4 * 4);
+  w.ppbuf = a.take(static_cast<size_t>(B) * Hj * 4);
+  w.counters = a.take(static_cast<size_t>(kBarCounters) * kBarStride * 4);
+  w.prof = a.take(12 * 8);
+  w.best = a.take(static_cast<size_t>(3) * B * kFrames * 8);
+  w.total = a.off;
+  return w;
 }
 
 template <int HJ, int HP>
@@ -624,19 +629,20 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   p.tokens = a.tokens; p.frames = a.frames; p.n_tok = a.n_tok;
   if (reinterpret_cast<uintptr_t>(workspace) & 15u) return cudaErrorInvalidValue;   // the window is read with 16-byte loads
   char* ws = static_cast<char*>(workspace);
-  p.hbuf = reinterpret_cast<float*>(ws);
-  p.rec = reinterpret_cast<float*>(ws + static_cast<size_t>(a.B) * a.Hp * 4);
-  p.ppbuf = reinterpret_cast<float*>(ws + static_cast<size_t>(5) * a.B * a.Hp * 4);
-  p.counter = reinterpret_cast<unsigned int*>(ws + spec_counter_offset(a.B, a.Hj, a.Hp));
-  p.prof = reinterpret_cast<long long*>(ws + rnnt_spec_prof_offset(a.B, a.Hj, a.Hp));
-  p.best = reinterpret_cast<unsigned long long*>(ws + rnnt_spec_prof_offset(a.B, a.Hj, a.Hp) + 128);
+  const SpecWorkspace w = rnnt_spec_workspace(a.B, a.Hj, a.Hp);
+  p.hbuf = reinterpret_cast<float*>(ws + w.hbuf);
+  p.rec = reinterpret_cast<float*>(ws + w.rec);
+  p.ppbuf = reinterpret_cast<float*>(ws + w.ppbuf);
+  p.counter = reinterpret_cast<unsigned int*>(ws + w.counters);
+  p.prof = reinterpret_cast<long long*>(ws + w.prof);
+  p.best = reinterpret_cast<unsigned long long*>(ws + w.best);
   p.B = a.B; p.T_max = a.T_max; p.V = a.V; p.U_max = a.U_max; p.max_symbols = a.max_symbols;
   p.S = G / kGroups;
   p.rows_j = (a.V + 1 + p.S - 1) / p.S;
   p.units = (a.Hp + G - 1) / G;
   p.rows_p = (a.Hj + G - 1) / G;
   if (4 * p.units > 24 || p.rows_p > 8 || a.gate_tab == nullptr) return cudaErrorInvalidValue;   // the n8 tiles of phase P
-  cudaError_t e = cudaMemsetAsync(workspace, 0, rnnt_spec_workspace_bytes(a.B, a.Hj, a.Hp), stream);
+  cudaError_t e = cudaMemsetAsync(workspace, 0, w.total, stream);
   if (e != cudaSuccess) return e;
   const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + (kPassRows * kSpWarps + 12) * 8 + static_cast<size_t>(a.B) * 7 * 4 +
                        (2 + 2 * kSpWarps) * 4 + 64;

@@ -11,6 +11,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/rs_engine.h"
@@ -165,17 +166,7 @@ int drain_log(rs_engine* e, F&& visit) {
   return RS_OK;
 }
 
-size_t align_up(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-
-// Workspace layout: regions taken one after another, each starting 256-byte aligned.
-struct Arena {
-  size_t off = 0;
-  size_t take(size_t bytes) { const size_t o = off; off = align_up(off + bytes); return o; }
-};
-
-inline size_t dec_ws_bytes(const rs_engine* e, int B) {
-  return rs::rnnt_spec_workspace_bytes(B, e->cfg.joint_hidden, e->cfg.pred_hidden);
-}
+inline rs::SpecWorkspace dec_ws(const rs_engine* e, int B) { return rs::rnnt_spec_workspace(B, e->cfg.joint_hidden, e->cfg.pred_hidden); }
 
 Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
   const rs_model_config& c = e->cfg;
@@ -188,7 +179,7 @@ Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
   p.M = B * p.T3;
   const size_t C = c.sub_channels, d = c.d_model;
   const size_t wide = static_cast<size_t>(c.d_ff) > 3 * d ? c.d_ff : 3 * d;
-  Arena a;
+  rs::Arena a;
   p.wav = a.take(static_cast<size_t>(B) * L_max * 4);
   p.len = a.take(static_cast<size_t>(B) * 4);
   p.mel = a.take(static_cast<size_t>(B) * p.F_max * c.n_mels * 4);
@@ -213,7 +204,7 @@ Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
   p.tokens = a.take(static_cast<size_t>(B) * U_max * 4);
   p.frames = a.take(static_cast<size_t>(B) * U_max * 4);
   p.ntok = a.take(static_cast<size_t>(B) * 4);
-  p.dec_ws = a.take(dec_ws_bytes(e, B));
+  p.dec_ws = a.take(dec_ws(e, B).total);
   p.total = a.off;
   return p;
 }
@@ -536,10 +527,10 @@ int rs_rnnt_greedy(rs_engine* e, const float* enc, const int32_t* enc_len, int B
   Plan p{};
   // only xn / encp / dec_ws are touched: size them for M = B*T_max rows
   p.B = B; p.M = B * T_max;
-  Arena a;
+  rs::Arena a;
   p.xn = a.take(static_cast<size_t>(p.M) * e->cfg.d_model * 2);
   p.encp = a.take(static_cast<size_t>(p.M) * e->cfg.joint_hidden * 4);
-  p.dec_ws = a.take(dec_ws_bytes(e, B));
+  p.dec_ws = a.take(dec_ws(e, B).total);
   p.total = a.off;
   RS_TRY(check_ws(e, p));
   return do_greedy(e, p, enc, enc_len, T_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
@@ -672,15 +663,17 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
   const int M = B * T_max, R = B * beam;
   const int total_steps = T_max + static_cast<int>(u_max_ratio * static_cast<float>(T_max));
   const int max_nodes = 1 + beam * (total_steps + 1);
-  // ---- workspace
-  Arena a;
+  // ---- workspace: scratch, then the search state, laid out once to size it and once more to bind it
+  rs::Arena a;
   const size_t o_xn = a.take(static_cast<size_t>(M) * d * 2), o_encp = a.take(static_cast<size_t>(M) * Hj * 4);
   const size_t plane_cols = static_cast<size_t>(3 * Hj > 6 * Hp ? 3 * Hj : 6 * Hp);
   const size_t o_planes = a.take(static_cast<size_t>(R) * plane_cols * 2), o_logits = a.take(static_cast<size_t>(R) * n_pad * 4);
-  const size_t o_gates = a.take(static_cast<size_t>(R) * 4 * Hp * 4), o_pp = a.take(static_cast<size_t>(R) * Hj * 4);
-  const size_t state_bytes = rs::alsd_state_bytes(B, beam, Hp, Hj, max_nodes);
-  const size_t o_state = a.take(state_bytes);
-  const size_t need_bytes = a.off;
+  const size_t o_gates = a.take(static_cast<size_t>(R) * 4 * Hp * 4);
+  const size_t o_state = a.off;
+  rs::AlsdState st{};
+  rs::Arena state_plan = a;
+  rs::alsd_layout_state(st, state_plan, nullptr, B, beam, Hp, Hj, max_nodes, score_norm != 0);
+  const size_t need_bytes = state_plan.off;
   if (need_bytes > e->alsd_ws_bytes) {
     RS_CUDA(e, cudaStreamSynchronize(s));
     cudaFree(e->alsd_ws); e->alsd_ws = nullptr; e->alsd_ws_bytes = 0;
@@ -690,20 +683,19 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
   if (e->alsd_done_host == nullptr) RS_CUDA(e, cudaMallocHost(reinterpret_cast<void**>(&e->alsd_done_host), sizeof(int)));
   char* ws = static_cast<char*>(e->alsd_ws);
   void* xn = ws + o_xn; float* encp = reinterpret_cast<float*>(ws + o_encp); void* planes = ws + o_planes;
-  float* logits = reinterpret_cast<float*>(ws + o_logits); float* gates = reinterpret_cast<float*>(ws + o_gates); float* ppn = reinterpret_cast<float*>(ws + o_pp);
-  RS_CUDA(e, cudaMemsetAsync(ws + o_state, 0, state_bytes, s));
-  rs::AlsdState st{};
-  rs::alsd_bind_state(st, ws + o_state, B, beam, Hp, Hj, max_nodes, score_norm != 0);
+  float* logits = reinterpret_cast<float*>(ws + o_logits); float* gates = reinterpret_cast<float*>(ws + o_gates);
+  RS_CUDA(e, cudaMemsetAsync(ws + o_state, 0, need_bytes - o_state, s));
+  rs::alsd_layout_state(st, a, ws, B, beam, Hp, Hj, max_nodes, score_norm != 0);
   // ---- joint.enc over every frame (as in the greedy path)
   RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, xn, static_cast<int64_t>(M) * d, s));
   RS_TRY(gemm(e, {xn, e->dec.enc_w, e->dec.enc_b, nullptr, encp, M, Hj, d, RS_EPI_BIAS_F32, 1.f}, s));
-  // predictor of the extended hypotheses of the beam being built (also the start: [blank] from the zero state)
+  // predictor of the beam being built (also the start: [blank] from the zero state), which then becomes the current one
   auto predictor = [&]() -> int {
     RS_LAUNCH(e, s, 1, rs::alsd_launch_lstm_in(st, B, e->dec.embed, Hp, planes, s));
     RS_TRY(gemm(e, {planes, e->alsd.lstm_w3, e->dec.lstm_b, nullptr, gates, R, 4 * Hp, 6 * Hp, RS_EPI_BIAS_F32, 1.f}, s));
     RS_LAUNCH(e, s, 1, rs::alsd_launch_cell(st, B, gates, Hp, planes, s));
-    RS_TRY(gemm(e, {planes, e->alsd.pred_w3, e->dec.pred_b, nullptr, ppn, R, Hj, 3 * Hp, RS_EPI_BIAS_F32, 1.f}, s));
-    RS_LAUNCH(e, s, 2, rs::alsd_launch_commit(st, B, ppn, Hp, Hj, s));
+    RS_TRY(gemm(e, {planes, e->alsd.pred_w3, e->dec.pred_b, nullptr, st.nx.pp, R, Hj, 3 * Hp, RS_EPI_BIAS_F32, 1.f}, s));
+    std::swap(st.cur, st.nx);
     return RS_OK;
   };
   RS_LAUNCH(e, s, 1, rs::alsd_launch_init(st, B, blank, s));
@@ -712,7 +704,7 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
     RS_LAUNCH(e, s, 1, rs::alsd_launch_rows(st, B, encp, enc_len, T_max, Hj, step, planes, s));
     RS_TRY(gemm(e, {planes, e->alsd.out_w3, e->alsd.out_b, nullptr, logits, R, n_pad, 3 * Hj, RS_EPI_BIAS_F32, 1.f}, s));
     RS_LAUNCH(e, s, 1, rs::alsd_launch_reduce(st, B, logits, n_pad, V, s));
-    RS_LAUNCH(e, s, 1, rs::alsd_launch_select(st, B, enc_len, step, blank, u_max_ratio, recombine_returns_input != 0, s));
+    RS_LAUNCH(e, s, 1, rs::alsd_launch_select(st, B, enc_len, step, u_max_ratio, recombine_returns_input != 0, s));
     RS_TRY(predictor());
     if ((step & 31) == 31) {
       RS_CUDA(e, cudaMemcpyAsync(e->alsd_done_host, st.n_done, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -771,14 +763,15 @@ int rs_stage_times_ms(const rs_engine* e, float* ms) {
   return RS_OK;
 }
 
-// Debug: cycle counters of the batched decode kernel's CTA 0 from the last rs_transcribe_* call for (B, L_max):
-// phase J, barrier, token reduce, phase L, barrier, phase P, barrier, iterations.  Synchronises the device.
-int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* out8) {
-  if (!e || !out8) return RS_ERR_INVALID_ARG;
+// Debug: the 12 cycle counters of the batched decode kernel's CTA 0 from the last rs_transcribe_* call for (B, L_max):
+// phase J, barrier, token reduce, phase L, barrier, phase P, barrier, iterations, three sub-timers of phase J, one unused slot.
+// Synchronises the device.
+int rs_debug_decode_cycles(rs_engine* e, int B, int L_max, int U_max, int64_t* out12) {
+  if (!e || !out12) return RS_ERR_INVALID_ARG;
   Plan p = make_plan(e, B, L_max, U_max);
   RS_CUDA(e, cudaDeviceSynchronize());
-  const size_t off = p.dec_ws + rs::rnnt_spec_prof_offset(B, e->cfg.joint_hidden, e->cfg.pred_hidden);
-  RS_CUDA(e, cudaMemcpy(out8, static_cast<char*>(e->ws) + off, 96, cudaMemcpyDeviceToHost));
+  const size_t off = p.dec_ws + dec_ws(e, B).prof;
+  RS_CUDA(e, cudaMemcpy(out12, static_cast<char*>(e->ws) + off, 12 * sizeof(int64_t), cudaMemcpyDeviceToHost));
   return RS_OK;
 }
 

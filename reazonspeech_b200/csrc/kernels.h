@@ -6,6 +6,12 @@
 
 namespace rs {
 
+// Memory layout: regions taken one after another, each starting 256-byte aligned (offsets from a 256-byte-aligned base).
+struct Arena {
+  size_t off = 0;
+  size_t take(size_t bytes) { const size_t o = off; off = (off + bytes + 255) & ~static_cast<size_t>(255); return o; }
+};
+
 // out = epi(A[M,K] * W[N,K]^T); the output row pitch is N (N / 2 for RS_EPI_BIAS_GLU_BF16)
 struct GemmArgs {
   const void* a;       // bf16 [M,K] row-major
@@ -75,9 +81,10 @@ struct DecodeArgs {
   int32_t* tokens; int32_t* frames; int32_t* n_tok;
   int B, T_max, Hj, Hp, V, U_max, max_symbols;
 };
-// windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace from rnnt_spec_workspace_bytes()
-size_t rnnt_spec_workspace_bytes(int B, int Hj, int Hp);
-size_t rnnt_spec_prof_offset(int B, int Hj, int Hp);        // where the kernel's 12 cycle counters sit inside that workspace
+// Byte offsets of the decode workspace's regions and its size (decode_spec.cu describes the regions)
+struct SpecWorkspace { size_t hbuf, rec, ppbuf, counters, prof, best, total; };
+SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp);
+// windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace laid out by rnnt_spec_workspace()
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream);
 
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)

@@ -27,18 +27,29 @@ def _encode(eng, waves):
     return eng.encode(mel, mel_len)
 
 
-@pytest.mark.parametrize("beam,returns_input,score_norm", [(1, True, True), (2, True, True), (4, True, True), (4, False, True), (4, True, False), (8, True, True)])
-def test_alsd_matches_the_oracle(alsd_engine, tiny_cfg, tiny_sd, beam, returns_input, score_norm):
+# u_max_ratio < 2 ends most searches before any hypothesis finishes, so the winner comes from the last beam; the batch mixes
+# lengths, so utterances end on steps of both parities and the beam is read from either half of the engine's double buffer
+_CASES = [(1, True, True, 2.0), (2, True, True, 2.0), (4, True, True, 2.0), (4, False, True, 2.0), (4, True, False, 2.0), (8, True, True, 2.0),
+          (4, True, True, 0.0), (4, True, True, 0.3)]
+
+
+@pytest.mark.parametrize("beam,returns_input,score_norm,u_max_ratio", _CASES,
+                         ids=[f"{b}-{r}-{s}" + ("" if u == 2.0 else f"-{u}") for b, r, s, u in _CASES])
+def test_alsd_matches_the_oracle(alsd_engine, tiny_cfg, tiny_sd, beam, returns_input, score_norm, u_max_ratio):
     from oracle.alsd_restated import alsd_beam
     eng = alsd_engine
     waves = [np.pad(synth_clip(200 + i, s), 8000) for i, s in enumerate((2.0, 3.3, 0.9, 2.6, 1.4))]
     enc, enc_len = _encode(eng, waves)
-    y, steps, n, score = [a.cpu() for a in eng.alsd(enc, enc_len, beam=beam, recombine_returns_input=returns_input, score_norm=score_norm)]
+    y, steps, n, score = [a.cpu() for a in eng.alsd(enc, enc_len, beam=beam, u_max_ratio=u_max_ratio, recombine_returns_input=returns_input,
+                                                    score_norm=score_norm)]
     enc = enc.cpu()
     same = 0
+    from_last_beam = 0
     for i in range(len(waves)):
         T = int(enc_len[i])
-        ref = alsd_beam(enc[i, :T], tiny_sd, tiny_cfg, beam=beam, recombine_returns_input=returns_input, score_norm=score_norm, emulate=True)
+        ref = alsd_beam(enc[i, :T], tiny_sd, tiny_cfg, beam=beam, u_max_ratio=u_max_ratio, recombine_returns_input=returns_input,
+                        score_norm=score_norm, emulate=True)
+        from_last_beam += not ref.from_final
         k = int(n[i])
         got_y, got_steps = y[i, : k + 1].tolist(), steps[i, :k].tolist()
         print(f"beam {beam} utt{i}: T={T}, {k} tokens (oracle {len(ref.tokens)}), score {float(score[i]):.4f} (oracle {ref.score:.4f})")
@@ -50,6 +61,8 @@ def test_alsd_matches_the_oracle(alsd_engine, tiny_cfg, tiny_sd, beam, returns_i
             assert abs(key(float(score[i]), k + 1) - key(ref.score, len(ref.y_sequence))) < 1e-3, (got_y[:12], ref.y_sequence[:12])
         assert got_y[0] == tiny_cfg.blank and all(0 <= s - j < T for j, s in enumerate(got_steps))     # frame = step - tokens before it
     assert same >= len(waves) - 1
+    if u_max_ratio < 2.0:
+        assert from_last_beam >= 1
 
 
 def test_alsd_beam_one_equals_the_greedy_kernel_where_the_cap_does_not_bind(alsd_engine, tiny_cfg):

@@ -1,5 +1,5 @@
 """The engine's measurement aids on one step of the tiny model: the launch counter, the per-kernel and GEMM event logs, and
-the stage events of the host-buffer path."""
+the stage events of the host-buffer path; the launch count of an ALSD beam search."""
 import pytest
 import torch
 
@@ -38,6 +38,26 @@ def test_launch_count_per_step(engine, tiny_cfg):
     engine.transcribe_device(wav, lens)
     a = 2 if tiny_cfg.global_tokens > 0 else 1          # the global-token row kernel follows the local attention
     assert engine.launch_count - n0 == 13 + tiny_cfg.n_layers * (13 + a)
+
+
+def test_launch_count_of_alsd(tiny_cfg, tiny_sd):
+    """Eight launches per anti-diagonal step (rows, GEMM, reduce, select, lstm_in, GEMM, cell, GEMM) and eight around them
+    (f32 -> bf16, joint.enc GEMM, init, the first predictor pass, output)."""
+    from reazonspeech_b200.engine import Engine
+    eng = Engine(tiny_cfg, tiny_sd, "cuda:0", alsd=True)
+    wav, lens = _batch(B)
+    mel, mel_len = eng.log_mel(wav.cuda(), lens.cuda())
+    enc, enc_len = eng.encode(mel, mel_len)
+    eng.alsd(enc, enc_len, beam=4)                      # loads every kernel
+    torch.cuda.synchronize()
+    eng.kernel_timing(True)
+    n0 = eng.launch_count
+    eng.alsd(enc, enc_len, beam=4)
+    kt = eng.kernel_timing()
+    eng.kernel_timing(False)
+    steps = kt["alsd_launch_rows"][0]
+    assert steps > 0
+    assert eng.launch_count - n0 == 8 + 8 * steps
 
 
 def test_kernel_timing_of_one_step(engine, tiny_cfg):
