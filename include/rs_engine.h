@@ -137,6 +137,24 @@ int rs_transcribe_batch_pcm16(rs_engine* e, const int16_t* wav_host, const int32
                               int L_max, int32_t* tokens_host, int32_t* frames_host,
                               int32_t* n_tok_host, int U_max, void* stream);
 
+/* Confidence statistics of the greedy decode (what NeMo's ConfidenceConfig turns into token / word confidence): the three
+ * calls above plus `alpha` (> 0, finite; RS_ERR_INVALID_ARG otherwise) and `stats` f32 [B, U_max, 4].  For every stored
+ * token n of utterance b, stats[b][n] = (lp, H1, A, G) of the softmax p over all vocab_size + 1 classes (blank included) of
+ * the joint evaluation that emitted it: lp = log p of the emitted (argmax) token, H1 = sum p log p, A = sum p^alpha,
+ * G = sum p^alpha log p.  Every confidence measure NeMo defines is a function of these four numbers and the class count
+ * (reazonspeech_b200/confidence.py).  Blank decisions and tokens at or beyond U_max store nothing.  Tokens, frames and n_tok
+ * are exactly those of the calls without statistics.  wav_is_pcm16: the samples are int16 PCM (as in the _pcm16 calls).
+ * rs_transcribe_batch_confidence synchronises; its statistics are copied back with the tokens. */
+int rs_rnnt_greedy_confidence(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B,
+                              int T_max, int32_t* tokens_dev, int32_t* frames_dev, int32_t* n_tok_dev,
+                              int U_max, float alpha, float* stats_dev, void* stream);
+int rs_transcribe_device_confidence(rs_engine* e, const void* wav_dev, int wav_is_pcm16, const int32_t* len_dev,
+                                    int B, int L_max, int32_t* tokens_dev, int32_t* frames_dev,
+                                    int32_t* n_tok_dev, int U_max, float alpha, float* stats_dev, void* stream);
+int rs_transcribe_batch_confidence(rs_engine* e, const void* wav_host, int wav_is_pcm16, const int32_t* len_host,
+                                   int B, int L_max, int32_t* tokens_host, int32_t* frames_host,
+                                   int32_t* n_tok_host, int U_max, float alpha, float* stats_host, void* stream);
+
 /* ALSD beam search (NeMo BeamRNNTInfer.align_length_sync_decoding, the shipped checkpoint's default strategy; the reference's
  * decode.py is written for its hypotheses, pkg/nemo-asr/src/decode.py:29,38-40,48): enc f32[B,T_max,d_model] + enc_len ->
  * y i32[B, U_cap + 1] (leading blank, then the tokens), step i32[B, U_cap] (alignment step t + u of every token =

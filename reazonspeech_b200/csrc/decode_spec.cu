@@ -29,6 +29,12 @@
 //   barrier
 //   phase P  utterances that emitted: pred_proj rows and rec = W_hh . h of the CTA from the new h
 //   barrier
+//
+// Confidence (kConf = true; the decisions never depend on it).  Phase J also reduces, over the same fp32 logits l of the CTA's
+// vocabulary slice, one softmax tuple per (utterance, frame): m = max l, s = sum e^(l-m), g = sum e^(l-m) (l-m),
+// a = sum e^(alpha (l-m)), ga = sum e^(alpha (l-m)) (l-m), and stores it in the conf ring (one slot per slice).  After the
+// consume step every emission below U_max is merged over the S slices by one warp (emission e: CTA e % G) into
+// stats[b][n] = (log p of the emitted token, sum p log p, sum p^alpha, sum p^alpha log p) over all V + 1 classes.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -52,9 +58,33 @@ struct SpecDev {
   float* ppbuf;               // [B][Hj]
   unsigned int* counter;      // grid barrier: kBarCounters arrival counters, one per 128-byte line
   long long* prof;            // [12] cycle counters of CTA 0
+  float* conf;                // [3][B][kFrames][S][5] softmax tuples of each vocabulary slice, 3-deep ring like best (kConf)
+  float* stats;               // [B][U_max][4] (lp, H1, A_alpha, G_alpha) of every stored token (kConf)
+  float alpha, alpha_l2;      // alpha and alpha * log2(e) (kConf)
   int B, T_max, V, U_max, max_symbols;
   int S, rows_j, units, rows_p;
 };
+
+// Softmax statistics of a set of logits relative to its maximum m (an empty set: m = -inf, all sums zero):
+// s = sum e^(l-m), g = sum e^(l-m) (l-m), a = sum e^(alpha (l-m)), ga = sum e^(alpha (l-m)) (l-m).
+struct SoftStat { float m, s, g, a, ga; };
+constexpr float kLog2e = 1.4426950408889634f;
+__device__ __forceinline__ SoftStat soft_one(float l) { return {l, 1.f, 0.f, 1.f, 0.f}; }
+__device__ __forceinline__ SoftStat soft_empty() { return {-INFINITY, 0.f, 0.f, 0.f, 0.f}; }
+// union of two disjoint sets: the smaller-maximum side is rescaled by e^d (resp. e^(alpha d)), d = its m - the larger m
+__device__ __forceinline__ SoftStat soft_merge(SoftStat x, SoftStat y, float alpha_l2) {
+  if (y.m > x.m) { const SoftStat t = x; x = y; y = t; }
+  if (y.m == -INFINITY) return x;
+  const float d = y.m - x.m;
+  const float r = exp2f(d * kLog2e), ra = exp2f(d * alpha_l2);
+  x.s += r * y.s; x.g += r * (y.g + y.s * d);
+  x.a += ra * y.a; x.ga += ra * (y.ga + y.a * d);
+  return x;
+}
+__device__ __forceinline__ SoftStat soft_shfl_xor(const SoftStat& x, int o) {
+  return {__shfl_xor_sync(0xffffffffu, x.m, o), __shfl_xor_sync(0xffffffffu, x.s, o), __shfl_xor_sync(0xffffffffu, x.g, o),
+          __shfl_xor_sync(0xffffffffu, x.a, o), __shfl_xor_sync(0xffffffffu, x.ga, o)};
+}
 
 // Grid barrier over kBarCounters arrival counters, each in its own 128-byte line: CTA i arrives on counter i % kBarCounters,
 // threads 0..kBarCounters-1 each poll one counter.  Arrivals of every CTA on ONE address are serialised by the L2 slice that
@@ -127,7 +157,7 @@ __device__ __forceinline__ unsigned long long pack_best(float v, int row) {
 // is one m64n64k16 per warpgroup and the two halves of D are added in the epilogue.
 static_assert(kSpThreads == 256, "the joint is issued by two warpgroups");
 
-template <int HJ, int HP>
+template <int HJ, int HP, bool kConf>
 __global__ void __launch_bounds__(kSpThreads, 1)
 rnnt_greedy_spec_kernel(const SpecDev p) {
   constexpr int KH = HJ / 2;                 // joint k-half staged in shared memory at a time
@@ -182,6 +212,8 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   int* s_emit = s_tok + B; int* s_len = s_emit + B;
   int* s_act = s_len + B;                                                            // ordered list of the utterances with frames left
   int* s_cnt = s_act + B;                                                            // [0] n_emit, [1] n_active, [2..2+8) warp counts x2
+  int* s_cj = s_cnt + 2 + 2 * kSpWarps;                                              // kConf: window frame of b's stored emission, -1: none
+  float* s_conf = reinterpret_cast<float*>(s_cj + B);                                // kConf: [32 rows][kSpWarps][5] per-warp softmax tuples
 
   {
     const uint32_t zero = 0;
@@ -518,12 +550,22 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
             for (int j = 0; j < 4; ++j) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                unsigned long long k0 = v0 ? pack_best((dj[4 * j + e] + dj[4 * (j + 4) + e]) + bias0, j0 + rr) : 0ull;
-                const unsigned long long k1 = v1 ? pack_best((dj[4 * j + 2 + e] + dj[4 * (j + 4) + 2 + e]) + bias1, j0 + rr + 8) : 0ull;
+                const float l0 = (dj[4 * j + e] + dj[4 * (j + 4) + e]) + bias0, l1 = (dj[4 * j + 2 + e] + dj[4 * (j + 4) + 2 + e]) + bias1;
+                unsigned long long k0 = v0 ? pack_best(l0, j0 + rr) : 0ull;
+                const unsigned long long k1 = v1 ? pack_best(l1, j0 + rr + 8) : 0ull;
                 k0 = k1 > k0 ? k1 : k0;                       // higher logit first, ties -> lower row
 #pragma unroll
                 for (int o = 4; o < 32; o <<= 1) { const unsigned long long ot = __shfl_xor_sync(0xffffffffu, k0, o); k0 = ot > k0 ? ot : k0; }
                 if (gid == 0) s_best[(8 * j + 2 * tig + e) * kSpWarps + warp] = k0;
+                if constexpr (kConf) {                        // the same logits and lanes -> the warp's softmax tuple of the column
+                  SoftStat c = soft_merge(v0 ? soft_one(l0) : soft_empty(), v1 ? soft_one(l1) : soft_empty(), p.alpha_l2);
+#pragma unroll
+                  for (int o = 4; o < 32; o <<= 1) c = soft_merge(c, soft_shfl_xor(c, o), p.alpha_l2);
+                  if (gid == 0) {
+                    float* d = s_conf + ((8 * j + 2 * tig + e) * kSpWarps + warp) * 5;
+                    d[0] = c.m; d[1] = c.s; d[2] = c.g; d[3] = c.a; d[4] = c.ga;
+                  }
+                }
               }
             }
           }
@@ -534,9 +576,17 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
 #pragma unroll
           for (int q = 1; q < kSpWarps; ++q) { const unsigned long long o = s_best[lane * kSpWarps + q]; m = o > m ? o : m; }
           asm volatile("red.relaxed.gpu.global.max.u64 [%0], %1;" ::"l"(p.best + (static_cast<size_t>(iter % 3) * B + row_b) * kFrames + (lane % kFrames)), "l"(m) : "memory");
+          if constexpr (kConf) {                              // the slice's tuple: a plain store into the slot it owns
+            const float* sc = s_conf + lane * kSpWarps * 5;
+            SoftStat c = {sc[0], sc[1], sc[2], sc[3], sc[4]};
+#pragma unroll
+            for (int q = 1; q < kSpWarps; ++q) c = soft_merge(c, {sc[5 * q], sc[5 * q + 1], sc[5 * q + 2], sc[5 * q + 3], sc[5 * q + 4]}, p.alpha_l2);
+            float* d = p.conf + ((((static_cast<size_t>(iter % 3) * B + row_b) * kFrames + (lane % kFrames)) * p.S) + slice) * 5;
+            __stcg(d, c.m); __stcg(d + 1, c.s); __stcg(d + 2, c.g); __stcg(d + 3, c.a); __stcg(d + 4, c.ga);
+          }
         }
         jtick(10);
-        // s_best / s_g are rewritten only after the next pass's first __syncthreads pair; the reads above are by warp 0
+        // s_best / s_conf / s_g are rewritten only after the next pass's first __syncthreads pair; the reads above are by warp 0
         // before it reaches that barrier
       }
     }
@@ -547,7 +597,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     for (int b = tid; b < B; b += kSpThreads) {
       int t = s_t[b];
       const int len = s_len[b];
-      int tok = -1;
+      int tok = -1, cj = -1;
       if (t < len) {
         const int nv = min(kFrames, len - t);
         int sym = s_sym[b];
@@ -566,6 +616,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
             p.tokens[static_cast<size_t>(b) * p.U_max + n] = k;
             p.frames[static_cast<size_t>(b) * p.U_max + n] = t;
           }
+          if (kConf && n < p.U_max) cj = j;
           s_n[b] = n + 1;
           tok = k;
           if (++sym >= p.max_symbols) { t += 1; sym = 0; }
@@ -574,6 +625,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
         s_t[b] = t; s_sym[b] = sym;
       }
       s_tok[b] = tok;
+      if constexpr (kConf) s_cj[b] = cj;
     }
     // the slot that iteration iter+2 will use was last read two barriers ago: clear it now (visible through the
     // next barrier, which precedes that iteration's red.max)
@@ -585,6 +637,26 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     tick(2, tk);
     if (cta == 0 && tid == 0) s_prof[7] += 1;
     if (has_j) fetch_enc(0);                      // the next window's enc_proj rows, in flight under phases L and P
+    if constexpr (kConf) {
+      // statistics of the emissions just consumed: emission e (in s_emit order) is merged by warp e / G of CTA e % G, lane
+      // i taking slices i, i + 32, ...; the slot was written before the barrier that preceded the consume step
+      const int n_emit = s_cnt[0], slot = (iter + 2) % 3;
+      for (int e = cta + G * warp; e < n_emit; e += G * kSpWarps) {
+        const int b = s_emit[e], j = s_cj[b];
+        if (j < 0) continue;                                  // beyond U_max: nothing is stored
+        const float* src = p.conf + ((static_cast<size_t>(slot) * B + b) * kFrames + j) * p.S * 5;
+        SoftStat c = soft_empty();
+        for (int s = lane; s < p.S; s += 32)
+          c = soft_merge(c, {__ldcg(src + 5 * s), __ldcg(src + 5 * s + 1), __ldcg(src + 5 * s + 2), __ldcg(src + 5 * s + 3), __ldcg(src + 5 * s + 4)}, p.alpha_l2);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) c = soft_merge(c, soft_shfl_xor(c, o), p.alpha_l2);
+        if (lane == 0) {                                      // c is relative to the argmax logit: log p = (l - m) - log s
+          const float log_s = logf(c.s), inv_s = 1.f / c.s, s_ma = expf(-p.alpha * log_s), a_alpha = s_ma * c.a;
+          const float4 st = make_float4(-log_s, c.g * inv_s - log_s, a_alpha, s_ma * c.ga - log_s * a_alpha);
+          __stcg(reinterpret_cast<float4*>(p.stats + (static_cast<size_t>(b) * p.U_max + (s_n[b] - 1)) * 4), st);
+        }
+      }
+    }
     if (s_cnt[0] > 0) lstm_and_pred();
     if (n_active == 0) break;
   }
@@ -592,8 +664,9 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   if (cta == 0 && tid == 0) for (int i = 0; i < 12; ++i) p.prof[i] = s_prof[i];
 }
 
-// workspace (SpecDev's global buffers): hbuf | rec | ppbuf | barrier counters (kBarCounters 128-byte lines) | prof | best
-SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp) {
+// workspace (SpecDev's global buffers): hbuf | rec | ppbuf | barrier counters (kBarCounters 128-byte lines) | prof | best | conf.
+// Everything before conf is zeroed by the launch; every conf slot that is read was written first.
+SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms) {
   Arena a;
   SpecWorkspace w;
   w.hbuf = a.take(static_cast<size_t>(B) * Hp * 4);
@@ -602,20 +675,26 @@ SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp) {
   w.counters = a.take(static_cast<size_t>(kBarCounters) * kBarStride * 4);
   w.prof = a.take(12 * 8);
   w.best = a.take(static_cast<size_t>(3) * B * kFrames * 8);
+  w.conf = a.take(static_cast<size_t>(3) * B * kFrames * (num_sms / kGroups) * 5 * 4);
   w.total = a.off;
   return w;
 }
 
-template <int HJ, int HP>
+template <int HJ, int HP, bool kConf>
 static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
-  cudaError_t e = cudaFuncSetAttribute(rnnt_greedy_spec_kernel<HJ, HP>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  cudaError_t e = cudaFuncSetAttribute(rnnt_greedy_spec_kernel<HJ, HP, kConf>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   int per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnnt_greedy_spec_kernel<HJ, HP>, kSpThreads, smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnnt_greedy_spec_kernel<HJ, HP, kConf>, kSpThreads, smem);
   if (e != cudaSuccess) return e;
   if (per_sm < 1) return cudaErrorLaunchOutOfResources;
   void* args[] = {&p};
-  return cudaLaunchCooperativeKernel(reinterpret_cast<void*>(rnnt_greedy_spec_kernel<HJ, HP>), dim3(grid), dim3(kSpThreads), args, smem, stream);
+  return cudaLaunchCooperativeKernel(reinterpret_cast<void*>(rnnt_greedy_spec_kernel<HJ, HP, kConf>), dim3(grid), dim3(kSpThreads), args, smem, stream);
+}
+
+template <int HJ, int HP>
+static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
+  return p.stats != nullptr ? launch_sp<HJ, HP, true>(p, grid, smem, stream) : launch_sp<HJ, HP, false>(p, grid, smem, stream);
 }
 
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream) {
@@ -629,23 +708,28 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   p.tokens = a.tokens; p.frames = a.frames; p.n_tok = a.n_tok;
   if (reinterpret_cast<uintptr_t>(workspace) & 15u) return cudaErrorInvalidValue;   // the window is read with 16-byte loads
   char* ws = static_cast<char*>(workspace);
-  const SpecWorkspace w = rnnt_spec_workspace(a.B, a.Hj, a.Hp);
+  const SpecWorkspace w = rnnt_spec_workspace(a.B, a.Hj, a.Hp, num_sms);
   p.hbuf = reinterpret_cast<float*>(ws + w.hbuf);
   p.rec = reinterpret_cast<float*>(ws + w.rec);
   p.ppbuf = reinterpret_cast<float*>(ws + w.ppbuf);
   p.counter = reinterpret_cast<unsigned int*>(ws + w.counters);
   p.prof = reinterpret_cast<long long*>(ws + w.prof);
   p.best = reinterpret_cast<unsigned long long*>(ws + w.best);
+  p.conf = reinterpret_cast<float*>(ws + w.conf);
+  p.stats = a.stats;
+  if (a.stats != nullptr && !(a.alpha > 0.f && a.alpha < INFINITY)) return cudaErrorInvalidValue;
+  p.alpha = a.alpha; p.alpha_l2 = a.alpha * kLog2e;
   p.B = a.B; p.T_max = a.T_max; p.V = a.V; p.U_max = a.U_max; p.max_symbols = a.max_symbols;
   p.S = G / kGroups;
   p.rows_j = (a.V + 1 + p.S - 1) / p.S;
   p.units = (a.Hp + G - 1) / G;
   p.rows_p = (a.Hj + G - 1) / G;
   if (4 * p.units > 24 || p.rows_p > 8 || a.gate_tab == nullptr) return cudaErrorInvalidValue;   // the n8 tiles of phase P
-  cudaError_t e = cudaMemsetAsync(workspace, 0, w.total, stream);
+  cudaError_t e = cudaMemsetAsync(workspace, 0, w.conf, stream);
   if (e != cudaSuccess) return e;
   const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + (kPassRows * kSpWarps + 12) * 8 + static_cast<size_t>(a.B) * 7 * 4 +
-                       (2 + 2 * kSpWarps) * 4 + 64;
+                       (2 + 2 * kSpWarps) * 4 + 64 +
+                       (a.stats != nullptr ? static_cast<size_t>(a.B) * 4 + kPassRows * kSpWarps * 5 * 4 : 0);   // kConf: s_cj, s_conf
   const size_t w_lp = (static_cast<size_t>(4 * p.units) * (a.Hp + 8) + static_cast<size_t>(p.rows_p) * (a.Hp + 8)) * 2;
   if (p.rows_j > 128) return cudaErrorInvalidValue;
   const size_t rows_a8 = (p.rows_j + 7) & ~7;

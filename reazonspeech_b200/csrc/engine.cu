@@ -50,7 +50,7 @@ struct Plan {           // workspace offsets (bytes) for one (B, L_max)
   int B, L_max, F_max, T1, F1, T2, F2, T3, F3, M;
   size_t wav, len, mel, mel_len, mel_part, mel_stats, enc_len, sub1, sub2, sub3, sub4, x, xn, hbuf, abuf, cbuf, vt, enc, encp;
   int n_rel_pad, ld_vt;
-  size_t tokens, frames, ntok, dec_ws, total;
+  size_t tokens, frames, ntok, stats, dec_ws, total;
 };
 
 inline int conv_len(int n) { return n > 0 ? (n - 1) / 2 + 1 : 0; }   // floor division as in NeMo's calc_length: 0 stays 0
@@ -166,7 +166,7 @@ int drain_log(rs_engine* e, F&& visit) {
   return RS_OK;
 }
 
-inline rs::SpecWorkspace dec_ws(const rs_engine* e, int B) { return rs::rnnt_spec_workspace(B, e->cfg.joint_hidden, e->cfg.pred_hidden); }
+inline rs::SpecWorkspace dec_ws(const rs_engine* e, int B) { return rs::rnnt_spec_workspace(B, e->cfg.joint_hidden, e->cfg.pred_hidden, e->num_sms); }
 
 Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
   const rs_model_config& c = e->cfg;
@@ -204,6 +204,7 @@ Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
   p.tokens = a.take(static_cast<size_t>(B) * U_max * 4);
   p.frames = a.take(static_cast<size_t>(B) * U_max * 4);
   p.ntok = a.take(static_cast<size_t>(B) * 4);
+  p.stats = a.take(static_cast<size_t>(B) * U_max * 4 * 4);                // rs_transcribe_batch_confidence's statistics
   p.dec_ws = a.take(dec_ws(e, B).total);
   p.total = a.off;
   return p;
@@ -401,8 +402,9 @@ int do_encode(rs_engine* e, const Plan& p, const int32_t* mel_len, float* enc, i
   return RS_OK;
 }
 
+// stats == nullptr: tokens only; otherwise stats f32 [B, U_max, 4] receives (lp, H1, A_alpha, G_alpha) of every stored token
 int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_len, int T_max, int32_t* tokens,
-              int32_t* frames, int32_t* ntok, int U_max, cudaStream_t s) {
+              int32_t* frames, int32_t* ntok, int U_max, float* stats, float alpha, cudaStream_t s) {
   Nvtx range("rs::rnnt_greedy (joint.enc projection + persistent decode)");
   const rs_model_config& c = e->cfg;
   const int M = p.B * T_max;
@@ -410,7 +412,8 @@ int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_
   RS_TRY(gemm(e, {at<void>(e, p.xn), e->dec.enc_w, e->dec.enc_b, nullptr, at<void>(e, p.encp), M, c.joint_hidden, c.d_model, RS_EPI_BIAS_F32, 1.f}, s));
   mark(e, 4, s);
   rs::DecodeArgs da{at<float>(e, p.encp), enc_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w, e->dec.gate_tab, e->dec.pred_w,
-                    e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, c.max_symbols};
+                    e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, c.max_symbols,
+                    stats, alpha};
   // One decode kernel for every batch size (windowed, weights-stationary, joint on wgmma: decode_spec.cu): an utterance's
   // logits are accumulated in the same order whether it is decoded alone or inside a batch, so results do not depend on
   // batch composition.
@@ -519,10 +522,16 @@ int rs_encode(rs_engine* e, const float* mel, const int32_t* mel_len, int B, int
   return do_encode(e, p, mel_len, enc, enc_len, n_layers, s);
 }
 
-int rs_rnnt_greedy(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int32_t* tokens,
-                   int32_t* frames, int32_t* n_tok, int U_max, void* stream) {
+}  // extern "C"
+
+namespace {
+
+bool alpha_ok(float alpha) { return alpha > 0.f && std::isfinite(alpha); }
+
+int rnnt_greedy(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, int32_t* tokens,
+                int32_t* frames, int32_t* n_tok, int U_max, float* stats, float alpha, cudaStream_t s) {
   if (!e || !enc || !enc_len || !tokens || !frames || !n_tok || B <= 0 || T_max <= 0 || U_max <= 0)
-    return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_greedy: bad arguments");
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
   RS_CUDA(e, cudaSetDevice(e->device));
   Plan p{};
   // only xn / encp / dec_ws are touched: size them for M = B*T_max rows
@@ -533,7 +542,23 @@ int rs_rnnt_greedy(rs_engine* e, const float* enc, const int32_t* enc_len, int B
   p.dec_ws = a.take(dec_ws(e, B).total);
   p.total = a.off;
   RS_TRY(check_ws(e, p));
-  return do_greedy(e, p, enc, enc_len, T_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
+  return do_greedy(e, p, enc, enc_len, T_max, tokens, frames, n_tok, U_max, stats, alpha, s);
+}
+
+}  // namespace
+
+extern "C" {
+
+int rs_rnnt_greedy(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int32_t* tokens,
+                   int32_t* frames, int32_t* n_tok, int U_max, void* stream) {
+  return rnnt_greedy(e, "rs_rnnt_greedy", enc, enc_len, B, T_max, tokens, frames, n_tok, U_max, nullptr, 0.f, static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_greedy_confidence(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int32_t* tokens,
+                              int32_t* frames, int32_t* n_tok, int U_max, float alpha, float* stats, void* stream) {
+  if (!stats || !alpha_ok(alpha)) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_greedy_confidence: bad arguments (stats must be set, alpha > 0 and finite)");
+  return rnnt_greedy(e, "rs_rnnt_greedy_confidence", enc, enc_len, B, T_max, tokens, frames, n_tok, U_max, stats, alpha,
+                     static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
@@ -553,7 +578,7 @@ int check_transcribe_args(rs_engine* e, const char* fn, const void* wav, const i
 // landed[c] (when not null) is recorded once chunk c's samples have been copied in.  `wav` holds f32 samples, or int16 PCM
 // (scaled by 2^-15 inside the log-mel kernel) when i16.
 int run_pipeline(rs_engine* e, const Plan& p, const void* wav, bool i16, const int32_t* len, int n_chunks, const cudaEvent_t* landed,
-                 int32_t* tokens, int32_t* frames, int32_t* n_tok, int U_max, cudaStream_t s) {
+                 int32_t* tokens, int32_t* frames, int32_t* n_tok, int U_max, float* conf_stats, float alpha, cudaStream_t s) {
   const int B = p.B, per = (B + n_chunks - 1) / n_chunks;
   const size_t row_bytes = static_cast<size_t>(p.L_max) * (i16 ? 2 : 4);
   float* mel = at<float>(e, p.mel);
@@ -570,23 +595,25 @@ int run_pipeline(rs_engine* e, const Plan& p, const void* wav, bool i16, const i
   }
   RS_TRY(do_encode(e, p, mel_len, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), -1, s));
   mark(e, 3, s);
-  RS_TRY(do_greedy(e, p, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), p.T3, tokens, frames, n_tok, U_max, s));
+  RS_TRY(do_greedy(e, p, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), p.T3, tokens, frames, n_tok, U_max, conf_stats, alpha, s));
   mark(e, 5, s);
   return RS_OK;
 }
 
 int transcribe_device(rs_engine* e, const char* fn, const void* wav, bool i16, const int32_t* len, int B, int L_max, int32_t* tokens,
-                      int32_t* frames, int32_t* n_tok, int U_max, cudaStream_t s) {
+                      int32_t* frames, int32_t* n_tok, int U_max, float* stats, float alpha, cudaStream_t s) {
   RS_TRY(check_transcribe_args(e, fn, wav, len, B, L_max, tokens, frames, n_tok, U_max));
   Plan p = make_plan(e, B, L_max, U_max);
   RS_TRY(check_ws(e, p));
-  return run_pipeline(e, p, wav, i16, len, 1, nullptr, tokens, frames, n_tok, U_max, s);
+  return run_pipeline(e, p, wav, i16, len, 1, nullptr, tokens, frames, n_tok, U_max, stats, alpha, s);
 }
 
 // Host buffers in, host buffers out (the model.transcribe seam): H2D in utterance chunks on the copy stream, overlapped with
-// the frontend of the chunks that have landed; D2H of the tokens; synchronises before returning.
+// the frontend of the chunks that have landed; D2H of the tokens (and of the statistics when stats_host is set); synchronises
+// before returning.
 int transcribe_batch(rs_engine* e, const char* fn, const void* wav_host, bool i16, const int32_t* len_host, int B, int L_max,
-                     int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, cudaStream_t s) {
+                     int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, float* stats_host, float alpha,
+                     cudaStream_t s) {
   RS_TRY(check_transcribe_args(e, fn, wav_host, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max));
   Plan p = make_plan(e, B, L_max, U_max);
   RS_TRY(check_ws(e, p));
@@ -613,10 +640,12 @@ int transcribe_batch(rs_engine* e, const char* fn, const void* wav_host, bool i1
     }
   }
   RS_TRY(run_pipeline(e, p, wav, i16, len, n_chunks, n_chunks > 1 ? e->copy_ev : nullptr, at<int32_t>(e, p.tokens),
-                      at<int32_t>(e, p.frames), at<int32_t>(e, p.ntok), U_max, s));
+                      at<int32_t>(e, p.frames), at<int32_t>(e, p.ntok), U_max, stats_host ? at<float>(e, p.stats) : nullptr, alpha, s));
   RS_CUDA(e, cudaMemcpyAsync(tokens_host, at<int32_t>(e, p.tokens), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(frames_host, at<int32_t>(e, p.frames), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(n_tok_host, at<int32_t>(e, p.ntok), static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
+  if (stats_host)
+    RS_CUDA(e, cudaMemcpyAsync(stats_host, at<float>(e, p.stats), static_cast<size_t>(B) * U_max * 4 * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaStreamSynchronize(s));
   return RS_OK;
 }
@@ -627,24 +656,40 @@ extern "C" {
 
 int rs_transcribe_device(rs_engine* e, const float* wav, const int32_t* len, int B, int L_max, int32_t* tokens,
                          int32_t* frames, int32_t* n_tok, int U_max, void* stream) {
-  return transcribe_device(e, "rs_transcribe_device", wav, false, len, B, L_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
+  return transcribe_device(e, "rs_transcribe_device", wav, false, len, B, L_max, tokens, frames, n_tok, U_max, nullptr, 0.f, static_cast<cudaStream_t>(stream));
 }
 
 int rs_transcribe_device_pcm16(rs_engine* e, const int16_t* wav, const int32_t* len, int B, int L_max, int32_t* tokens,
                                int32_t* frames, int32_t* n_tok, int U_max, void* stream) {
-  return transcribe_device(e, "rs_transcribe_device_pcm16", wav, true, len, B, L_max, tokens, frames, n_tok, U_max, static_cast<cudaStream_t>(stream));
+  return transcribe_device(e, "rs_transcribe_device_pcm16", wav, true, len, B, L_max, tokens, frames, n_tok, U_max, nullptr, 0.f,
+                           static_cast<cudaStream_t>(stream));
+}
+
+int rs_transcribe_device_confidence(rs_engine* e, const void* wav, int wav_is_pcm16, const int32_t* len, int B, int L_max, int32_t* tokens,
+                                    int32_t* frames, int32_t* n_tok, int U_max, float alpha, float* stats, void* stream) {
+  if (!stats || !alpha_ok(alpha)) return fail(e, RS_ERR_INVALID_ARG, "rs_transcribe_device_confidence: bad arguments (stats must be set, alpha > 0 and finite)");
+  return transcribe_device(e, "rs_transcribe_device_confidence", wav, wav_is_pcm16 != 0, len, B, L_max, tokens, frames, n_tok, U_max, stats, alpha,
+                           static_cast<cudaStream_t>(stream));
 }
 
 int rs_transcribe_batch(rs_engine* e, const float* wav_host, const int32_t* len_host, int B, int L_max,
                         int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, void* stream) {
   return transcribe_batch(e, "rs_transcribe_batch", wav_host, false, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max,
-                          static_cast<cudaStream_t>(stream));
+                          nullptr, 0.f, static_cast<cudaStream_t>(stream));
 }
 
 int rs_transcribe_batch_pcm16(rs_engine* e, const int16_t* wav_host, const int32_t* len_host, int B, int L_max,
                               int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, void* stream) {
   return transcribe_batch(e, "rs_transcribe_batch_pcm16", wav_host, true, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max,
-                          static_cast<cudaStream_t>(stream));
+                          nullptr, 0.f, static_cast<cudaStream_t>(stream));
+}
+
+int rs_transcribe_batch_confidence(rs_engine* e, const void* wav_host, int wav_is_pcm16, const int32_t* len_host, int B, int L_max,
+                                   int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, float alpha,
+                                   float* stats_host, void* stream) {
+  if (!stats_host || !alpha_ok(alpha)) return fail(e, RS_ERR_INVALID_ARG, "rs_transcribe_batch_confidence: bad arguments (stats must be set, alpha > 0 and finite)");
+  return transcribe_batch(e, "rs_transcribe_batch_confidence", wav_host, wav_is_pcm16 != 0, len_host, B, L_max, tokens_host, frames_host, n_tok_host,
+                          U_max, stats_host, alpha, static_cast<cudaStream_t>(stream));
 }
 
 // ALSD beam search over encoder outputs (decode_alsd.cu; semantics: oracle/alsd_restated.py).  Synchronises: the host checks every

@@ -80,11 +80,14 @@ struct DecodeArgs {
   const float* b_pred;        // f32 [Hj]
   int32_t* tokens; int32_t* frames; int32_t* n_tok;
   int B, T_max, Hj, Hp, V, U_max, max_symbols;
+  float* stats = nullptr;     // f32 [B, U_max, 4] (lp, H1, A_alpha, G_alpha) per stored token; nullptr: no confidence statistics
+  float alpha = 0.f;          // > 0 and finite when stats is set
 };
 // Byte offsets of the decode workspace's regions and its size (decode_spec.cu describes the regions)
-struct SpecWorkspace { size_t hbuf, rec, ppbuf, counters, prof, best, total; };
-SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp);
-// windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace laid out by rnnt_spec_workspace()
+struct SpecWorkspace { size_t hbuf, rec, ppbuf, counters, prof, best, conf, total; };
+SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms);
+// windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace laid out by rnnt_spec_workspace();
+// a.stats != nullptr selects the instance that also reduces the softmax statistics of every emitted token
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream);
 
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)

@@ -50,6 +50,7 @@ EXPORTS = [
     "rs_transcribe_batch", "rs_transcribe_device_pcm16", "rs_transcribe_batch_pcm16", "rs_resample_mono", "rs_rnnt_alsd", "rs_gemm_bf16", "rs_layernorm", "rs_launch_count", "rs_enable_stage_timing",
     "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing", "rs_debug_decode_cycles",
     "rs_enable_kernel_timing", "rs_kernel_timing", "rs_stage_rows",
+    "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
 ]
 
 
@@ -85,6 +86,9 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_transcribe_batch.argtypes = [vp, vp, vp, ip, ip, vp, vp, vp, ip, vp]
     lib.rs_transcribe_device_pcm16.argtypes = [vp, vp, vp, ip, ip, vp, vp, vp, ip, vp]
     lib.rs_transcribe_batch_pcm16.argtypes = [vp, vp, vp, ip, ip, vp, vp, vp, ip, vp]
+    lib.rs_rnnt_greedy_confidence.argtypes = [vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
+    lib.rs_transcribe_device_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
+    lib.rs_transcribe_batch_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
     lib.rs_rnnt_alsd.argtypes = [vp, vp, vp, ip, ip, ip, C.c_float, ip, ip, vp, vp, vp, vp, ip, vp]
     lib.rs_rnnt_alsd.restype = ip
     lib.rs_resample_mono.argtypes = [vp, vp, ip, vp, ip, ip, ip, vp, ip, ip, ip, ip, ip, vp, ip, vp, vp]
@@ -107,6 +111,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_gemm_timing.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     for fn in ("rs_workspace_bytes", "rs_set_workspace", "rs_mel_frames", "rs_enc_frames", "rs_mel_valid", "rs_enc_valid", "rs_logmel", "rs_encode",
                "rs_rnnt_greedy", "rs_transcribe_device", "rs_transcribe_batch", "rs_transcribe_device_pcm16", "rs_transcribe_batch_pcm16",
+               "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
                "rs_gemm_bf16", "rs_layernorm",
                "rs_enable_stage_timing", "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing"):
         getattr(lib, fn).restype = ip
@@ -335,7 +340,9 @@ class Engine:
                                        n_layers, self._stream()), "rs_encode")
         return enc, enc_len
 
-    def greedy(self, enc: torch.Tensor, enc_len: torch.Tensor, U_max: Optional[int] = None):
+    def greedy(self, enc: torch.Tensor, enc_len: torch.Tensor, U_max: Optional[int] = None, alpha: Optional[float] = None):
+        """-> (tokens, frames, n_tok), plus stats f32 [B, U, 4] = (lp, H1, A_alpha, G_alpha) per stored token when ``alpha`` is
+        given (rs_rnnt_greedy_confidence; the tokens are the same either way)."""
         B, T, _ = enc.shape
         assert enc.dtype == torch.float32 and enc.is_contiguous()
         self.ensure_workspace(B, (T * 8 + 8) * self.cfg.n_window_stride)
@@ -343,11 +350,17 @@ class Engine:
         tokens = torch.zeros(B, U, dtype=torch.int32, device=self.device)
         frames = torch.zeros(B, U, dtype=torch.int32, device=self.device)
         ntok = torch.zeros(B, dtype=torch.int32, device=self.device)
-        self._check(self.lib.rs_rnnt_greedy(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, tokens.data_ptr(),
-                                            frames.data_ptr(), ntok.data_ptr(), U, self._stream()), "rs_rnnt_greedy")
-        return tokens, frames, ntok
+        if alpha is None:
+            self._check(self.lib.rs_rnnt_greedy(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, tokens.data_ptr(),
+                                                frames.data_ptr(), ntok.data_ptr(), U, self._stream()), "rs_rnnt_greedy")
+            return tokens, frames, ntok
+        stats = torch.zeros(B, U, 4, dtype=torch.float32, device=self.device)
+        self._check(self.lib.rs_rnnt_greedy_confidence(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, tokens.data_ptr(), frames.data_ptr(),
+                                                       ntok.data_ptr(), U, float(alpha), stats.data_ptr(), self._stream()), "rs_rnnt_greedy_confidence")
+        return tokens, frames, ntok, stats
 
-    def transcribe_device(self, wav: torch.Tensor, lens: torch.Tensor, U_max: Optional[int] = None, out=None):
+    def transcribe_device(self, wav: torch.Tensor, lens: torch.Tensor, U_max: Optional[int] = None, out=None, alpha: Optional[float] = None):
+        """With ``alpha``: also the confidence statistics (``greedy``), ``out`` then holds four tensors."""
         B, L = wav.shape
         self.ensure_workspace(B, L)
         U = U_max or self.u_max(L)
@@ -355,15 +368,23 @@ class Engine:
             out = (torch.zeros(B, U, dtype=torch.int32, device=self.device),
                    torch.zeros(B, U, dtype=torch.int32, device=self.device),
                    torch.zeros(B, dtype=torch.int32, device=self.device))
-        tokens, frames, ntok = out
+            if alpha is not None:
+                out += (torch.zeros(B, U, 4, dtype=torch.float32, device=self.device),)
+        tokens, frames, ntok = out[:3]
         assert wav.dtype in (torch.float32, torch.int16) and wav.is_contiguous()
+        if alpha is not None:
+            self._check(self.lib.rs_transcribe_device_confidence(self.h, wav.data_ptr(), int(wav.dtype == torch.int16), lens.data_ptr(), B, L,
+                                                                 tokens.data_ptr(), frames.data_ptr(), ntok.data_ptr(), U, float(alpha),
+                                                                 out[3].data_ptr(), self._stream()), "rs_transcribe_device_confidence")
+            return tokens, frames, ntok, out[3]
         fn, name = ((self.lib.rs_transcribe_device_pcm16, "rs_transcribe_device_pcm16") if wav.dtype == torch.int16
                     else (self.lib.rs_transcribe_device, "rs_transcribe_device"))        # int16: PCM, scaled by 2^-15 on the device
         self._check(fn(self.h, wav.data_ptr(), lens.data_ptr(), B, L, tokens.data_ptr(), frames.data_ptr(), ntok.data_ptr(), U, self._stream()), name)
         return tokens, frames, ntok
 
-    def transcribe_host(self, wav: torch.Tensor, lens: torch.Tensor, U_max: Optional[int] = None, out=None):
-        """wav: host float32 or int16 (PCM) [B, L] (pinned for speed), lens: host int32 [B] -> host tokens/frames/n_tok."""
+    def transcribe_host(self, wav: torch.Tensor, lens: torch.Tensor, U_max: Optional[int] = None, out=None, alpha: Optional[float] = None):
+        """wav: host float32 or int16 (PCM) [B, L] (pinned for speed), lens: host int32 [B] -> host tokens/frames/n_tok, plus
+        the confidence statistics [B, U, 4] when ``alpha`` is given (``out`` then holds four tensors)."""
         B, L = wav.shape
         assert wav.device.type == "cpu" and wav.dtype in (torch.float32, torch.int16) and wav.is_contiguous()
         self.ensure_workspace(B, L)
@@ -371,7 +392,14 @@ class Engine:
         if out is None:
             out = (torch.zeros(B, U, dtype=torch.int32).pin_memory(), torch.zeros(B, U, dtype=torch.int32).pin_memory(),
                    torch.zeros(B, dtype=torch.int32).pin_memory())
-        tokens, frames, ntok = out
+            if alpha is not None:
+                out += (torch.zeros(B, U, 4, dtype=torch.float32).pin_memory(),)
+        tokens, frames, ntok = out[:3]
+        if alpha is not None:
+            self._check(self.lib.rs_transcribe_batch_confidence(self.h, wav.data_ptr(), int(wav.dtype == torch.int16), lens.data_ptr(), B, L,
+                                                                tokens.data_ptr(), frames.data_ptr(), ntok.data_ptr(), U, float(alpha),
+                                                                out[3].data_ptr(), self._stream()), "rs_transcribe_batch_confidence")
+            return tokens, frames, ntok, out[3]
         fn, name = ((self.lib.rs_transcribe_batch_pcm16, "rs_transcribe_batch_pcm16") if wav.dtype == torch.int16
                     else (self.lib.rs_transcribe_batch, "rs_transcribe_batch"))
         self._check(fn(self.h, wav.data_ptr(), lens.data_ptr(), B, L, tokens.data_ptr(), frames.data_ptr(), ntok.data_ptr(), U, self._stream()), name)

@@ -8,7 +8,7 @@ i is timestamp[i] - i - 1 (decode.py:48).  The engine decodes greedily and prese
 in that same shape (see transcribe.Hypothesis.from_greedy)."""
 from __future__ import annotations
 
-from typing import List, Sequence
+from typing import List, Optional, Sequence
 
 from .interface import Segment, Subword, TranscribeResult
 
@@ -47,7 +47,9 @@ def find_end_of_segment(subwords: Sequence[Subword], start: int) -> int:
     return max(last, start)
 
 
-def build_result(tokenizer, token_ids: Sequence[int], steps: Sequence[int]) -> TranscribeResult:
+def build_result(tokenizer, token_ids: Sequence[int], steps: Sequence[int],
+                 token_confidence: Optional[Sequence[float]] = None) -> TranscribeResult:
+    """``token_confidence`` (one value per token id) is carried onto the subwords that are kept."""
     token_ids = [int(t) for t in token_ids]
     text = tokenizer.ids_to_text(token_ids)
     # ids_to_text([tid]) is a pure function of tid: remembered per tokenizer object (a 30 s clip asks ~100 times, a batched
@@ -62,7 +64,8 @@ def build_result(tokenizer, token_ids: Sequence[int], steps: Sequence[int]) -> T
         if piece is None:
             piece = single[tid] = tokenizer.ids_to_text([tid])
         if piece:                                   # a bare word-boundary mark decodes to "" (decode.py:51-53)
-            pieces.append(Subword(max(SECONDS_PER_STEP * (int(step) - index - 1) - PAD_SECONDS, 0), tid, piece))   # token_seconds, inlined
+            pieces.append(Subword(max(SECONDS_PER_STEP * (int(step) - index - 1) - PAD_SECONDS, 0), tid, piece,   # token_seconds, inlined
+                                  None if token_confidence is None else float(token_confidence[index])))
     segments: List[Segment] = []
     begin = 0
     while begin < len(pieces):
@@ -76,5 +79,6 @@ def build_result(tokenizer, token_ids: Sequence[int], steps: Sequence[int]) -> T
 
 def decode_hypothesis(model, hyp) -> TranscribeResult:
     """Same signature as the reference: `model` needs .tokenizer.ids_to_text, `hyp` needs
-    .y_sequence (tensor-like with .tolist(), leading blank) and .timestamp."""
-    return build_result(model.tokenizer, hyp.y_sequence.tolist()[1:], list(hyp.timestamp))
+    .y_sequence (tensor-like with .tolist(), leading blank) and .timestamp; its .token_confidence, when present and not
+    None, goes onto the subwords."""
+    return build_result(model.tokenizer, hyp.y_sequence.tolist()[1:], list(hyp.timestamp), getattr(hyp, "token_confidence", None))

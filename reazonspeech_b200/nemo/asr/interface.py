@@ -23,13 +23,18 @@ class AudioData:
 
 @dataclass
 class Subword:
-    """One emitted token with the time of the encoder frame that emitted it."""
+    """One emitted token with the time of the encoder frame that emitted it, and its confidence when the model was loaded
+    with a ``ConfidenceConfig`` (None otherwise)."""
     seconds: float
     token_id: int
     token: str
+    confidence: Optional[float] = None
 
     def as_dict(self) -> dict:
-        return {"seconds": self.seconds, "token_id": self.token_id, "token": self.token}
+        d = {"seconds": self.seconds, "token_id": self.token_id, "token": self.token}
+        if self.confidence is not None:
+            d["confidence"] = self.confidence
+        return d
 
 
 @dataclass

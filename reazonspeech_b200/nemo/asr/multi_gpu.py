@@ -32,13 +32,15 @@ class MultiGpuRnntModel:
         self.cfg = self.replicas[0].cfg
         self.tokenizer = self.replicas[0].tokenizer
         self.max_batch = self.replicas[0].max_batch
+        self.confidence = getattr(self.replicas[0], "confidence", None)
 
     @property
     def devices(self) -> List[str]:
         return [str(r.engine.device) for r in self.replicas]
 
     def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
-        """Yields ``(indices, [(tokens, frames)])`` per finished engine batch of any device, indices into ``waveforms``."""
+        """Yields ``(indices, [(tokens, frames)])`` per finished engine batch of any device, indices into ``waveforms``
+        (``(tokens, frames, stats)`` items with confidence on, as ``B200RnntModel.iter_token_batches``)."""
         if len(waveforms) == 0:
             return
         shards = [s for s in shard_indices([len(w) for w in waveforms], len(self.replicas))]
@@ -82,9 +84,9 @@ class MultiGpuRnntModel:
     def transcribe(self, audio, batch_size: int = 1, return_hypotheses: bool = True, verbose: bool = True, **_):
         """NeMo's call shape (pkg/nemo-asr/src/transcribe.py:48-53) over all devices."""
         import torch
-        from .transcribe import Hypothesis
+        from .transcribe import greedy_hypothesis
         waves = [a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a) for a in audio]
-        hyps = [Hypothesis.from_greedy(t, f, self.cfg.blank) for t, f in self.transcribe_tokens(waves)]
+        hyps = [greedy_hypothesis(self, item) for item in self.transcribe_tokens(waves)]
         if return_hypotheses:
             return hyps
         return [self.tokenizer.ids_to_text(h.y_sequence.tolist()[1:]) for h in hyps]

@@ -12,12 +12,14 @@ from __future__ import annotations
 import glob
 import os
 from dataclasses import dataclass
+from functools import partial
 from typing import List, Optional, Sequence
 
 import numpy as np
 import torch
 
 from ...config import ModelConfig
+from ...confidence import ConfidenceConfig, measure, word_confidence
 from ...engine import Engine
 from ...tokenizer import PieceTableTokenizer, SentencePieceTokenizer, synthetic_pieces
 from ...weights import load_nemo_archive, random_state_dict
@@ -38,11 +40,29 @@ class Hypothesis:
     y_sequence: torch.Tensor
     timestamp: List[int]
     score: float = 0.0
+    token_confidence: Optional[List[float]] = None
+    word_confidence: Optional[List[float]] = None
 
     @staticmethod
     def from_greedy(tokens: Sequence[int], frames: Sequence[int], blank: int) -> "Hypothesis":
         y = torch.tensor([blank, *[int(t) for t in tokens]], dtype=torch.long)
         return Hypothesis(y, [int(f) + i + 1 for i, f in enumerate(frames)])
+
+
+def greedy_hypothesis(model, item) -> Hypothesis:
+    """One item of ``iter_token_batches`` -> Hypothesis.  With confidence on, the item carries the utterance's statistics
+    rows (lp, H1, A_alpha, G_alpha) and the hypothesis gets token / word confidence and score = sum of the emitted tokens'
+    log-probabilities.  (NeMo's greedy loop adds the joint's maximum output, which is a log-probability only where the joint
+    is log-normalised (R): the sum of log-probabilities is the score a corpus filter can compare across utterances.)"""
+    hyp = Hypothesis.from_greedy(item[0], item[1], model.cfg.blank)
+    conf: Optional[ConfidenceConfig] = getattr(model, "confidence", None)
+    if conf is not None:
+        stats = np.asarray(item[2], dtype=np.float64).reshape(-1, 4)
+        tc = [float(x) for x in measure(stats, model.cfg.vocab_size + 1, conf.method_cfg)]
+        hyp.token_confidence = tc
+        hyp.word_confidence = word_confidence(tc, model.tokenizer.ids_to_pieces(item[0]), conf.aggregation)
+        hyp.score = float(stats[:, 0].sum())
+    return hyp
 
 
 class HostStaging:
@@ -92,29 +112,38 @@ class HostStaging:
         lens.copy_(torch.tensor([a.shape[0] + 2 * pad for a in srcs], dtype=torch.int32))
         return wav, lens
 
-    def outputs(self, B: int, U: int):
+    def outputs(self, B: int, U: int, stats: bool = False):
+        """(tokens [B, U], frames [B, U], n_tok [B]), plus the confidence statistics [B, U, 4] with ``stats``."""
         self._tok = self._grown(self._tok, B * U, torch.int32)
         self._frm = self._grown(self._frm, B * U, torch.int32)
         self._ntok = self._grown(self._ntok, B, torch.int32)
-        return self._tok[: B * U].view(B, U), self._frm[: B * U].view(B, U), self._ntok[:B]
+        out = self._tok[: B * U].view(B, U), self._frm[: B * U].view(B, U), self._ntok[:B]
+        if not stats:
+            return out
+        self._stats = self._grown(getattr(self, "_stats", None), B * U * 4, torch.float32)
+        return out + (self._stats[: B * U * 4].view(B, U, 4),)
 
 
 class B200RnntModel:
     """Engine + tokenizer behind NeMo's model surface."""
 
-    def __init__(self, engine: Engine, tokenizer, max_batch: int = 64, decoding: str = "greedy", beam_size: int = 4):
+    def __init__(self, engine: Engine, tokenizer, max_batch: int = 64, decoding: str = "greedy", beam_size: int = 4,
+                 confidence: Optional[ConfidenceConfig] = None):
         self.engine = engine
         self.cfg = engine.cfg
         self.tokenizer = tokenizer
         self.max_batch = max_batch
         self.decoding, self.beam_size = decoding, beam_size       # "greedy" (north_star's parity target) or "alsd" (the checkpoint's default)
+        if confidence is not None and decoding != "greedy":
+            raise ValueError("confidence is computed by the greedy decode only (NeMo offers none for beam search)")
+        self.confidence = confidence.validate() if confidence is not None else None
         pin = torch.cuda.is_available()
         self._staging = (HostStaging(pin), HostStaging(pin))      # double buffer: stage batch k+1 while batch k runs
 
     # -- token-level batched path
     def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
         """16 kHz mono waveforms (each gets ``pad`` zero samples on both sides) -> yields ``(indices, [(tokens, frames)])``
-        batch by batch.
+        batch by batch; with confidence on, ``(tokens, frames, stats)``, stats float32 [n_tokens, 4] (lp, H1, A_alpha, G_alpha).
 
         Utterances are sorted by length and cut into batches of at most ``max_batch`` so padding waste stays small.
         The engine call of batch k runs on a worker thread (ctypes drops the GIL) while this thread stages batch k+1
@@ -127,26 +156,27 @@ class B200RnntModel:
         batches = [order[lo:lo + self.max_batch] for lo in range(0, len(order), self.max_batch)]
         eng = self.engine
         eng.ensure_workspace(len(batches[0]), (len(waveforms[order[-1]]) + 2 * pad + 3) & ~3)   # once, on this thread (stage() rounds rows up to 4 samples)
+        alpha = self.confidence.alpha if self.confidence is not None else None
+        call = eng.transcribe_host if alpha is None else partial(eng.transcribe_host, alpha=alpha)
 
         def run(staging, idx):
             wav, lens = staging.stage([waveforms[i] for i in idx], pad)
-            out = staging.outputs(len(idx), eng.u_max(wav.shape[1]))
+            U = eng.u_max(wav.shape[1])
+            out = staging.outputs(len(idx), U) if alpha is None else staging.outputs(len(idx), U, stats=True)
             return wav, lens, out
 
         def collect(done, idx):
-            tokens, frames, ntok = done
-            counts = ntok.tolist()
-            return idx, [(tokens[r, :n].tolist(), frames[r, :n].tolist()) for r, n in enumerate(counts[: len(idx)])]
+            return idx, _items(done, len(idx))
 
         if len(batches) == 1:                                         # nothing to overlap: skip the thread hand-off (one-clip calls)
             wav, lens, out = run(self._staging[0], batches[0])
-            yield collect(eng.transcribe_host(wav, lens, out[0].shape[1], out), batches[0])
+            yield collect(call(wav, lens, out[0].shape[1], out), batches[0])
             return
         with ThreadPoolExecutor(max_workers=1) as pool:
             in_flight = None
             for k, idx in enumerate(batches):
                 wav, lens, out = run(self._staging[k & 1], idx)
-                nxt = (pool.submit(eng.transcribe_host, wav, lens, out[0].shape[1], out), idx)
+                nxt = (pool.submit(call, wav, lens, out[0].shape[1], out), idx)
                 if in_flight is not None:
                     yield collect(in_flight[0].result(), in_flight[1])
                 in_flight = nxt
@@ -188,9 +218,9 @@ class B200RnntModel:
             lens = torch.tensor([waves[i].shape[1] for i in idx], dtype=torch.int32)
             with torch.cuda.device(eng.device):
                 wav, wl = eng.resample_mono(raw.to(eng.device, non_blocking=True), lens.to(eng.device, non_blocking=True), samplerate, pad)
-                tokens, frames, ntok = eng.transcribe_device(wav, wl)
-                tokens, frames, counts = tokens.cpu(), frames.cpu(), ntok.cpu().tolist()
-            yield idx, [(tokens[r, :n].tolist(), frames[r, :n].tolist()) for r, n in enumerate(counts)]
+                done = [a.cpu() for a in (eng.transcribe_device(wav, wl) if self.confidence is None else
+                                          eng.transcribe_device(wav, wl, alpha=self.confidence.alpha))]
+            yield idx, _items(done, len(idx))
 
     # -- NeMo's call shape (transcribe.py:48-53): already padded tensors
     def transcribe_alsd(self, waveforms: Sequence[np.ndarray], pad: int = 0) -> List[Hypothesis]:
@@ -219,10 +249,21 @@ class B200RnntModel:
         if self.decoding == "alsd":
             out = self.transcribe_alsd(waves)
         else:
-            out = [Hypothesis.from_greedy(t, f, self.cfg.blank) for t, f in self.transcribe_tokens(waves)]
+            out = [greedy_hypothesis(self, item) for item in self.transcribe_tokens(waves)]
         if return_hypotheses:
             return out
         return [self.tokenizer.ids_to_text(h.y_sequence.tolist()[1:]) for h in out]
+
+
+def _items(done, B: int):
+    """Host outputs of one engine call -> per utterance (tokens, frames), or (tokens, frames, stats) with the statistics."""
+    tokens, frames, ntok = done[:3]
+    U = tokens.shape[1]
+    counts = ntok.tolist()[:B]
+    if len(done) == 3:
+        return [(tokens[r, :n].tolist(), frames[r, :n].tolist()) for r, n in enumerate(counts)]
+    stats = done[3]
+    return [(tokens[r, :n].tolist(), frames[r, :n].tolist(), stats[r, : min(n, U)].numpy().copy()) for r, n in enumerate(counts)]
 
 
 def _find_checkpoint() -> Optional[str]:
@@ -236,7 +277,7 @@ def _find_checkpoint() -> Optional[str]:
 
 def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Optional[bool] = None,
                config: Optional[ModelConfig] = None, seed: int = 0, max_batch: int = 64, devices: Optional[Sequence] = None,
-               decoding: str = "greedy", beam_size: int = 4):
+               decoding: str = "greedy", beam_size: int = 4, confidence: Optional[ConfidenceConfig] = None):
     """Load the ReazonSpeech FastConformer-RNNT onto a B200.
 
     ``device``: None / "cuda" / "cuda:N" as in the reference (transcribe.py:9-22, eval.py:26).
@@ -247,7 +288,12 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     (``multi_gpu.MultiGpuRnntModel``; same surface, results in input order).  Weights come from ``checkpoint`` (a .nemo file),
     $REAZONSPEECH_NEMO_CHECKPOINT or the local Hugging Face cache of reazonspeech-nemo-v2.
     With ``synthetic=True`` (or $REAZONSPEECH_B200_SYNTHETIC=1) seeded random weights of the same
-    architecture are used instead -- the only option offline."""
+    architecture are used instead -- the only option offline.  ``confidence``: a ``ConfidenceConfig`` turns on token / word
+    confidence and log-probability scores of the greedy decode (``confidence.py``); not available with ``decoding="alsd"``."""
+    if confidence is not None:
+        if decoding == "alsd":
+            raise ValueError("confidence is computed by the greedy decode only (NeMo offers none for beam search)")
+        confidence.validate()
     if device is None:
         device = "cuda"
     if str(device).startswith("cpu"):
@@ -273,7 +319,8 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     if decoding not in ("greedy", "alsd"):
         raise ValueError(f"decoding must be 'greedy' or 'alsd', got {decoding!r}")
     if devices is None:
-        return B200RnntModel(Engine(cfg, sd, str(device), alsd=decoding == "alsd"), tokenizer, max_batch=max_batch, decoding=decoding, beam_size=beam_size)
+        return B200RnntModel(Engine(cfg, sd, str(device), alsd=decoding == "alsd"), tokenizer, max_batch=max_batch, decoding=decoding, beam_size=beam_size,
+                             confidence=confidence)
     if decoding != "greedy":
         raise ValueError("the one-process multi-GPU model decodes greedily; load one model per device for beam search")
     names = [d if isinstance(d, str) else f"cuda:{int(d)}" for d in devices]
@@ -282,7 +329,8 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     from ...engine import pack_weights
     from .multi_gpu import MultiGpuRnntModel
     packed = pack_weights(sd, cfg)                                   # repacked once, uploaded once per device
-    return MultiGpuRnntModel([B200RnntModel(Engine(cfg, None, n, packed=packed), tokenizer, max_batch=max_batch) for n in names])
+    return MultiGpuRnntModel([B200RnntModel(Engine(cfg, None, n, packed=packed), tokenizer, max_batch=max_batch, confidence=confidence)
+                              for n in names])
 
 
 def _prepare(audio: AudioData) -> np.ndarray:
@@ -320,7 +368,6 @@ def transcribe_batch(model, audios: Sequence[AudioData], config: Optional[Transc
         out[i] = r
 
     if hasattr(model, "iter_token_batches") and getattr(model, "decoding", "greedy") == "greedy":
-        blank = model.cfg.blank
         pad = int(PAD_SECONDS * SAMPLERATE)
         # audio that still needs norm_audio (another rate, several channels) and is uniform in both goes to the GPU as it is:
         # resampling, down-mixing and padding run there (iter_token_batches_raw); anything else is normalised on the host
@@ -333,8 +380,8 @@ def transcribe_batch(model, audios: Sequence[AudioData], config: Optional[Transc
         else:
             batches = model.iter_token_batches([np.asarray(norm_audio(a).waveform) for a in audios], pad=pad)
         for idx, items in batches:
-            for i, (tokens, frames) in zip(idx, items):
-                finish(i, Hypothesis.from_greedy(tokens, frames, blank))
+            for i, item in zip(idx, items):
+                finish(i, greedy_hypothesis(model, item))
     else:
         tensors = [torch.from_numpy(_prepare(a)) for a in audios]
         hyps = model.transcribe(tensors, batch_size=max(len(tensors), 1), return_hypotheses=True, verbose=config.verbose)

@@ -53,3 +53,6 @@ class SentencePieceTokenizer:
 
     def ids_to_text(self, ids: Iterable[int]) -> str:
         return self.sp.decode_ids([int(i) for i in ids])
+
+    def ids_to_pieces(self, ids: Iterable[int]) -> List[str]:
+        return [self.sp.id_to_piece(int(i)) for i in ids]
