@@ -183,13 +183,39 @@ int rs_resample_mono(rs_engine* e, const void* in_dev, int in_is_pcm16, const in
 int rs_stage_rows(void* dst, int64_t L, const void* const* src, const int64_t* n, const int32_t* src_is_pcm16,
                   int dst_is_pcm16, int B, int64_t pad, int threads);
 
-/* ---- kernel-level seams (parity tests and roofline measurement) --------------------------- */
+/* ---- kernel-level seams (parity tests and roofline measurement) ---------------------------
+ * Each calls one kernel launcher with the shapes given (not the engine's configuration); none needs the workspace.
+ * A shape or parameter the kernel does not implement is rejected before any launch (RS_ERR_UNSUPPORTED /
+ * RS_ERR_INVALID_ARG). */
+/* out2 / split / ld2: RS_EPI_QKV_VT only (columns >= split go transposed to out2 bf16 [N - split, ld2], ld2 >= M). */
 int rs_gemm_bf16(rs_engine* e, const void* a_bf16, const void* w_bf16, const float* bias,
                  const float* resid, void* out, int M, int N, int K, int epilogue, float alpha,
-                 void* stream);
+                 void* out2, int split, int ld2, void* stream);
+/* gamma2 / beta2 (nullable): a second LayerNorm chained on the first's result, written to out_bf16 (norm_out of one layer
+ * feeding the next layer's first pre-norm); out_f32 may be x (in place). */
 int rs_layernorm(rs_engine* e, const float* x, const float* gamma, const float* beta,
-                 float* out_f32 /*nullable*/, void* out_bf16 /*nullable*/, int rows, int d,
-                 void* stream);
+                 float* out_f32 /*nullable*/, void* out_bf16 /*nullable*/, const float* gamma2,
+                 const float* beta2, int rows, int d, void* stream);
+/* Local attention + global token (head dim 128): qkv bf16 [B*T_max, 3*H*128] with q + pos_bias_u in the q columns and k
+ * after them, V^T bf16 [H*128, ld_vt] (column = b*T_max + t), pos bf16 [H, n_rel_pad, 128], bd_bias f32 [H, n_rel_pad],
+ * bias_u f32 [H, 128] -> out bf16 [B*T_max, H*128] (rows >= enc_len[b] zero). */
+int rs_attention(rs_engine* e, const void* qkv_bf16, const void* vt_bf16, int ld_vt, const void* pos_bf16,
+                 const float* bd_bias, int n_rel_pad, const float* bias_u, void* out_bf16, const int32_t* enc_len,
+                 int B, int T_max, int H, int w_left, int w_right, int n_global, void* stream);
+/* Depthwise conv (k taps, BatchNorm folded into w [k, d] and shift [d]) + Swish on bf16 [B*T_max, d]; input rows
+ * t >= enc_len[b] read as zero. */
+int rs_conv_dw(rs_engine* e, const void* u_bf16, void* out_bf16, const float* w_f32, const float* shift_f32,
+               const int32_t* enc_len, int B, int T_max, int d, int k, void* stream);
+/* Subsampling conv.0 (1 -> C, 3x3 s2) + ReLU + conv.2 (depthwise 3x3 s2) on mel f32 [B, F_max, n_mels] -> bf16
+ * [B, T2, F2, C] with T1 = conv_len(F_max), T2 = conv_len(T1), F2 = conv_len(conv_len(n_mels)).  mel_stats
+ * [B, n_mels, 2] = (mean, 1 / (std + eps)) normalises the features on load; NULL: they are already normalised. */
+int rs_sub_conv0_dw1(rs_engine* e, const float* mel, const int32_t* mel_len, const float* mel_stats, int B, int F_max,
+                     int n_mels, int C, const float* w0, const float* b0, const float* wd, const float* bd,
+                     void* out_bf16, void* stream);
+/* Depthwise 3x3 s2 on channels-last bf16 [B, Tin, Fin, C] -> [B, Tout, Fout, C]; the valid input length of utterance b
+ * is conv_len applied len_shift times to mel_len[b]. */
+int rs_sub_dw(rs_engine* e, const void* in_bf16, void* out_bf16, const float* w, const float* b, const int32_t* mel_len,
+              int len_shift, int B, int Tin, int Fin, int Tout, int Fout, int C, void* stream);
 /* Counters: kernels launched by this engine since creation (bench.py's gpu_launches). */
 int64_t rs_launch_count(const rs_engine* e);
 /* Per-stage device time of the last rs_transcribe_* call when timing was enabled. */

@@ -197,7 +197,7 @@ Plan make_plan(const rs_engine* e, int B, int L_max, int U_max) {
   p.abuf = a.take(static_cast<size_t>(p.M) * d * 2);
   p.cbuf = a.take(static_cast<size_t>(p.M) * d * 2);
   p.n_rel_pad = ((c.att_left + c.att_right + 1 + 31) / 32) * 32;
-  p.ld_vt = ((p.M + 255) / 256) * 256 + 64;                               // V^T row pitch: covers the GEMM's 256-row tile overhang
+  p.ld_vt = ((p.M + 255) / 256) * 256 + 64;                               // V^T row pitch (the GEMM writes columns < M only; any ld_vt >= M works)
   p.vt = a.take(static_cast<size_t>(d) * p.ld_vt * 2);
   p.enc = a.take(static_cast<size_t>(p.M) * d * 4);
   p.encp = a.take(static_cast<size_t>(p.M) * c.joint_hidden * 4);
@@ -776,18 +776,77 @@ int rs_resample_mono(rs_engine* e, const void* in_dev, int in_is_pcm16, const in
 }
 
 int rs_gemm_bf16(rs_engine* e, const void* a, const void* w, const float* bias, const float* resid, void* out, int M,
-                 int N, int K, int epilogue, float alpha, void* stream) {
+                 int N, int K, int epilogue, float alpha, void* out2, int split, int ld2, void* stream) {
   if (!e || !a || !w || !out) return fail(e, RS_ERR_INVALID_ARG, "rs_gemm_bf16: bad arguments");
+  if (epilogue == RS_EPI_QKV_VT && (!out2 || split <= 0 || split >= N || split % 32 || M % 8 || ld2 % 8 || ld2 < M))
+    return fail(e, RS_ERR_INVALID_ARG, "rs_gemm_bf16: RS_EPI_QKV_VT needs out2, 0 < split < N, split %% 32 == 0, M %% 8 == 0, ld2 %% 8 == 0, ld2 >= M");
   RS_CUDA(e, cudaSetDevice(e->device));
-  return gemm(e, {a, w, bias, resid, out, M, N, K, epilogue, alpha}, static_cast<cudaStream_t>(stream));
+  return gemm(e, {a, w, bias, resid, out, M, N, K, epilogue, alpha, out2, split, ld2}, static_cast<cudaStream_t>(stream));
 }
 
 int rs_layernorm(rs_engine* e, const float* x, const float* gamma, const float* beta, float* out_f32, void* out_bf16,
-                 int rows, int d, void* stream) {
-  if (!e || !x || !gamma || !beta) return fail(e, RS_ERR_INVALID_ARG, "rs_layernorm: bad arguments");
+                 const float* gamma2, const float* beta2, int rows, int d, void* stream) {
+  if (!e || !x || !gamma || !beta || (gamma2 == nullptr) != (beta2 == nullptr)) return fail(e, RS_ERR_INVALID_ARG, "rs_layernorm: bad arguments");
+  if (gamma2 != nullptr && out_bf16 == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_layernorm: the chained LayerNorm writes out_bf16");
+  if (d != 256 && d != 512 && d != 1024) return fail(e, RS_ERR_UNSUPPORTED, "rs_layernorm: d=%d unsupported (256/512/1024)", d);
   RS_CUDA(e, cudaSetDevice(e->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, gamma, beta, out_f32, out_bf16, nullptr, nullptr, rows, d, e->cfg.ln_eps, s));
+  RS_LAUNCH(e, s, 1, rs::launch_layernorm(x, gamma, beta, out_f32, out_bf16, gamma2, beta2, rows, d, e->cfg.ln_eps, s));
+  return RS_OK;
+}
+
+int rs_attention(rs_engine* e, const void* qkv, const void* vt, int ld_vt, const void* pos, const float* bd_bias, int n_rel_pad,
+                 const float* bias_u, void* out, const int32_t* enc_len, int B, int T_max, int H, int w_left, int w_right,
+                 int n_global, void* stream) {
+  if (!e || !qkv || !vt || !pos || !bd_bias || !bias_u || !out || !enc_len || B <= 0 || T_max <= 0 || H <= 0)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_attention: bad arguments");
+  rs::AttnArgs aa{qkv, pos, bd_bias, n_rel_pad, bias_u, out, enc_len, B, T_max, H, 128, w_left, w_right, n_global};
+  aa.vt = vt; aa.ld_vt = ld_vt;
+  if (!rs::attention_tc_supported(aa))
+    return fail(e, RS_ERR_UNSUPPORTED, "rs_attention: unsupported geometry (0 <= w_left, w_right <= 128, w_left %% 8 == 0, n_global 0/1, "
+                "T_max %% 8 == 0, n_rel_pad a multiple of 32 in [w_left + w_right + 1, 288])");
+  // the global-row kernel keeps max(T_max, 1024) scores in at most 200 KB of shared memory
+  if (ld_vt % 8 || static_cast<int64_t>(ld_vt) < static_cast<int64_t>(B) * T_max || (n_global > 0 && (T_max + 8 + 128) * 4 > 200 * 1024))
+    return fail(e, RS_ERR_INVALID_ARG, "rs_attention: ld_vt must be a multiple of 8 and >= B*T_max; T_max too large for the global row");
+  RS_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  RS_LAUNCH(e, s, n_global > 0 ? 2 : 1, rs::launch_attention_tc(aa, s));
+  return RS_OK;
+}
+
+int rs_conv_dw(rs_engine* e, const void* u, void* out, const float* w, const float* shift, const int32_t* enc_len, int B, int T_max,
+               int d, int k, void* stream) {
+  if (!e || !u || !out || !w || !shift || !enc_len || B <= 0 || T_max <= 0 || d <= 0) return fail(e, RS_ERR_INVALID_ARG, "rs_conv_dw: bad arguments");
+  if (k != 9) return fail(e, RS_ERR_UNSUPPORTED, "rs_conv_dw: k=%d unsupported (9)", k);
+  if (d % 4) return fail(e, RS_ERR_INVALID_ARG, "rs_conv_dw: d %% 4 != 0");
+  RS_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  RS_LAUNCH(e, s, 1, rs::launch_conv_dw(u, out, w, shift, enc_len, B, T_max, d, k, s));
+  return RS_OK;
+}
+
+int rs_sub_conv0_dw1(rs_engine* e, const float* mel, const int32_t* mel_len, const float* mel_stats, int B, int F_max, int n_mels, int C,
+                     const float* w0, const float* b0, const float* wd, const float* bd, void* out, void* stream) {
+  if (!e || !mel || !mel_len || !w0 || !b0 || !wd || !bd || !out || B <= 0 || F_max <= 0 || n_mels <= 0 || C <= 0)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_sub_conv0_dw1: bad arguments");
+  // the kernel stages 19 rows of n_mels + 8 floats in the default 48 KB of shared memory
+  if (n_mels > 600) return fail(e, RS_ERR_UNSUPPORTED, "rs_sub_conv0_dw1: n_mels=%d unsupported (<= 600)", n_mels);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  const int T1 = conv_len(F_max), F1 = conv_len(n_mels);
+  rs::SubsampleArgs sa{mel, mel_len, mel_stats, B, F_max, n_mels, C, w0, b0, wd, bd, out, T1, F1, conv_len(T1), conv_len(F1)};
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  RS_LAUNCH(e, s, 1, rs::launch_sub_conv0_dw1(sa, s));
+  return RS_OK;
+}
+
+int rs_sub_dw(rs_engine* e, const void* in, void* out, const float* w, const float* b, const int32_t* mel_len, int len_shift, int B,
+              int Tin, int Fin, int Tout, int Fout, int C, void* stream) {
+  if (!e || !in || !out || !w || !b || !mel_len || len_shift < 0 || B <= 0 || Tin <= 0 || Fin <= 0 || Tout <= 0 || Fout <= 0 || C <= 0)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_sub_dw: bad arguments");
+  if (C % 8 || C / 8 > 128 || 128 % (C / 8)) return fail(e, RS_ERR_UNSUPPORTED, "rs_sub_dw: C=%d unsupported (C / 8 must divide 128)", C);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  RS_LAUNCH(e, s, 1, rs::launch_sub_dw(in, out, w, b, mel_len, len_shift, B, Tin, Fin, Tout, Fout, C, s));
   return RS_OK;
 }
 

@@ -22,7 +22,7 @@ struct GemmArgs {
   int M, N, K;
   int epilogue;        // rs_epilogue
   float alpha;
-  // RS_EPI_QKV_VT: columns >= split go, transposed, to out2 (bf16 [N - split, ld2]; ld2 >= M rounded up to 256)
+  // RS_EPI_QKV_VT: columns >= split go, transposed, to out2 (bf16 [N - split, ld2]; ld2 >= M, only columns < M are written)
   void* out2 = nullptr; int split = 0, ld2 = 0;
 };
 

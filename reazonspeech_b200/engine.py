@@ -21,7 +21,7 @@ from .weights import StateDict, rel_pos_table
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "librs_engine.so")
 
-EPI_BIAS_BF16, EPI_BIAS_RELU_BF16, EPI_BIAS_SWISH_BF16, EPI_BIAS_GLU_BF16, EPI_RESID_F32, EPI_BIAS_F32, EPI_BIAS_F16 = range(7)
+EPI_BIAS_BF16, EPI_BIAS_RELU_BF16, EPI_BIAS_SWISH_BF16, EPI_BIAS_GLU_BF16, EPI_RESID_F32, EPI_BIAS_F32, EPI_BIAS_F16, EPI_QKV_VT = range(8)
 
 
 class RsModelConfig(C.Structure):
@@ -51,6 +51,7 @@ EXPORTS = [
     "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing", "rs_debug_decode_cycles",
     "rs_enable_kernel_timing", "rs_kernel_timing", "rs_stage_rows",
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
+    "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
 ]
 
 
@@ -93,8 +94,12 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_alsd.restype = ip
     lib.rs_resample_mono.argtypes = [vp, vp, ip, vp, ip, ip, ip, vp, ip, ip, ip, ip, ip, vp, ip, vp, vp]
     lib.rs_resample_mono.restype = ip
-    lib.rs_gemm_bf16.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, ip, ip, C.c_float, vp]
-    lib.rs_layernorm.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, vp]
+    lib.rs_gemm_bf16.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, ip, ip, C.c_float, vp, ip, ip, vp]
+    lib.rs_layernorm.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, ip, ip, vp]
+    lib.rs_attention.argtypes = [vp, vp, vp, ip, vp, vp, ip, vp, vp, vp, ip, ip, ip, ip, ip, ip, vp]
+    lib.rs_conv_dw.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, ip, ip, vp]
+    lib.rs_sub_conv0_dw1.argtypes = [vp, vp, vp, vp, ip, ip, ip, ip, vp, vp, vp, vp, vp, vp]
+    lib.rs_sub_dw.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, ip, ip, ip, ip, ip, vp]
     lib.rs_launch_count.argtypes = [vp]
     lib.rs_launch_count.restype = C.c_int64
     lib.rs_enable_stage_timing.argtypes = [vp, ip]
@@ -112,7 +117,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     for fn in ("rs_workspace_bytes", "rs_set_workspace", "rs_mel_frames", "rs_enc_frames", "rs_mel_valid", "rs_enc_valid", "rs_logmel", "rs_encode",
                "rs_rnnt_greedy", "rs_transcribe_device", "rs_transcribe_batch", "rs_transcribe_device_pcm16", "rs_transcribe_batch_pcm16",
                "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
-               "rs_gemm_bf16", "rs_layernorm",
+               "rs_gemm_bf16", "rs_layernorm", "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
                "rs_enable_stage_timing", "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing"):
         getattr(lib, fn).restype = ip
     _lib = lib
@@ -444,7 +449,10 @@ class Engine:
 
     # -- kernel seams
     def gemm(self, a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], epilogue: int,
-             resid: Optional[torch.Tensor] = None, alpha: float = 1.0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+             resid: Optional[torch.Tensor] = None, alpha: float = 1.0, out: Optional[torch.Tensor] = None,
+             out2: Optional[torch.Tensor] = None, split: int = 0) -> torch.Tensor:
+        """``out2`` / ``split``: EPI_QKV_VT only -- columns >= split go transposed into out2 (bf16 [N - split, ld2], its row
+        pitch ld2 = out2.stride(0)); ``out`` keeps the row pitch N and its columns >= split are not written."""
         M, K = a.shape
         N = w.shape[0]
         assert a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and a.is_contiguous() and w.is_contiguous()
@@ -457,9 +465,14 @@ class Engine:
                 out = torch.empty(M, N // 2, dtype=torch.bfloat16, device=self.device)
             else:
                 out = torch.empty(M, N, dtype=torch.bfloat16, device=self.device)
+        ld2 = 0
+        if out2 is not None:
+            assert out2.dtype == torch.bfloat16 and out2.dim() == 2 and out2.stride(1) == 1
+            ld2 = out2.stride(0)
         self._check(self.lib.rs_gemm_bf16(self.h, a.data_ptr(), w.data_ptr(), bias.data_ptr() if bias is not None else None,
                                           resid.data_ptr() if resid is not None else None, out.data_ptr(), M, N, K,
-                                          epilogue, alpha, self._stream()), "rs_gemm_bf16")
+                                          epilogue, alpha, out2.data_ptr() if out2 is not None else None, split, ld2,
+                                          self._stream()), "rs_gemm_bf16")
         return out
 
     def layernorm(self, x: torch.Tensor, g: torch.Tensor, b: torch.Tensor, bf16_out: bool = True) -> torch.Tensor:
@@ -467,7 +480,62 @@ class Engine:
         out = torch.empty(rows, d, dtype=torch.bfloat16 if bf16_out else torch.float32, device=self.device)
         self._check(self.lib.rs_layernorm(self.h, x.data_ptr(), g.data_ptr(), b.data_ptr(),
                                           None if bf16_out else out.data_ptr(), out.data_ptr() if bf16_out else None,
-                                          rows, d, self._stream()), "rs_layernorm")
+                                          None, None, rows, d, self._stream()), "rs_layernorm")
+        return out
+
+    def layernorm_chained(self, x: torch.Tensor, g: torch.Tensor, b: torch.Tensor, g2: torch.Tensor, b2: torch.Tensor,
+                          out_f32: torch.Tensor, out_bf16: torch.Tensor) -> None:
+        """out_f32 = LN1(x) (``out_f32`` may be ``x``: in place, as the encoder runs it), out_bf16 = LN2(LN1(x))."""
+        rows, d = x.shape
+        assert x.dtype == out_f32.dtype == torch.float32 and out_bf16.dtype == torch.bfloat16
+        self._check(self.lib.rs_layernorm(self.h, x.data_ptr(), g.data_ptr(), b.data_ptr(), out_f32.data_ptr(), out_bf16.data_ptr(),
+                                          g2.data_ptr(), b2.data_ptr(), rows, d, self._stream()), "rs_layernorm")
+
+    def attention(self, qkv: torch.Tensor, vt: torch.Tensor, pos: torch.Tensor, bd_bias: torch.Tensor, bias_u: torch.Tensor,
+                  enc_len: torch.Tensor, B: int, T_max: int, w_left: int, w_right: int, n_global: int,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The local-attention kernels alone: qkv bf16 [B*T_max, 3*H*128] (q + pos_bias_u | k | unused), vt bf16 [H*128, ld_vt]
+        (row pitch vt.stride(0)), pos bf16 [H, n_rel_pad, 128], bd_bias f32 [H, n_rel_pad], bias_u f32 [H, 128] ->
+        bf16 [B*T_max, H*128]."""
+        H, n_rel_pad, _ = pos.shape
+        assert qkv.dtype == vt.dtype == pos.dtype == torch.bfloat16 and vt.stride(1) == 1 and enc_len.dtype == torch.int32
+        if out is None:
+            out = torch.empty(B * T_max, H * 128, dtype=torch.bfloat16, device=self.device)
+        self._check(self.lib.rs_attention(self.h, qkv.data_ptr(), vt.data_ptr(), vt.stride(0), pos.data_ptr(), bd_bias.data_ptr(),
+                                          n_rel_pad, bias_u.data_ptr(), out.data_ptr(), enc_len.data_ptr(), B, T_max, H,
+                                          w_left, w_right, n_global, self._stream()), "rs_attention")
+        return out
+
+    def conv_dw(self, u: torch.Tensor, w: torch.Tensor, shift: torch.Tensor, enc_len: torch.Tensor, T_max: int) -> torch.Tensor:
+        """u bf16 [B*T_max, d], w f32 [k, d] (BatchNorm folded), shift f32 [d] -> swish(depthwise conv + shift) bf16."""
+        rows, d = u.shape
+        assert u.dtype == torch.bfloat16 and u.is_contiguous() and enc_len.dtype == torch.int32
+        out = torch.empty_like(u)
+        self._check(self.lib.rs_conv_dw(self.h, u.data_ptr(), out.data_ptr(), w.data_ptr(), shift.data_ptr(), enc_len.data_ptr(),
+                                        rows // T_max, T_max, d, w.shape[0], self._stream()), "rs_conv_dw")
+        return out
+
+    def sub_conv0_dw1(self, mel: torch.Tensor, mel_len: torch.Tensor, mel_stats: Optional[torch.Tensor], w0: torch.Tensor,
+                      b0: torch.Tensor, wd: torch.Tensor, bd: torch.Tensor) -> torch.Tensor:
+        """mel f32 [B, F_max, n_mels] (+ (mean, 1 / (std + eps)) [B, n_mels, 2]) -> conv.0 + ReLU + conv.2, bf16 [B, T2, F2, C]."""
+        B, F_max, n_mels = mel.shape
+        C = w0.shape[0]
+        T2, F2 = conv_out_len(conv_out_len(F_max)), conv_out_len(conv_out_len(n_mels))
+        assert mel.dtype == torch.float32 and mel.is_contiguous() and mel_len.dtype == torch.int32
+        out = torch.empty(B, T2, F2, C, dtype=torch.bfloat16, device=self.device)
+        self._check(self.lib.rs_sub_conv0_dw1(self.h, mel.data_ptr(), mel_len.data_ptr(), mel_stats.data_ptr() if mel_stats is not None else None,
+                                              B, F_max, n_mels, C, w0.data_ptr(), b0.data_ptr(), wd.data_ptr(), bd.data_ptr(),
+                                              out.data_ptr(), self._stream()), "rs_sub_conv0_dw1")
+        return out
+
+    def sub_dw(self, x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, mel_len: torch.Tensor, len_shift: int) -> torch.Tensor:
+        """Depthwise 3x3 s2 on channels-last bf16 [B, Tin, Fin, C] -> [B, conv_len(Tin), conv_len(Fin), C]."""
+        B, Tin, Fin, C = x.shape
+        Tout, Fout = conv_out_len(Tin), conv_out_len(Fin)
+        assert x.dtype == torch.bfloat16 and x.is_contiguous() and mel_len.dtype == torch.int32
+        out = torch.empty(B, Tout, Fout, C, dtype=torch.bfloat16, device=self.device)
+        self._check(self.lib.rs_sub_dw(self.h, x.data_ptr(), out.data_ptr(), w.data_ptr(), b.data_ptr(), mel_len.data_ptr(), len_shift,
+                                       B, Tin, Fin, Tout, Fout, C, self._stream()), "rs_sub_dw")
         return out
 
     def enable_stage_timing(self, on: bool = True):
