@@ -1,10 +1,19 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a:  out = epi(A[M,K] * W[N,K]^T)
 //
-//   warpgroup 0     TMA producer   one thread: cp.async.bulk.tensor 2-D tiles (128B swizzle) -> smem ring
+//   warpgroup 0     TMA producer   one thread: cp.async.bulk.tensor 2-D tiles (128B swizzle) -> smem ring; the warpgroup
+//                                  hands most of its registers to the consumers (setmaxnreg)
 //   warpgroups 1,2  consumers      each owns 64 rows of the 128 x BN tile: wgmma.mma_async m64nBNk16 straight from the ring,
 //                                  fp32 accumulators in registers, then the fused epilogue (bias / activation / GLU /
 //                                  residual) staged per warp through shared memory so that global stores cover whole lines;
 //                                  the producer keeps filling the ring with the next tile's operands meanwhile
+//
+// Two instances of the one kernel body:
+//   BN = 256  128 fp32 accumulators per consumer thread (the producer's registers moved over with setmaxnreg); a CTA
+//             pulls 48 KB from L2 per 4.2 MFLOP k-block (85 FLOP/B, against 64 for a 128 x 128 tile).
+//   BN = 64   for launches whose 256-wide tiling would not give every SM a tile or would leave part of its last W tile
+//             empty (the ALSD search's products, single-clip encoder passes, N = 640): more, smaller tiles.
+// Both run the same k16 steps in the same k order with fp32 accumulation and the same epilogue operations, so a row's
+// result does not depend on which instance computed it.
 //
 // Covers every dense contraction of the FastConformer encoder (SURVEY.md App. A.3): FFN W1/W2,
 // fused QKV, attention out-proj, conv pointwise 1/2, the subsampling 1x1 convs and out-linear,
@@ -28,6 +37,7 @@ constexpr int kGemmThreads = 128 + 32 * kConsumerWarps;
 constexpr int kABytes = BM * BK * 2;   // 16 KiB
 constexpr int kStageLd = 40;           // floats per staged row (160 B: 16 B-aligned; the fragment's float2 writes are conflict-free)
 constexpr int kStageBytesPerWarp = 16 * kStageLd * 4;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 
 struct GemmDev {
   const float* bias;
@@ -43,9 +53,10 @@ template <int BN>
 struct GemmCfg {
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = BN == 128 ? 6 : 8;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kConsumerWarps * kStageBytesPerWarp;
-  static_assert(kSmemBytes <= 227 * 1024, "shared memory layout");
+  static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kConsumerWarps * kStageBytesPerWarp;
+  static constexpr int kStages = (227 * 1024 - kFixedBytes) / kStageBytes;   // 4 (BN = 256), 8 (BN = 64)
+  static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
+  static_assert(2 * 8 * kStages <= 256, "barrier area");
 };
 
 // Fused epilogue of one 16-row x 32-column chunk (one consumer warp) whose biased fp32 values sit in the warp's staging
@@ -162,6 +173,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
 
   if (warp < 4) {
     // ------------------------------------------------------------------ TMA producer
+    setmaxnreg_dec<kProducerRegs>();
     if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -177,6 +189,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
     }
   } else {
     // ------------------------------------------------------------------ consumer warpgroups
+    setmaxnreg_inc<kConsumerRegs>();
     const int cw = warp - 4;                                   // consumer warp 0..7
     const int rows0 = (cw >> 2) * 64;                          // the warpgroup's rows of the tile
     float* stage_f = reinterpret_cast<float*>(stage_gen + cw * kStageBytesPerWarp);
@@ -193,7 +206,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
-          if constexpr (BN == 128) wgmma_bf16_ss_n128(d, da + 2u * k, db + 2u * k, (kb | k) != 0 ? 1u : 0u);
+          if constexpr (BN == 256) wgmma_bf16_ss_n256(d, da + 2u * k, db + 2u * k, (kb | k) != 0 ? 1u : 0u);
           else wgmma_bf16_ss_n64(d, da + 2u * k, db + 2u * k, (kb | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
@@ -303,8 +316,10 @@ cudaError_t launch_gemm(const GemmArgs& g, int num_sms, cudaStream_t stream, cha
     snprintf(err, 256, "gemm: RS_EPI_QKV_VT needs out2, split %% 32 == 0, ld2 %% 8 == 0, M %% 8 == 0, ld2 >= M");
     return cudaErrorInvalidValue;
   }
-  // kernel choice depends on N only (never on M): a row's result must not depend on the batch it sits in
-  if (g.N % 128 == 0) return launch_bn<128>(g, num_sms, stream, err);
+  // 256-wide tiles when N fills them and they give every SM a tile, else 64-wide ones on more SMs.  The two instances
+  // compute every element alike, so the choice (which depends on M) cannot make a row's result depend on the batch it
+  // sits in (tests/test_gpu_gemm_cluster.py).
+  if (g.N % 256 == 0 && ((g.M + BM - 1) / BM) * (g.N / 256) >= num_sms) return launch_bn<256>(g, num_sms, stream, err);
   return launch_bn<64>(g, num_sms, stream, err);
 }
 
