@@ -155,6 +155,18 @@ int rs_transcribe_batch_confidence(rs_engine* e, const void* wav_host, int wav_i
                                    int B, int L_max, int32_t* tokens_host, int32_t* frames_host,
                                    int32_t* n_tok_host, int U_max, float alpha, float* stats_host, void* stream);
 
+/* Phrase boosting (context biasing) of the greedy decode.  bonus f32 and next i32, both [n_states, pitch] in device memory
+ * and 16-byte aligned, are the tables of a phrase automaton (reazonspeech_b200/boosting.py builds them): emitting non-blank
+ * token k from state n adds bonus[n][k] to token k's logit before the argmax and moves the utterance to next[n][k] (a value
+ * outside [0, n_states) counts as the root, state 0).  Every utterance starts at the root in every call; blank is never
+ * boosted.  pitch >= vocab_size and a multiple of 4; 1 <= n_states <= RS_MAX_BOOST_STATES; otherwise RS_ERR_INVALID_ARG and
+ * the previous setting stays.  n_states = 0 clears the setting (the pointers are then ignored).  While a table is set, every
+ * greedy entry point (rs_rnnt_greedy, rs_transcribe_device / _batch and their _pcm16 / _confidence forms) decodes with it; the
+ * confidence statistics stay those of the unboosted softmax at the boosted decisions.  The tables stay owned by the caller
+ * and must outlive every call that uses them; the engine keeps only the pointers.  rs_rnnt_alsd ignores them. */
+#define RS_MAX_BOOST_STATES 8192
+int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* next_dev, int n_states, int pitch);
+
 /* ALSD beam search (NeMo BeamRNNTInfer.align_length_sync_decoding, the shipped checkpoint's default strategy; the reference's
  * decode.py is written for its hypotheses, pkg/nemo-asr/src/decode.py:29,38-40,48): enc f32[B,T_max,d_model] + enc_len ->
  * y i32[B, U_cap + 1] (leading blank, then the tokens), step i32[B, U_cap] (alignment step t + u of every token =

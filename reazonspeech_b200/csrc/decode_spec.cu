@@ -35,6 +35,15 @@
 // a = sum e^(alpha (l-m)), ga = sum e^(alpha (l-m)) (l-m), and stores it in the conf ring (one slot per slice).  After the
 // consume step every emission below U_max is merged over the S slices by one warp (emission e: CTA e % G) into
 // stats[b][n] = (log p of the emitted token, sum p log p, sum p^alpha, sum p^alpha log p) over all V + 1 classes.
+//
+// Phrase boosting (kBoost = true; tables built by reazonspeech_b200/boosting.py).  Every utterance carries a state of the
+// phrase automaton, s_state[b], advanced identically by every CTA in the consume step: s_state = next[s_state][token] on
+// every emission (a value outside [0, n_states) becomes the root).  The decision for a (utterance, frame) is the argmax of
+// logit_k + bonus[s_state][k], blank never boosted.  The four frames of a window share the utterance's state, so a pass needs
+// the bonus rows of its <= 8 utterances over the CTA's vocabulary slice: cp.async'd into a shared tile when the pass's
+// rows are fetched (pass 0: under phases L and P) and added to the logits in the argmax epilogue.  With kConf as well, the
+// statistics stay those of the UNBOOSTED softmax at the boosted decision: log p = (l_emit - m) - log s, l_emit = the winner's
+// boosted value (recovered from its ordered bits) - its bonus, which is the raw logit to within one fp32 rounding.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -61,6 +70,9 @@ struct SpecDev {
   float* conf;                // [3][B][kFrames][S][5] softmax tuples of each vocabulary slice, 3-deep ring like best (kConf)
   float* stats;               // [B][U_max][4] (lp, H1, A_alpha, G_alpha) of every stored token (kConf)
   float alpha, alpha_l2;      // alpha and alpha * log2(e) (kConf)
+  const float* boost_bonus;   // [n_states][boost_pitch] bonus of each non-blank token per automaton state (kBoost)
+  const int32_t* boost_next;  // [n_states][boost_pitch] automaton transition on each non-blank token (kBoost)
+  int boost_states, boost_pitch;
   int B, T_max, V, U_max, max_symbols;
   int S, rows_j, units, rows_p;
 };
@@ -148,6 +160,19 @@ __device__ __forceinline__ unsigned long long pack_best(float v, int row) {
   fb = (fb & 0x80000000u) ? ~fb : (fb | 0x80000000u);           // order-preserving
   return (static_cast<unsigned long long>(fb) << 32) | (0xffffffffu - static_cast<unsigned int>(row));   // ties -> lower row
 }
+// the value pack_best ordered (inverse of its bit transform)
+__device__ __forceinline__ float best_value(unsigned long long v) {
+  const unsigned int fb = static_cast<unsigned int>(v >> 32);
+  return __uint_as_float((fb & 0x80000000u) ? (fb & 0x7fffffffu) : ~fb);
+}
+
+// Phrase-boosting tile: one bonus row per utterance of a pass, the CTA's vocabulary slice starting at the 16-byte boundary at or
+// below j0 (<= 3 + 128 + 3 floats copied)
+constexpr int kTileLd = 136;
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // The joint window runs on wgmma.  A = the CTA's W_out rows as IEEE half in 128B-swizzled K-major slabs of 64 columns
 // (88 rows stored per slab; the two warpgroups' m64 instructions cover 128 rows and read on into the next slab / region,
@@ -157,7 +182,7 @@ __device__ __forceinline__ unsigned long long pack_best(float v, int row) {
 // is one m64n64k16 per warpgroup and the two halves of D are added in the epilogue.
 static_assert(kSpThreads == 256, "the joint is issued by two warpgroups");
 
-template <int HJ, int HP, bool kConf>
+template <int HJ, int HP, bool kConf, bool kBoost>
 __global__ void __launch_bounds__(kSpThreads, 1)
 rnnt_greedy_spec_kernel(const SpecDev p) {
   constexpr int KH = HJ / 2;                 // joint k-half staged in shared memory at a time
@@ -214,6 +239,11 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   int* s_cnt = s_act + B;                                                            // [0] n_emit, [1] n_active, [2..2+8) warp counts x2
   int* s_cj = s_cnt + 2 + 2 * kSpWarps;                                              // kConf: window frame of b's stored emission, -1: none
   float* s_conf = reinterpret_cast<float*>(s_cj + B);                                // kConf: [32 rows][kSpWarps][5] per-warp softmax tuples
+  // kBoost: [kPassUtts][kTileLd] bonus tile (16-byte aligned, after the kConf arrays when they exist), automaton state per
+  // utterance, and with kConf the emitted token's unboosted logit per utterance
+  float* s_tile = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kConf ? s_conf + kPassRows * kSpWarps * 5 : reinterpret_cast<float*>(s_cj)) + 15) & ~static_cast<uintptr_t>(15));
+  int* s_state = reinterpret_cast<int*>(s_tile + kPassUtts * kTileLd);
+  float* s_le = reinterpret_cast<float*>(s_state + B);
 
   {
     const uint32_t zero = 0;
@@ -243,6 +273,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     for (int i = tid; i < B * p.units; i += kSpThreads) s_c[i] = 0.f;
     for (int b = tid; b < B; b += kSpThreads) {
       s_t[b] = 0; s_sym[b] = 0; s_n[b] = 0; s_tok[b] = blank; s_len[b] = p.enc_len[b];
+      if constexpr (kBoost) s_state[b] = 0;
     }
     if (tid < 12) s_prof[tid] = 0;
   }
@@ -429,6 +460,16 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
       const bool ok = ai < n_act && s_t[b] + j < s_len[b];
       row_b = ok ? b : -1; row_t = ok ? s_t[b] + j : 0;
     }
+    if constexpr (kBoost) {
+      // bonus rows [a0, min(j1, V)) of the pass's utterances in 16-byte pieces (rows are boost_pitch floats, a multiple of 4;
+      // the blank's column is never read); waited for before the argmax epilogue
+      const int a0 = j0 & ~3, n4 = (min(j1, p.V) - a0 + 3) >> 2;
+      for (int i = tid; i < kPassUtts * n4; i += kSpThreads) {
+        const int u = i / n4, c = i % n4, ai = grp + kGroups * (pass * kPassUtts + u);
+        if (ai < n_act)
+          cp_async16(s_tile + u * kTileLd + 4 * c, p.boost_bonus + static_cast<size_t>(s_state[s_act[ai]]) * p.boost_pitch + a0 + 4 * c);
+      }
+    }
 #pragma unroll
     for (int i = 0; i < PERU; ++i) {
       int c4, rb[kFrames], rt[kFrames];
@@ -535,6 +576,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
           wgmma_wait<0>();
           __syncthreads();                                    // half 0 consumed by both warpgroups: the planes may be rewritten
           write_planes(1);
+          if constexpr (kBoost) cp_async_wait_all();          // the bonus tile: visible to every thread after the barrier
           fence_proxy_async();
           __syncthreads();
           issue_half(1);
@@ -546,13 +588,26 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
             const int rr = (warp >> 2) * 64 + (warp & 3) * 16 + gid;
             const bool v0 = rr < nj, v1 = rr + 8 < nj;
             const float bias0 = s_bout[rr], bias1 = s_bout[rr + 8];
+            // kBoost: column 8j + 2t + e is frame (2t + e) % 4 of the pass's utterance 2j + t / 2, so both e share the bonus of
+            // rows rr, rr + 8; the eight values are read up front (blank, row V, gets none)
+            float bon[4][2];
+            if constexpr (kBoost) {
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const float* tr = s_tile + (2 * j + (tig >> 1)) * kTileLd + (j0 & 3) + rr;
+                bon[j][0] = j0 + rr < p.V ? tr[0] : 0.f;
+                bon[j][1] = j0 + rr + 8 < p.V ? tr[8] : 0.f;
+              }
+            }
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const float l0 = (dj[4 * j + e] + dj[4 * (j + 4) + e]) + bias0, l1 = (dj[4 * j + 2 + e] + dj[4 * (j + 4) + 2 + e]) + bias1;
-                unsigned long long k0 = v0 ? pack_best(l0, j0 + rr) : 0ull;
-                const unsigned long long k1 = v1 ? pack_best(l1, j0 + rr + 8) : 0ull;
+                float s0 = l0, s1 = l1;                       // the scores the argmax ranks
+                if constexpr (kBoost) { s0 += bon[j][0]; s1 += bon[j][1]; }
+                unsigned long long k0 = v0 ? pack_best(s0, j0 + rr) : 0ull;
+                const unsigned long long k1 = v1 ? pack_best(s1, j0 + rr + 8) : 0ull;
                 k0 = k1 > k0 ? k1 : k0;                       // higher logit first, ties -> lower row
 #pragma unroll
                 for (int o = 4; o < 32; o <<= 1) { const unsigned long long ot = __shfl_xor_sync(0xffffffffu, k0, o); k0 = ot > k0 ? ot : k0; }
@@ -617,6 +672,12 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
             p.frames[static_cast<size_t>(b) * p.U_max + n] = t;
           }
           if (kConf && n < p.U_max) cj = j;
+          if constexpr (kBoost) {
+            const size_t at = static_cast<size_t>(s_state[b]) * p.boost_pitch + k;
+            const int nx = __ldg(p.boost_next + at);
+            if constexpr (kConf) if (n < p.U_max) s_le[b] = best_value(v) - __ldg(p.boost_bonus + at);
+            s_state[b] = static_cast<unsigned int>(nx) < static_cast<unsigned int>(p.boost_states) ? nx : 0;
+          }
           s_n[b] = n + 1;
           tok = k;
           if (++sym >= p.max_symbols) { t += 1; sym = 0; }
@@ -650,9 +711,10 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
           c = soft_merge(c, {__ldcg(src + 5 * s), __ldcg(src + 5 * s + 1), __ldcg(src + 5 * s + 2), __ldcg(src + 5 * s + 3), __ldcg(src + 5 * s + 4)}, p.alpha_l2);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) c = soft_merge(c, soft_shfl_xor(c, o), p.alpha_l2);
-        if (lane == 0) {                                      // c is relative to the argmax logit: log p = (l - m) - log s
+        if (lane == 0) {                                      // c is relative to the maximum logit m: log p = (l - m) - log s
           const float log_s = logf(c.s), inv_s = 1.f / c.s, s_ma = expf(-p.alpha * log_s), a_alpha = s_ma * c.a;
-          const float4 st = make_float4(-log_s, c.g * inv_s - log_s, a_alpha, s_ma * c.ga - log_s * a_alpha);
+          const float lp = kBoost ? (s_le[b] - c.m) - log_s : -log_s;   // unboosted, the emitted token is the maximum
+          const float4 st = make_float4(lp, c.g * inv_s - log_s, a_alpha, s_ma * c.ga - log_s * a_alpha);
           __stcg(reinterpret_cast<float4*>(p.stats + (static_cast<size_t>(b) * p.U_max + (s_n[b] - 1)) * 4), st);
         }
       }
@@ -680,21 +742,24 @@ SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms) {
   return w;
 }
 
-template <int HJ, int HP, bool kConf>
+template <int HJ, int HP, bool kConf, bool kBoost>
 static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
-  cudaError_t e = cudaFuncSetAttribute(rnnt_greedy_spec_kernel<HJ, HP, kConf>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  const auto kernel = rnnt_greedy_spec_kernel<HJ, HP, kConf, kBoost>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   int per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rnnt_greedy_spec_kernel<HJ, HP, kConf>, kSpThreads, smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kSpThreads, smem);
   if (e != cudaSuccess) return e;
   if (per_sm < 1) return cudaErrorLaunchOutOfResources;
   void* args[] = {&p};
-  return cudaLaunchCooperativeKernel(reinterpret_cast<void*>(rnnt_greedy_spec_kernel<HJ, HP, kConf>), dim3(grid), dim3(kSpThreads), args, smem, stream);
+  return cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(kSpThreads), args, smem, stream);
 }
 
 template <int HJ, int HP>
 static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
-  return p.stats != nullptr ? launch_sp<HJ, HP, true>(p, grid, smem, stream) : launch_sp<HJ, HP, false>(p, grid, smem, stream);
+  if (p.boost_bonus != nullptr)
+    return p.stats != nullptr ? launch_sp<HJ, HP, true, true>(p, grid, smem, stream) : launch_sp<HJ, HP, false, true>(p, grid, smem, stream);
+  return p.stats != nullptr ? launch_sp<HJ, HP, true, false>(p, grid, smem, stream) : launch_sp<HJ, HP, false, false>(p, grid, smem, stream);
 }
 
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream) {
@@ -719,6 +784,11 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   p.stats = a.stats;
   if (a.stats != nullptr && !(a.alpha > 0.f && a.alpha < INFINITY)) return cudaErrorInvalidValue;
   p.alpha = a.alpha; p.alpha_l2 = a.alpha * kLog2e;
+  p.boost_bonus = a.boost_bonus; p.boost_next = a.boost_next; p.boost_states = a.boost_states; p.boost_pitch = a.boost_pitch;
+  const bool boost = a.boost_bonus != nullptr;
+  if (boost && (a.boost_next == nullptr || a.boost_states < 1 || a.boost_pitch < a.V || (a.boost_pitch & 3) ||
+                ((reinterpret_cast<uintptr_t>(a.boost_bonus) | reinterpret_cast<uintptr_t>(a.boost_next)) & 15u)))
+    return cudaErrorInvalidValue;                                  // the tile is copied in 16-byte pieces
   p.B = a.B; p.T_max = a.T_max; p.V = a.V; p.U_max = a.U_max; p.max_symbols = a.max_symbols;
   p.S = G / kGroups;
   p.rows_j = (a.V + 1 + p.S - 1) / p.S;
@@ -729,7 +799,8 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   if (e != cudaSuccess) return e;
   const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + (kPassRows * kSpWarps + 12) * 8 + static_cast<size_t>(a.B) * 7 * 4 +
                        (2 + 2 * kSpWarps) * 4 + 64 +
-                       (a.stats != nullptr ? static_cast<size_t>(a.B) * 4 + kPassRows * kSpWarps * 5 * 4 : 0);   // kConf: s_cj, s_conf
+                       (a.stats != nullptr ? static_cast<size_t>(a.B) * 4 + kPassRows * kSpWarps * 5 * 4 : 0) +   // kConf: s_cj, s_conf
+                       (boost ? 16 + kPassUtts * kTileLd * 4 + static_cast<size_t>(a.B) * 4 * (a.stats != nullptr ? 2 : 1) : 0);   // kBoost: align, s_tile, s_state (, s_le)
   const size_t w_lp = (static_cast<size_t>(4 * p.units) * (a.Hp + 8) + static_cast<size_t>(p.rows_p) * (a.Hp + 8)) * 2;
   if (p.rows_j > 128) return cudaErrorInvalidValue;
   const size_t rows_a8 = (p.rows_j + 7) & ~7;

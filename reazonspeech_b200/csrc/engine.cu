@@ -78,6 +78,8 @@ struct rs_engine {
   struct { const float *c0w, *c0b, *d1w, *d1b, *p1b, *d2w, *d2b, *p2b, *ob; const void *p1w, *p2w, *ow; } sub;
   std::vector<LayerW> layers;
   struct { const void *enc_w, *out_w, *lstm_w, *pred_w; const float *enc_b, *out_b, *embed, *lstm_b, *pred_b, *gate_tab; } dec;
+  // phrase boosting (rs_set_phrase_boosting): caller-owned device tables used by every greedy decode while set
+  struct { const float* bonus = nullptr; const int32_t* next = nullptr; int n_states = 0, pitch = 0; } boost;
   void* ws = nullptr;
   size_t ws_bytes = 0;
   mutable char err[512] = "";
@@ -413,7 +415,7 @@ int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_
   mark(e, 4, s);
   rs::DecodeArgs da{at<float>(e, p.encp), enc_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w, e->dec.gate_tab, e->dec.pred_w,
                     e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, c.max_symbols,
-                    stats, alpha};
+                    stats, alpha, e->boost.bonus, e->boost.next, e->boost.n_states, e->boost.pitch};
   // One decode kernel for every batch size (windowed, weights-stationary, joint on wgmma: decode_spec.cu): an utterance's
   // logits are accumulated in the same order whether it is decoded alone or inside a batch, so results do not depend on
   // batch composition.
@@ -480,6 +482,22 @@ void rs_engine_destroy(rs_engine* e) {
 }
 
 const char* rs_last_error(const rs_engine* e) { return e ? e->err : g_create_error; }
+
+int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* next_dev, int n_states, int pitch) {
+  if (e == nullptr) return RS_ERR_INVALID_ARG;
+  if (n_states == 0) {
+    e->boost = {};
+    return RS_OK;
+  }
+  if (n_states < 1 || n_states > RS_MAX_BOOST_STATES)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_set_phrase_boosting: n_states=%d outside [1, %d]", n_states, RS_MAX_BOOST_STATES);
+  if (pitch < e->cfg.vocab_size || pitch % 4 != 0)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_set_phrase_boosting: pitch=%d must be >= vocab_size (%d) and a multiple of 4", pitch, e->cfg.vocab_size);
+  if (bonus_dev == nullptr || next_dev == nullptr || ((reinterpret_cast<uintptr_t>(bonus_dev) | reinterpret_cast<uintptr_t>(next_dev)) & 15u))
+    return fail(e, RS_ERR_INVALID_ARG, "rs_set_phrase_boosting: bonus and next must be non-null and 16-byte aligned");
+  e->boost.bonus = bonus_dev; e->boost.next = next_dev; e->boost.n_states = n_states; e->boost.pitch = pitch;
+  return RS_OK;
+}
 
 int rs_workspace_bytes(const rs_engine* e, int B, int L_max, size_t* bytes) {
   if (e == nullptr || bytes == nullptr || B <= 0 || L_max <= 0) return fail(e, RS_ERR_INVALID_ARG, "bad arguments");

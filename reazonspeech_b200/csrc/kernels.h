@@ -82,12 +82,18 @@ struct DecodeArgs {
   int B, T_max, Hj, Hp, V, U_max, max_symbols;
   float* stats = nullptr;     // f32 [B, U_max, 4] (lp, H1, A_alpha, G_alpha) per stored token; nullptr: no confidence statistics
   float alpha = 0.f;          // > 0 and finite when stats is set
+  // phrase boosting (boosting.py): f32 bonus / i32 next [boost_states, boost_pitch], pitch >= V and a multiple of 4, both
+  // 16-byte aligned; nullptr: no boosting
+  const float* boost_bonus = nullptr;
+  const int32_t* boost_next = nullptr;
+  int boost_states = 0, boost_pitch = 0;
 };
 // Byte offsets of the decode workspace's regions and its size (decode_spec.cu describes the regions)
 struct SpecWorkspace { size_t hbuf, rec, ppbuf, counters, prof, best, conf, total; };
 SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms);
 // windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace laid out by rnnt_spec_workspace();
-// a.stats != nullptr selects the instance that also reduces the softmax statistics of every emitted token
+// a.stats != nullptr selects the instance that also reduces the softmax statistics of every emitted token,
+// a.boost_bonus != nullptr the one that adds the phrase-boosting bonus before the argmax
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream);
 
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)

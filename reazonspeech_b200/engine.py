@@ -51,7 +51,7 @@ EXPORTS = [
     "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing", "rs_debug_decode_cycles",
     "rs_enable_kernel_timing", "rs_kernel_timing", "rs_stage_rows",
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
-    "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
+    "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
 ]
 
 
@@ -90,6 +90,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_greedy_confidence.argtypes = [vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
     lib.rs_transcribe_device_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
     lib.rs_transcribe_batch_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
+    lib.rs_set_phrase_boosting.argtypes = [vp, vp, vp, ip, ip]
     lib.rs_rnnt_alsd.argtypes = [vp, vp, vp, ip, ip, ip, C.c_float, ip, ip, vp, vp, vp, vp, ip, vp]
     lib.rs_rnnt_alsd.restype = ip
     lib.rs_resample_mono.argtypes = [vp, vp, ip, vp, ip, ip, ip, vp, ip, ip, ip, ip, ip, vp, ip, vp, vp]
@@ -117,7 +118,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     for fn in ("rs_workspace_bytes", "rs_set_workspace", "rs_mel_frames", "rs_enc_frames", "rs_mel_valid", "rs_enc_valid", "rs_logmel", "rs_encode",
                "rs_rnnt_greedy", "rs_transcribe_device", "rs_transcribe_batch", "rs_transcribe_device_pcm16", "rs_transcribe_batch_pcm16",
                "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
-               "rs_gemm_bf16", "rs_layernorm", "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
+               "rs_set_phrase_boosting", "rs_gemm_bf16", "rs_layernorm", "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
                "rs_enable_stage_timing", "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing"):
         getattr(lib, fn).restype = ip
     _lib = lib
@@ -282,6 +283,7 @@ class Engine:
         self.h = h
         self._ws: Optional[torch.Tensor] = None
         self._ws_key: Tuple[int, int] = (0, 0)
+        self._boost: Optional[Tuple[torch.Tensor, torch.Tensor]] = None
 
     def __del__(self):
         h = getattr(self, "h", None)
@@ -308,6 +310,28 @@ class Engine:
         ptr = (self._ws.data_ptr() + 255) // 256 * 256
         self._check(self.lib.rs_set_workspace(self.h, ptr, n.value), "rs_set_workspace")
         self._ws_key = (B2, L2)
+
+    def set_phrase_boosting(self, bonus, next_state=None):
+        """Phrase boosting of every greedy decode (rs_set_phrase_boosting): ``bonus`` float32 / ``next_state`` int32, both
+        [n_states, pitch] (``boosting.PhraseBoostingTables`` fields; host or device tensors / arrays), or ``None`` to clear.
+        The engine keeps its device copies alive while they are set; replacing or clearing a table first waits for the work
+        queued on this device's current stream, which may still read the old one."""
+        if bonus is None:
+            new = None
+        else:
+            bonus_d = torch.as_tensor(bonus).to(self.device, torch.float32).contiguous()
+            next_d = torch.as_tensor(next_state).to(self.device, torch.int32).contiguous()
+            if bonus_d.dim() != 2 or bonus_d.shape != next_d.shape:
+                raise ValueError(f"bonus and next must be [n_states, pitch] tensors of one shape, got {tuple(bonus_d.shape)} and {tuple(next_d.shape)}")
+            new = (bonus_d, next_d)
+        if self._boost is not None:
+            torch.cuda.current_stream(self.device).synchronize()
+        if new is None:
+            self._check(self.lib.rs_set_phrase_boosting(self.h, None, None, 0, 0), "rs_set_phrase_boosting")
+        else:
+            self._check(self.lib.rs_set_phrase_boosting(self.h, new[0].data_ptr(), new[1].data_ptr(), new[0].shape[0], new[0].shape[1]),
+                        "rs_set_phrase_boosting")
+        self._boost = new
 
     def mel_frames(self, n: int) -> int:
         return self.lib.rs_mel_frames(self.h, n)

@@ -10,9 +10,13 @@ Same contract as the reference's ``reazonspeech-nemo-asr`` entry point (pkg/nemo
   no AUDIO argument    "no audio file specified" + usage on stderr, exit status 1
   unknown option       getopt.GetoptError propagates, as in the reference
 
-One extension: several AUDIO arguments are transcribed as one batch on the GPU (the reference reads exactly one);
+First extension: several AUDIO arguments are transcribed as one batch on the GPU (the reference reads exactly one);
 their segments are written one file after the other through the same writer, every file's times shifted by the total
 duration of the files before it, i.e. the transcript of the files played back to back (subtitle formats need monotonic times).
+Second extension, phrase boosting (reazonspeech_b200/boosting.py): the greedy decode favours hypotheses that spell key phrases
+  --phrases=FILE       UTF-8 text, one phrase per line (blank lines ignored)
+  --phrase-score=L     bonus per phrase token in logit units, L > 0 (default 2.0; alone, without --phrases, it boosts nothing)
+With neither option the output is unchanged.
 Audio decoding: soundfile when installed, scipy for WAV, librosa for compressed containers, see audio.audio_from_path.
 """
 import dataclasses
@@ -23,7 +27,7 @@ from dataclasses import dataclass, field
 from typing import List, Optional
 
 SHORT_OPTS = "ho:"
-LONG_OPTS = ("help", "output=", "to=")
+LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=")
 
 
 @dataclass
@@ -32,6 +36,8 @@ class Options:
     output: Optional[str] = None
     fmt: Optional[str] = None
     audio: List[str] = field(default_factory=list)
+    phrases: Optional[str] = None
+    phrase_score: Optional[float] = None
 
 
 def parse(argv) -> Options:
@@ -45,6 +51,10 @@ def parse(argv) -> Options:
             opt.output = value
         if flag == "--to":
             opt.fmt = value
+        if flag == "--phrases":
+            opt.phrases = value
+        if flag == "--phrase-score":
+            opt.phrase_score = float(value)
     return opt
 
 
@@ -60,7 +70,13 @@ def run(opt: Options) -> None:
     sink = sys.stdout if opt.output is None else open(opt.output, "w")
     warnings.simplefilter("ignore")
     clips = [audio_from_path(path) for path in opt.audio]
-    model = load_model()
+    boosting = None
+    if opt.phrases is not None or opt.phrase_score is not None:
+        from ...boosting import PhraseBoostingConfig, load_phrases
+        boosting = PhraseBoostingConfig(load_phrases(opt.phrases) if opt.phrases is not None else [])
+        if opt.phrase_score is not None:
+            boosting.score = opt.phrase_score
+    model = load_model() if boosting is None else load_model(boosting=boosting)
     results = transcribe_batch(model, clips) if len(clips) > 1 else [transcribe(model, clips[0])]
     with sink:
         out = get_writer(sink, opt.fmt)

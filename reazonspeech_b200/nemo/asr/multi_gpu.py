@@ -33,6 +33,15 @@ class MultiGpuRnntModel:
         self.tokenizer = self.replicas[0].tokenizer
         self.max_batch = self.replicas[0].max_batch
         self.confidence = getattr(self.replicas[0], "confidence", None)
+        self.boosting = getattr(self.replicas[0], "boosting", None)
+
+    def set_phrase_boosting(self, boosting) -> None:
+        """``B200RnntModel.set_phrase_boosting`` on every replica: the tables are built once and uploaded once per device."""
+        from .transcribe import boosting_tables
+        tables = boosting_tables(self, boosting)
+        for r in self.replicas:
+            r.set_phrase_boosting_tables(tables, boosting)
+        self.boosting = boosting
 
     @property
     def devices(self) -> List[str]:

@@ -18,6 +18,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
+from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables
 from ...config import ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
 from ...engine import Engine
@@ -128,7 +129,7 @@ class B200RnntModel:
     """Engine + tokenizer behind NeMo's model surface."""
 
     def __init__(self, engine: Engine, tokenizer, max_batch: int = 64, decoding: str = "greedy", beam_size: int = 4,
-                 confidence: Optional[ConfidenceConfig] = None):
+                 confidence: Optional[ConfidenceConfig] = None, boosting: Optional[PhraseBoostingConfig] = None):
         self.engine = engine
         self.cfg = engine.cfg
         self.tokenizer = tokenizer
@@ -139,6 +140,19 @@ class B200RnntModel:
         self.confidence = confidence.validate() if confidence is not None else None
         pin = torch.cuda.is_available()
         self._staging = (HostStaging(pin), HostStaging(pin))      # double buffer: stage batch k+1 while batch k runs
+        self.boosting: Optional[PhraseBoostingConfig] = None
+        if boosting is not None:
+            self.set_phrase_boosting(boosting)
+
+    def set_phrase_boosting(self, boosting: Optional[PhraseBoostingConfig]) -> None:
+        """Boost the phrases of ``boosting`` in every following greedy decode (boosting.py), or stop with None.  Call it
+        between calls, not while one is running."""
+        self.set_phrase_boosting_tables(boosting_tables(self, boosting), boosting)
+
+    def set_phrase_boosting_tables(self, tables: Optional[PhraseBoostingTables], boosting: Optional[PhraseBoostingConfig]) -> None:
+        """Upload tables already built from ``boosting`` (the multi-GPU model builds them once for all replicas)."""
+        self.engine.set_phrase_boosting(None if tables is None else tables.bonus, None if tables is None else tables.next)
+        self.boosting = boosting
 
     # -- token-level batched path
     def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
@@ -255,6 +269,15 @@ class B200RnntModel:
         return [self.tokenizer.ids_to_text(h.y_sequence.tolist()[1:]) for h in out]
 
 
+def boosting_tables(model, boosting: Optional[PhraseBoostingConfig]) -> Optional[PhraseBoostingTables]:
+    """Validated tables of ``boosting`` for ``model``'s vocabulary and tokenizer (None: boosting off)."""
+    if boosting is None:
+        return None
+    if getattr(model, "decoding", "greedy") != "greedy":
+        raise ValueError("phrase boosting is applied by the greedy decode only (not by ALSD beam search)")
+    return build_tables(boosting, model.cfg.vocab_size, model.tokenizer)
+
+
 def _items(done, B: int):
     """Host outputs of one engine call -> per utterance (tokens, frames), or (tokens, frames, stats) with the statistics."""
     tokens, frames, ntok = done[:3]
@@ -277,7 +300,8 @@ def _find_checkpoint() -> Optional[str]:
 
 def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Optional[bool] = None,
                config: Optional[ModelConfig] = None, seed: int = 0, max_batch: int = 64, devices: Optional[Sequence] = None,
-               decoding: str = "greedy", beam_size: int = 4, confidence: Optional[ConfidenceConfig] = None):
+               decoding: str = "greedy", beam_size: int = 4, confidence: Optional[ConfidenceConfig] = None,
+               boosting: Optional[PhraseBoostingConfig] = None):
     """Load the ReazonSpeech FastConformer-RNNT onto a B200.
 
     ``device``: None / "cuda" / "cuda:N" as in the reference (transcribe.py:9-22, eval.py:26).
@@ -289,11 +313,17 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     $REAZONSPEECH_NEMO_CHECKPOINT or the local Hugging Face cache of reazonspeech-nemo-v2.
     With ``synthetic=True`` (or $REAZONSPEECH_B200_SYNTHETIC=1) seeded random weights of the same
     architecture are used instead -- the only option offline.  ``confidence``: a ``ConfidenceConfig`` turns on token / word
-    confidence and log-probability scores of the greedy decode (``confidence.py``); not available with ``decoding="alsd"``."""
+    confidence and log-probability scores of the greedy decode (``confidence.py``); not available with ``decoding="alsd"``.
+    ``boosting``: a ``PhraseBoostingConfig`` boosts its key phrases in the greedy decode (``boosting.py``); change or clear
+    them later with ``model.set_phrase_boosting``; not available with ``decoding="alsd"``."""
     if confidence is not None:
         if decoding == "alsd":
             raise ValueError("confidence is computed by the greedy decode only (NeMo offers none for beam search)")
         confidence.validate()
+    if boosting is not None:
+        if decoding == "alsd":
+            raise ValueError("phrase boosting is applied by the greedy decode only (not by ALSD beam search)")
+        boosting.validate()
     if device is None:
         device = "cuda"
     if str(device).startswith("cpu"):
@@ -320,7 +350,7 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
         raise ValueError(f"decoding must be 'greedy' or 'alsd', got {decoding!r}")
     if devices is None:
         return B200RnntModel(Engine(cfg, sd, str(device), alsd=decoding == "alsd"), tokenizer, max_batch=max_batch, decoding=decoding, beam_size=beam_size,
-                             confidence=confidence)
+                             confidence=confidence, boosting=boosting)
     if decoding != "greedy":
         raise ValueError("the one-process multi-GPU model decodes greedily; load one model per device for beam search")
     names = [d if isinstance(d, str) else f"cuda:{int(d)}" for d in devices]
@@ -329,8 +359,11 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     from ...engine import pack_weights
     from .multi_gpu import MultiGpuRnntModel
     packed = pack_weights(sd, cfg)                                   # repacked once, uploaded once per device
-    return MultiGpuRnntModel([B200RnntModel(Engine(cfg, None, n, packed=packed), tokenizer, max_batch=max_batch, confidence=confidence)
-                              for n in names])
+    model = MultiGpuRnntModel([B200RnntModel(Engine(cfg, None, n, packed=packed), tokenizer, max_batch=max_batch, confidence=confidence)
+                               for n in names])
+    if boosting is not None:
+        model.set_phrase_boosting(boosting)
+    return model
 
 
 def _prepare(audio: AudioData) -> np.ndarray:

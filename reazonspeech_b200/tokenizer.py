@@ -5,7 +5,13 @@ makes: pkg/nemo-asr/src/decode.py:41,47).
 ``PieceTableTokenizer`` is the stand-in used with synthetic weights: a deterministic table of
 3000 pieces decoded with SentencePiece's rules (concatenate pieces, U+2581 -> space, drop the
 leading space) so a bare U+2581 decodes to the empty string exactly like the real model does
-(which is why decode.py:51-53 filters empty tokens)."""
+(which is why decode.py:51-53 filters empty tokens).
+
+``text_to_ids`` (phrase boosting's tokenisation, boosting.py) segments a phrase ON ITS OWN, with the word-boundary piece that
+SentencePiece puts in front of a text dropped when it stands alone: a phrase inside a Japanese sentence carries no word
+boundary.  Known limitation: a phrase's segmentation alone may differ from its segmentation inside the sentences the model
+transcribes, and then boosting the phrase's ids favours a spelling the model would not produce; pass token-id sequences
+where that matters."""
 from __future__ import annotations
 
 from typing import Iterable, List, Sequence
@@ -27,6 +33,26 @@ class PieceTableTokenizer:
 
     def ids_to_pieces(self, ids: Iterable[int]) -> List[str]:
         return [self.pieces[int(i)] for i in ids]
+
+    def text_to_ids(self, text: str) -> List[int]:
+        """Longest match over the pieces (SentencePiece's space handling: a leading boundary, spaces -> U+2581), a leading lone
+        U+2581 piece dropped.  A character no piece covers raises ValueError."""
+        if not hasattr(self, "_index"):
+            self._index = {}
+            for i, piece in enumerate(self.pieces):
+                self._index.setdefault(piece, i)
+            self._longest = max((len(piece) for piece in self.pieces), default=1)
+        s = WORD_BOUNDARY + text.replace(" ", WORD_BOUNDARY)
+        ids, i = [], 0
+        while i < len(s):
+            for n in range(min(self._longest, len(s) - i), 0, -1):
+                k = self._index.get(s[i:i + n])
+                if k is not None:
+                    ids.append(k); i += n
+                    break
+            else:
+                raise ValueError(f"{text!r}: no piece covers {s[i]!r}")
+        return _drop_lone_boundary(ids, self.pieces[ids[0]] if ids else "")
 
 
 def synthetic_pieces(vocab_size: int) -> List[str]:
@@ -56,3 +82,12 @@ class SentencePieceTokenizer:
 
     def ids_to_pieces(self, ids: Iterable[int]) -> List[str]:
         return [self.sp.id_to_piece(int(i)) for i in ids]
+
+    def text_to_ids(self, text: str) -> List[int]:
+        """SentencePiece's ``encode``, a leading lone U+2581 piece dropped."""
+        ids = [int(i) for i in self.sp.encode(text)]
+        return _drop_lone_boundary(ids, self.sp.id_to_piece(ids[0]) if ids else "")
+
+
+def _drop_lone_boundary(ids: List[int], first_piece: str) -> List[int]:
+    return ids[1:] if first_piece == WORD_BOUNDARY else ids
