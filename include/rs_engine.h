@@ -69,8 +69,12 @@ typedef enum rs_epilogue {
   RS_EPI_BIAS_RELU_BF16 = 1,  /* out_bf16[M,N]   = relu(acc + bias)                            */
   RS_EPI_BIAS_SWISH_BF16 = 2, /* out_bf16[M,N]   = swish(acc + bias)                           */
   RS_EPI_BIAS_GLU_BF16 = 3,   /* out_bf16[M,N/2] = a * sigmoid(g); W rows interleaved 16/16    */
-  RS_EPI_RESID_F32 = 4,       /* out_f32[M,N]    = resid + alpha * (acc + bias)  (out may alias resid: each element is
-                                 read and written by one lane)                                                        */
+  RS_EPI_RESID_F32 = 4,       /* out_f32[M,N]    = resid + alpha * (acc + bias), added into out in L2 by a TMA f32
+                                 reduction (out may alias resid; a separate resid is first copied to out on the same
+                                 stream).  Rounded twice, fl(fl(alpha * s) + resid) with s = fl(acc + bias): bit-equal
+                                 to resid + RS_EPI_BIAS_F32(alpha) computed in fp32, and to a fused multiply-add
+                                 whenever alpha is a power of two.  Subnormal residuals and sums are kept, not
+                                 flushed to zero.                                                                     */
   RS_EPI_BIAS_F32 = 5,        /* out_f32[M,N]    = alpha * (acc + bias)                        */
   RS_EPI_BIAS_F16 = 6,        /* out_f16[M,N]    = acc + bias  (IEEE half)                          */
   RS_EPI_QKV_VT = 7           /* fused QKV projection: columns [0, split) -> out_bf16[M, ldo] as RS_EPI_BIAS_BF16,

@@ -112,6 +112,44 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* desc,
       : "memory");
 }
 
+// 2-D tiled store / element-wise f32 add of a shared-memory box into global memory (rows and columns outside the map
+// are not written), committed to the issuing thread's bulk async-group.  Before the source buffer is rewritten, the
+// issuing thread waits with bulk_wait_read; before the CTA exits, with bulk_wait.
+__device__ __forceinline__ void tma_store_2d(const void* desc, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(desc), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_reduce_add_2d(const void* desc, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(desc), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// At most N of this thread's committed bulk groups still read shared memory.
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// At most N of this thread's committed bulk groups are incomplete.
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// ---------------------------------------------------------------- cp.async (16 B, L2 only)
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// ---------------------------------------------------------------- stmatrix
+// Four 8 x 8 b16 matrices; register k holds, as an mma accumulator fragment does, (row lane / 4, columns 2 (lane % 4), +1)
+// of matrix k, and lanes 8k..8k+7 give the shared addresses of its eight rows.  _trans stores each matrix transposed:
+// row i at the address of lane 8k + i holds column i.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+
 // Hand registers between the warpgroups of a warp-specialised kernel (all threads of the warpgroup execute it).
 template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }

@@ -169,10 +169,6 @@ __device__ __forceinline__ float best_value(unsigned long long v) {
 // Phrase-boosting tile: one bonus row per utterance of a pass, the CTA's vocabulary slice starting at the 16-byte boundary at or
 // below j0 (<= 3 + 128 + 3 floats copied)
 constexpr int kTileLd = 136;
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // The joint window runs on wgmma.  A = the CTA's W_out rows as IEEE half in 128B-swizzled K-major slabs of 64 columns
 // (88 rows stored per slab; the two warpgroups' m64 instructions cover 128 rows and read on into the next slab / region,

@@ -4,8 +4,10 @@
 //                                  hands most of its registers to the consumers (setmaxnreg)
 //   warpgroups 1,2  consumers      each owns 64 rows of the 128 x BN tile: wgmma.mma_async m64nBNk16 straight from the ring,
 //                                  fp32 accumulators in registers, then the fused epilogue (bias / activation / GLU /
-//                                  residual) staged per warp through shared memory so that global stores cover whole lines;
-//                                  the producer keeps filling the ring with the next tile's operands meanwhile
+//                                  V^T) in registers, written as 64-row subtiles into swizzled shared buffers from which
+//                                  one thread issues TMA stores (the residual: a TMA f32 add into out, done in L2).  The
+//                                  stores drain while the warpgroup runs the next tile's main loop; the tile's bias slice
+//                                  arrives by cp.async during that loop.  Rows past M are clipped by the tensor maps.
 //
 // Two instances of the one kernel body:
 //   BN = 256  128 fp32 accumulators per consumer thread (the producer's registers moved over with setmaxnreg); a CTA
@@ -35,126 +37,51 @@ constexpr int BK = 64;                 // 64 bf16 = 128 B = one swizzle atom row
 constexpr int kConsumerWarps = 8;      // two warpgroups
 constexpr int kGemmThreads = 128 + 32 * kConsumerWarps;
 constexpr int kABytes = BM * BK * 2;   // 16 KiB
-constexpr int kStageLd = 40;           // floats per staged row (160 B: 16 B-aligned; the fragment's float2 writes are conflict-free)
-constexpr int kStageBytesPerWarp = 16 * kStageLd * 4;
+// Epilogue subtile of one consumer warpgroup: its 64 rows x 64 B (32 bf16 / f16 or 16 f32 columns, 64 B swizzle), or for
+// V^T 32 head dims x 64 frames (128 B swizzle).  Three buffers per warpgroup: one is written while the stores of the other
+// two drain.
+constexpr int kEpiBufs = 3, kEpiBufBytes = 4096;
+constexpr int kBiasBytes = 256 * 4;    // the tile's bias slice, one copy per warpgroup
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 
 struct GemmDev {
   const float* bias;
-  const float* resid;
-  void* out;
   int M, N, K;
   int epilogue;
   float alpha;
-  int ldo;              // output (and residual) row stride in elements
-  void* out2; int split, ld2;    // RS_EPI_QKV_VT
+  int split;            // RS_EPI_QKV_VT
 };
 template <int BN>
 struct GemmCfg {
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kConsumerWarps * kStageBytesPerWarp;
+  static constexpr int kEpiBytes = 2 * (kEpiBufs * kEpiBufBytes + kBiasBytes);
+  static constexpr int kFixedBytes = 1024 /*align slack*/ + 256 /*barriers*/ + kEpiBytes;
   static constexpr int kStages = (227 * 1024 - kFixedBytes) / kStageBytes;   // 4 (BN = 256), 8 (BN = 64)
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
   static_assert(2 * 8 * kStages <= 256, "barrier area");
+  static_assert(kStageBytes % 1024 == 0, "epilogue buffers need the 1024 B alignment of the 128 B swizzle");
 };
 
-// Fused epilogue of one 16-row x 32-column chunk (one consumer warp) whose biased fp32 values sit in the warp's staging
-// buffer: activation / GLU / residual, conversion, store.  The accumulator fragment gives a lane two columns of two rows;
-// storing that directly would write 8- or 4-byte pieces of 16 different lines per instruction, so the chunk is re-read
-// from the staging buffer in an ownership where one instruction covers whole rows of the chunk.
-// EG: epilogue group compiled into a kernel instance -- 0: the common epilogues, 1: RS_EPI_QKV_VT.
-template <int EG>
-__device__ __forceinline__ void epilogue_store(const GemmDev& p, const float* stage, int tile_row0, int lane, int col0) {
-  int epi = p.epilogue;
-  if constexpr (EG == 1) {
-    if (col0 < p.split) {
-      epi = RS_EPI_BIAS_BF16;                                  // q | k columns: plain row-major bf16
-    } else {
-      // V columns: out2[col - split][row] = bf16(v).  Lane = head dim; its 16 frames are 32 contiguous bytes of out2.
-      uint32_t w[8];
-#pragma unroll
-      for (int r = 0; r < 8; ++r) w[r] = pack_bf16x2(stage[(2 * r) * kStageLd + lane], stage[(2 * r + 1) * kStageLd + lane]);
-      __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out2) + static_cast<size_t>(col0 - p.split + lane) * p.ld2 + tile_row0;
-      // M is a multiple of 8 (checked at launch): frames beyond it belong to another row range of the same buffer
-      if (tile_row0 < p.M) *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
-      if (tile_row0 + 8 < p.M) *reinterpret_cast<uint4*>(dst + 8) = make_uint4(w[4], w[5], w[6], w[7]);
-      return;
-    }
-  }
-  switch (epi) {
-    case RS_EPI_BIAS_F16:
-    case RS_EPI_BIAS_BF16:
-    case RS_EPI_BIAS_RELU_BF16:
-    case RS_EPI_BIAS_SWISH_BF16: {
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {                            // 8 rows x 64 B per instruction
-        const int rl = i * 8 + (lane >> 2), c8 = (lane & 3) * 8;
-        const int row = tile_row0 + rl;
-        const float4 a = *reinterpret_cast<const float4*>(stage + rl * kStageLd + c8), b = *reinterpret_cast<const float4*>(stage + rl * kStageLd + c8 + 4);
-        float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        if (epi == RS_EPI_BIAS_RELU_BF16) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.0f);
-        } else if (epi == RS_EPI_BIAS_SWISH_BF16) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = swishf_fast(v[j]);
-        }
-        const uint4 o = epi == RS_EPI_BIAS_F16
-                            ? make_uint4(pack_f16x2(v[0], v[1]), pack_f16x2(v[2], v[3]), pack_f16x2(v[4], v[5]), pack_f16x2(v[6], v[7]))
-                            : make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-        if (row < p.M)       // __half and __nv_bfloat16 are both two bytes: one address computation
-          *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + static_cast<size_t>(row) * p.ldo + col0 + c8) = o;
-      }
-      break;
-    }
-    case RS_EPI_BIAS_GLU_BF16: {
-      // columns [0,16) of the chunk are values, [16,32) the matching gates (weights interleaved at pack time)
-      const int rl = lane >> 1, c8 = (lane & 1) * 8;           // 16 rows x 32 B in one instruction
-      const int row = tile_row0 + rl;
-      float g[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) g[j] = stage[rl * kStageLd + c8 + j] * sigmoidf_fast(stage[rl * kStageLd + 16 + c8 + j]);
-      if (row < p.M)
-        *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out) + static_cast<size_t>(row) * p.ldo + col0 / 2 + c8) =
-            make_uint4(pack_bf16x2(g[0], g[1]), pack_bf16x2(g[2], g[3]), pack_bf16x2(g[4], g[5]), pack_bf16x2(g[6], g[7]));
-      break;
-    }
-    default: {  // RS_EPI_RESID_F32 / RS_EPI_BIAS_F32
-      const bool add = p.epilogue == RS_EPI_RESID_F32;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {                            // 4 rows x 128 B per instruction
-        const int rl = i * 4 + (lane >> 3), cw = (lane & 7) * 4;
-        const int row = tile_row0 + rl;
-        if (row < p.M) {
-          const size_t off = static_cast<size_t>(row) * p.ldo + col0 + cw;
-          float4 a = *reinterpret_cast<const float4*>(stage + rl * kStageLd + cw);
-          a.x *= p.alpha; a.y *= p.alpha; a.z *= p.alpha; a.w *= p.alpha;
-          if (add) {                                           // out may be resid (in place): each element is read and written by this lane only
-            const float4 r = *reinterpret_cast<const float4*>(p.resid + off);
-            a.x += r.x; a.y += r.y; a.z += r.z; a.w += r.w;
-          }
-          *reinterpret_cast<float4*>(static_cast<float*>(p.out) + off) = a;
-        }
-      }
-      break;
-    }
-  }
-}
+// Byte offset of 16-byte group `chunk` of row `row` in a 64 B-pitch buffer with the tensor map's 64 B swizzle
+// (address bits [4,6) ^= bits [7,9)): the eight rows a stmatrix matrix or a half-warp's f32 stores touch land in distinct banks.
+__device__ __forceinline__ uint32_t sw64(int row, int chunk) { return static_cast<uint32_t>(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4)); }
 
 template <int BN, int EG>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const GemmDev p) {
+gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                    const __grid_constant__ CUtensorMap tm_out, const __grid_constant__ CUtensorMap tm_out2, const GemmDev p) {
   using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled operand tiles need 1024 B alignment.
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + Cfg::kStages * Cfg::kStageBytes;
+  const uint32_t epi_base = smem_base + Cfg::kStages * Cfg::kStageBytes;   // 2 x 3 subtile buffers, then 2 bias slices
+  const uint32_t bar_base = epi_base + Cfg::kEpiBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (Cfg::kStages + s); };
-  uint8_t* stage_gen = smem_raw + ((bar_base + 256u) - smem_u32(smem_raw));   // generic pointer to the staging area
   auto smem_a = [&](int s) { return smem_base + s * Cfg::kStageBytes; };
   auto smem_b = [&](int s) { return smem_base + s * Cfg::kStageBytes + kABytes; };
+  auto smem_gen = [&](uint32_t addr) { return smem_raw + (addr - smem_u32(smem_raw)); };
 
   const int warp = warp_id_uniform();
   const int lane = lane_id();
@@ -166,6 +93,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
+    tma_prefetch_desc(&tm_out);
+    if constexpr (EG == 1) tma_prefetch_desc(&tm_out2);
     for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
     fence_barrier_init();
   }
@@ -191,12 +120,37 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
     // ------------------------------------------------------------------ consumer warpgroups
     setmaxnreg_inc<kConsumerRegs>();
     const int cw = warp - 4;                                   // consumer warp 0..7
-    const int rows0 = (cw >> 2) * 64;                          // the warpgroup's rows of the tile
-    float* stage_f = reinterpret_cast<float*>(stage_gen + cw * kStageBytesPerWarp);
+    const int wg = cw >> 2, wq = cw & 3;                       // warpgroup, warp within it
+    const int rows0 = wg * 64;                                 // the warpgroup's rows of the tile
+    const int tw = threadIdx.x & 127;                          // thread within the warpgroup; 0 issues its TMA stores
+    const uint32_t buf0 = epi_base + wg * kEpiBufs * kEpiBufBytes;
+    float* bias_s = reinterpret_cast<float*>(smem_gen(epi_base + 2 * kEpiBufs * kEpiBufBytes + wg * kBiasBytes));
     const int g = lane >> 2, t = lane & 3;
+    const int mi = lane >> 3, mr = lane & 7;                   // the stmatrix matrix and row this lane addresses
+    int nbuf = 0;                                              // the buffer the next subtile is written into
+    auto buf = [&]() { return buf0 + nbuf * kEpiBufBytes; };
+    // Hand the written buffer to one TMA store (or f32 add).  Once the barrier is passed, every store but the last has
+    // finished reading shared memory, so the buffer after this one is free for the next subtile.
+    auto flush = [&](const CUtensorMap* map, int c0, int c1, bool reduce) {
+      fence_proxy_async();
+      if (tw == 0) bulk_wait_read<kEpiBufs - 2>();
+      named_bar_sync(1 + wg, 128);
+      if (tw == 0) {
+        if (reduce) tma_reduce_add_2d(map, buf(), c0, c1);
+        else tma_store_2d(map, buf(), c0, c1);
+        bulk_commit();
+      }
+      nbuf = nbuf == kEpiBufs - 1 ? 0 : nbuf + 1;
+    };
+
     int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
+      // The tile's bias slice lands during the main loop.  The previous epilogue's last barrier ordered its reads before this.
+      if (4 * tw < min(BN, p.N - n0)) {
+        if (p.bias != nullptr) cp_async16(bias_s + 4 * tw, p.bias + n0 + 4 * tw);
+        else *reinterpret_cast<float4*>(bias_s + 4 * tw) = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
       float d[BN / 2];
       int prev = -1;
       for (int kb = 0; kb < num_k; ++kb) {
@@ -217,25 +171,87 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_const
       }
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(empty_bar(prev));
-      // ---- epilogue: 32-column chunks of the warp's 16 rows
-      const int tile_row0 = m0 + rows0 + (cw & 3) * 16;
+      cp_async_wait_all();
+      named_bar_sync(1 + wg, 128);                             // every thread's share of the bias slice has landed
+
+      // ---- epilogue: 32-column chunks of the warpgroup's 64 rows, in registers, then through the buffers to TMA
+      const int row_g = m0 + rows0;
 #pragma unroll
       for (int c = 0; c < BN / 32; ++c) {
         const int col0 = n0 + c * 32;
-        if (col0 < p.N && tile_row0 < p.M) {                   // warp-uniform
+        if (col0 < p.N) {                                      // warpgroup-uniform
+          // v[j][h][x]: row 16 wq + g + 8h of the warpgroup, column 32c + 8j + 2t + x of the tile, bias added
+          float v[4][2][2];
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const int col = 8 * j + 2 * t;
-            const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + col0 + col)) : make_float2(0.f, 0.f);
-            *reinterpret_cast<float2*>(stage_f + g * kStageLd + col) = make_float2(d[c * 16 + j * 4] + b.x, d[c * 16 + j * 4 + 1] + b.y);
-            *reinterpret_cast<float2*>(stage_f + (g + 8) * kStageLd + col) = make_float2(d[c * 16 + j * 4 + 2] + b.x, d[c * 16 + j * 4 + 3] + b.y);
+            const float2 b = *reinterpret_cast<const float2*>(bias_s + 32 * c + 8 * j + 2 * t);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) { v[j][h][0] = d[16 * c + 4 * j + 2 * h] + b.x; v[j][h][1] = d[16 * c + 4 * j + 2 * h + 1] + b.y; }
           }
-          __syncwarp();
-          epilogue_store<EG>(p, stage_f, tile_row0, lane, col0);
-          __syncwarp();                                        // staging buffer reusable
+          const int epi = EG == 1 ? RS_EPI_QKV_VT : p.epilogue;
+          if (EG == 1 && col0 >= p.split) {
+            // V columns -> out2[col - split][row]: each 8 x 8 block stored transposed; buffer row = head dim (64 frames,
+            // 128 B, 128 B swizzle), this warp's 16 frames are its 16-byte groups 2 wq and 2 wq + 1.
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+              const int dim = 8 * (2 * q + (mi >> 1)) + mr;
+              stmatrix_x4_trans(buf() + dim * 128 + (((2 * wq + (mi & 1)) ^ mr) << 4),
+                                pack_bf16x2(v[2 * q][0][0], v[2 * q][0][1]), pack_bf16x2(v[2 * q][1][0], v[2 * q][1][1]),
+                                pack_bf16x2(v[2 * q + 1][0][0], v[2 * q + 1][0][1]), pack_bf16x2(v[2 * q + 1][1][0], v[2 * q + 1][1][1]));
+            }
+            flush(&tm_out2, row_g, col0 - p.split, false);
+          } else if (epi == RS_EPI_BIAS_GLU_BF16) {
+            // columns [0,16) of the chunk are values, [16,32) the matching gates (weights interleaved at pack time); two
+            // chunks make one 32-column output subtile
+            uint32_t r[2][2];
+#pragma unroll
+            for (int j = 0; j < 2; ++j)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                r[j][h] = pack_bf16x2(v[j][h][0] * sigmoidf_fast(v[j + 2][h][0]), v[j][h][1] * sigmoidf_fast(v[j + 2][h][1]));
+            stmatrix_x4(buf() + sw64(16 * wq + 8 * (mi & 1) + mr, 2 * (c & 1) + (mi >> 1)), r[0][0], r[0][1], r[1][0], r[1][1]);
+            if ((c & 1) || col0 + 32 >= p.N) flush(&tm_out, (col0 & ~63) / 2, row_g, false);
+          } else if (epi == RS_EPI_BIAS_F32 || epi == RS_EPI_RESID_F32) {
+            // alpha (acc + bias) as two 16-column subtiles.  Lanes with bit 1 of g set store their column pairs in the other
+            // order, so that each half-warp's 8-byte stores cover all 32 banks.
+            const bool swp = (g >> 1) & 1;
+#pragma unroll
+            for (int s = 0; s < 2; ++s) {
+#pragma unroll
+              for (int k = 0; k < 2; ++k) {
+                const int jl = k ^ static_cast<int>(swp);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int row = 16 * wq + g + 8 * h;
+                  const float a0 = jl ? v[2 * s + 1][h][0] : v[2 * s][h][0], a1 = jl ? v[2 * s + 1][h][1] : v[2 * s][h][1];
+                  *reinterpret_cast<float2*>(smem_gen(buf() + sw64(row, 2 * jl + (t >> 1)) + 8 * (t & 1))) =
+                      make_float2(a0 * p.alpha, a1 * p.alpha);
+                }
+              }
+              flush(&tm_out, col0 + 16 * s, row_g, epi == RS_EPI_RESID_F32);
+            }
+          } else {
+            // bf16 / f16: q | k columns of RS_EPI_QKV_VT, RS_EPI_BIAS_BF16 / RELU / SWISH / F16
+            uint32_t r[4][2];
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float x0 = v[j][h][0], x1 = v[j][h][1];
+                if (epi == RS_EPI_BIAS_RELU_BF16) { x0 = fmaxf(x0, 0.0f); x1 = fmaxf(x1, 0.0f); }
+                else if (epi == RS_EPI_BIAS_SWISH_BF16) { x0 = swishf_fast(x0); x1 = swishf_fast(x1); }
+                r[j][h] = epi == RS_EPI_BIAS_F16 ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
+              }
+#pragma unroll
+            for (int q = 0; q < 2; ++q)
+              stmatrix_x4(buf() + sw64(16 * wq + 8 * (mi & 1) + mr, 2 * q + (mi >> 1)),
+                          r[2 * q][0], r[2 * q][1], r[2 * q + 1][0], r[2 * q + 1][1]);
+            flush(&tm_out, col0, row_g, false);
+          }
         }
       }
     }
+    if (tw == 0) bulk_wait<0>();
   }
 }
 
@@ -256,18 +272,23 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-bool make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, char* err) {
+// 2-D map over a row-major [rows, cols] array (row pitch ld elements of esize bytes) with a box_rows x box_cols box.
+static bool make_tmap_2d(CUtensorMap* m, CUtensorMapDataType dtype, int esize, const void* ptr, uint64_t rows, uint64_t cols,
+                         uint64_t ld, uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle swizzle, char* err) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) { snprintf(err, 256, "cuTensorMapEncodeTiled entry point unavailable"); return false; }
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), box_rows};
+  cuuint64_t strides[1] = {ld * esize};
+  cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = fn(m, dtype, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { snprintf(err, 256, "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu", (int)r, (unsigned long long)rows, (unsigned long long)cols); return false; }
   return true;
+}
+
+bool make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, char* err) {
+  return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, rows, cols, ld, BK, box_rows, CU_TENSOR_MAP_SWIZZLE_128B, err);
 }
 
 inline int epilogue_group(int epilogue) { return epilogue == RS_EPI_QKV_VT ? 1 : 0; }
@@ -281,14 +302,24 @@ static cudaError_t launch_bn_eg(const GemmArgs& g, int num_sms, cudaStream_t str
     if (e != cudaSuccess) { snprintf(err, 256, "cudaFuncSetAttribute(smem=%d): %s", Cfg::kSmemBytes, cudaGetErrorString(e)); return e; }
     attr_once.set();
   }
-  CUtensorMap tm_a, tm_b;
-  const int ldo = g.epilogue == RS_EPI_BIAS_GLU_BF16 ? g.N / 2 : g.N;
+  CUtensorMap tm_a, tm_b, tm_out, tm_out2;
   if (!make_tmap_bf16(&tm_a, g.a, g.M, g.K, g.K, BM, err)) return cudaErrorInvalidValue;
   if (!make_tmap_bf16(&tm_b, g.w, g.N, g.K, g.K, BN, err)) return cudaErrorInvalidValue;
-  GemmDev p{g.bias, g.resid, g.out, g.M, g.N, g.K, g.epilogue, g.alpha, ldo, g.out2, g.split, g.ld2};
+  // Output: 64-row subtiles of 64 B (16 f32 or 32 two-byte columns); the GLU writes N / 2 columns.
+  const bool f32 = g.epilogue == RS_EPI_RESID_F32 || g.epilogue == RS_EPI_BIAS_F32;
+  const int ldo = g.epilogue == RS_EPI_BIAS_GLU_BF16 ? g.N / 2 : g.N;
+  const CUtensorMapDataType dt = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                     : g.epilogue == RS_EPI_BIAS_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  if (!make_tmap_2d(&tm_out, dt, f32 ? 4 : 2, g.out, g.M, ldo, ldo, f32 ? 16 : 32, 64, CU_TENSOR_MAP_SWIZZLE_64B, err)) return cudaErrorInvalidValue;
+  // V^T: [N - split head dims, M frames] with row pitch ld2, 32 x 64 boxes; frames >= M are outside the map and untouched.
+  if (EG == 1 && !make_tmap_2d(&tm_out2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, g.out2, g.N - g.split, g.M, g.ld2, 64, 32,
+                               CU_TENSOR_MAP_SWIZZLE_128B, err))
+    return cudaErrorInvalidValue;
+  if (EG == 0) tm_out2 = tm_out;                             // not read
+  GemmDev p{g.bias, g.M, g.N, g.K, g.epilogue, g.alpha, g.split};
   const int tiles = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN);
   const int grid = tiles < num_sms ? tiles : num_sms;
-  gemm_bf16_tn_kernel<BN, EG><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(tm_a, tm_b, p);
+  gemm_bf16_tn_kernel<BN, EG><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(tm_a, tm_b, tm_out, tm_out2, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) snprintf(err, 256, "gemm launch (M=%d N=%d K=%d BN=%d): %s", g.M, g.N, g.K, BN, cudaGetErrorString(e));
   return e;
@@ -307,14 +338,20 @@ cudaError_t launch_gemm(const GemmArgs& g, int num_sms, cudaStream_t stream, cha
     snprintf(err, 256, "gemm shape unsupported: M=%d N=%d K=%d (need K%%64==0, N%%32==0)", g.M, g.N, g.K);
     return cudaErrorInvalidValue;
   }
-  if ((reinterpret_cast<uintptr_t>(g.a) | reinterpret_cast<uintptr_t>(g.w) | reinterpret_cast<uintptr_t>(g.out)) & 15u) {
-    snprintf(err, 256, "gemm operands must be 16-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(g.a) | reinterpret_cast<uintptr_t>(g.w) | reinterpret_cast<uintptr_t>(g.out) |
+       reinterpret_cast<uintptr_t>(g.bias) | reinterpret_cast<uintptr_t>(g.out2)) & 15u) {
+    snprintf(err, 256, "gemm operands, bias and outputs must be 16-byte aligned");
     return cudaErrorInvalidValue;
   }
   if (g.epilogue == RS_EPI_RESID_F32 && g.resid == nullptr) { snprintf(err, 256, "gemm: residual epilogue without resid"); return cudaErrorInvalidValue; }
   if (g.epilogue == RS_EPI_QKV_VT && (g.out2 == nullptr || g.split % 32 || g.ld2 % 8 || g.M % 8 || g.ld2 < g.M)) {
     snprintf(err, 256, "gemm: RS_EPI_QKV_VT needs out2, split %% 32 == 0, ld2 %% 8 == 0, M %% 8 == 0, ld2 >= M");
     return cudaErrorInvalidValue;
+  }
+  // The residual epilogue adds into out in place (a TMA reduction); a separate resid is copied to out first.
+  if (g.epilogue == RS_EPI_RESID_F32 && g.resid != g.out) {
+    cudaError_t e = cudaMemcpyAsync(g.out, g.resid, static_cast<size_t>(g.M) * g.N * sizeof(float), cudaMemcpyDeviceToDevice, stream);
+    if (e != cudaSuccess) { snprintf(err, 256, "gemm: residual copy: %s", cudaGetErrorString(e)); return e; }
   }
   // 256-wide tiles when N fills them and they give every SM a tile, else 64-wide ones on more SMs.  The two instances
   // compute every element alike, so the choice (which depends on M) cannot make a row's result depend on the batch it

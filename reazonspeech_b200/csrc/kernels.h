@@ -17,7 +17,7 @@ struct GemmArgs {
   const void* a;       // bf16 [M,K] row-major
   const void* w;       // bf16 [N,K] row-major (nn.Linear layout)
   const float* bias;   // f32 [N] or nullptr
-  const float* resid;  // f32 [M,N] for RS_EPI_RESID_F32 (may be out)
+  const float* resid;  // f32 [M,N] for RS_EPI_RESID_F32 (may be out; otherwise copied to out before the launch)
   void* out;
   int M, N, K;
   int epilogue;        // rs_epilogue

@@ -1,6 +1,7 @@
 """Per-shape timing of the wgmma GEMM (gemm_wgmma.cu) through Engine.gemm, the rs_gemm_bf16 seam.
 
     python scripts/bench_gemm.py [--lib path/to/librs_engine.so] [--launches 50] [--tiling current|n-only]
+                                 [--dump-outputs DIR]
 
 Shapes: the six GEMMs of a Conformer layer at configs[1] (M = 32 x 392 rows) with their own epilogues, the two
 subsampling 1x1 convs, the joint's encoder projection and the three products of an ALSD step (M = 32 clips x beam 4).
@@ -9,6 +10,8 @@ launch, algorithmic TFLOP/s (2 M N K), algorithmic HBM bytes (operands read once
 once) and GB/s, and the operand bytes a CTA pulls from L2 per FLOP for the tile the launch uses.  --lib loads another
 build of the library (the Python binding is the same), so two builds can be timed alternately on one machine; --tiling
 names the tile-selection rule of that build (n-only: 128 x 128 tiles when N % 128 == 0, else 128 x 64).
+--dump-outputs writes each shape's outputs of one launch on fresh buffers (raw bytes, <shape>.out / <shape>.out2) into
+DIR before it is timed, so that two builds can be compared byte for byte.
 Prints one JSON line, with the card's name and power limit read in the same run.
 """
 from __future__ import annotations
@@ -75,6 +78,7 @@ def main() -> None:
     ap.add_argument("--lib", default=None, help="librs_engine.so to load (default: the one in this tree)")
     ap.add_argument("--launches", type=int, default=50)
     ap.add_argument("--tiling", default="current", choices=["current", "n-only"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write each shape's outputs (raw bytes) into DIR")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_gemm.py needs a CUDA device")
@@ -104,6 +108,16 @@ def main() -> None:
             kw = dict(out=torch.empty(M, N, dtype=torch.float32, device="cuda"))
         else:
             kw = dict(out=torch.empty(M, N, dtype=torch.bfloat16, device="cuda"))
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            fresh = {k: v.clone() for k, v in kw.items() if k != "split"}
+            if epi == E.EPI_RESID_F32:
+                fresh["resid"] = fresh["out"]
+            eng.gemm(a, w, bias, epi, **fresh, **({"split": kw["split"]} if "split" in kw else {}))
+            torch.cuda.synchronize()
+            for k in ("out", "out2"):
+                if k in fresh:
+                    fresh[k].view(torch.uint8).cpu().numpy().tofile(os.path.join(args.dump_outputs, f"{name}.{k}"))
         for _ in range(5):
             eng.gemm(a, w, bias, epi, **kw)
         torch.cuda.synchronize()
