@@ -90,7 +90,9 @@ void rs_engine_destroy(rs_engine* e);
 /* Text of the last failure on `e` (or of the last failed rs_engine_create when e == NULL). */
 const char* rs_last_error(const rs_engine* e);
 
-/* Scratch the engine needs for a batch of B utterances of at most L_max samples. */
+/* Scratch the engine needs for a batch of B utterances of at most L_max samples.  It includes the ring of the n-gram LM
+ * fusion (96 * B * (multiprocessors / 4) bytes: about 100 KB for B = 32 on 132 multiprocessors) whether or not an LM is set,
+ * so that rs_set_ngram_lm never invalidates a workspace already set. */
 int rs_workspace_bytes(const rs_engine* e, int B, int L_max, size_t* bytes);
 int rs_set_workspace(rs_engine* e, void* dev_ptr, size_t bytes);
 
@@ -170,6 +172,37 @@ int rs_transcribe_batch_confidence(rs_engine* e, const void* wav_host, int wav_i
  * and must outlive every call that uses them; the engine keeps only the pointers.  rs_rnnt_alsd ignores them. */
 #define RS_MAX_BOOST_STATES 8192
 int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* next_dev, int n_states, int pitch);
+
+/* n-gram language-model shallow fusion of the greedy decode (reazonspeech_b200/ngram_lm.py builds the tables from an ARPA file
+ * over BPE token ids and states the semantics).  The decision of every (utterance, frame) is the argmax of
+ * logit_k + [k != blank] * (boosting bonus + LM term of k in the utterance's LM state); the state moves on emissions only and
+ * starts at start_state in every call.  The LM term of token k in state s is cb[s] + arc_w[a] for the highest-level arc a of
+ * token k on s's chain chain[s][0 .. order-1) (arcs of state o: arc_begin[o] .. arc_begin[o+1], sorted by arc_tok), or
+ * cb[s] + uni_w[k] when there is none; the state reached is arc_to[a] (or uni_to[k]).  State 0 is the empty context.  All
+ * arrays live in device memory, 16-byte aligned, owned by the caller, and must outlive every call that uses them; the engine
+ * keeps only the pointers.  2 <= order <= RS_MAX_LM_ORDER, n_states >= 1, n_arcs >= 0, pitch >= vocab_size and a multiple of
+ * 4, 0 <= start_state < n_states, no NULL array; otherwise RS_ERR_INVALID_ARG and the previous setting stays.  lm == NULL
+ * clears the setting.  While a table is set, every greedy entry point (rs_rnnt_greedy, rs_transcribe_device / _batch and
+ * their _pcm16 / _confidence forms) decodes with it; the confidence
+ * statistics stay those of the unfused softmax at the fused decisions.  rs_rnnt_alsd ignores it. */
+#define RS_MAX_LM_ORDER 6
+typedef struct rs_ngram_lm {
+  int order, n_states, n_arcs, pitch, start_state;
+  const float* cb;          /* [n_states] */
+  const int32_t* chain;     /* [n_states][order - 1] */
+  const int32_t* arc_begin; /* [n_states + 1] */
+  const int32_t* arc_tok;   /* [n_arcs] */
+  const int32_t* arc_to;    /* [n_arcs] */
+  const float* arc_w;       /* [n_arcs] */
+  const float* uni_w;       /* [pitch] */
+  const int32_t* uni_to;    /* [pitch] */
+} rs_ngram_lm;
+int rs_set_ngram_lm(rs_engine* e, const rs_ngram_lm* lm);
+/* The decode kernel's own LM lookup on n (state, token) pairs, device arrays states / tokens i32[n] -> score f32[n] (the LM
+ * term the decode adds to the token's logit in that state) and next i32[n] (the state emitting it leads to); a token outside
+ * [0, vocab_size) gives NaN and -1.  Needs a table set by rs_set_ngram_lm.  Asynchronous on stream.  A test seam. */
+int rs_ngram_lm_eval(rs_engine* e, const int32_t* states_dev, const int32_t* tokens_dev, int n, float* score_dev, int32_t* next_dev,
+                     void* stream);
 
 /* ALSD beam search (NeMo BeamRNNTInfer.align_length_sync_decoding, the shipped checkpoint's default strategy; the reference's
  * decode.py is written for its hypotheses, pkg/nemo-asr/src/decode.py:29,38-40,48): enc f32[B,T_max,d_model] + enc_len ->

@@ -44,6 +44,18 @@
 // rows are fetched (pass 0: under phases L and P) and added to the logits in the argmax epilogue.  With kConf as well, the
 // statistics stay those of the UNBOOSTED softmax at the boosted decision: log p = (l_emit - m) - log s, l_emit = the winner's
 // boosted value (recovered from its ordered bits) - its bonus, which is the raw logit to within one fp32 rounding.
+//
+// n-gram LM shallow fusion (kLM = true; tables built by reazonspeech_b200/ngram_lm.py, which states the semantics).  Every
+// utterance carries an LM state s_lm[b] (a context of the ARPA).  The LM term of token k in state s is cb[s] + w, w = arc_w of
+// the highest-level arc for k on s's back-off chain chain[s][0..order-1), or uni_w[k] (the dense root row) when there is none;
+// the state reached is that arc's arc_to (or uni_to[k]).  A pass fills, per utterance (one warp each), an LM tile of terms and
+// next states over the CTA's vocabulary slice: the root row first, then every chain level from the lowest to the highest
+// overwrites the tokens of its arcs (sorted, so a few 32-wide probe rounds narrow each level to the slice; all levels probe in
+// the same rounds).  The term is added to the logits next to the boosting bonus (the sum bonus + term when both are on).  The
+// transition costs no search: for the best token of every (row, slice), warp 0 writes (next state, added term) into the LM ring
+// ([3][B][kFrames][S], like conf); after the consume step the ring slot of the emitted token's slice holds the new state, which
+// phase L reads.  Pass 0's tile is filled between the arrival at and the release from the grid barrier that ends phase L,
+// i.e. under the barrier's latency.  With kConf the emitted token's unfused logit is its fused value - the added term.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -73,6 +85,8 @@ struct SpecDev {
   const float* boost_bonus;   // [n_states][boost_pitch] bonus of each non-blank token per automaton state (kBoost)
   const int32_t* boost_next;  // [n_states][boost_pitch] automaton transition on each non-blank token (kBoost)
   int boost_states, boost_pitch;
+  NgramLM lm;                 // (kLM)
+  int2* lm_ring;              // [3][B][kFrames][S] (next LM state, added term bits) of each slice's best token (kLM)
   int B, T_max, V, U_max, max_symbols;
   int S, rows_j, units, rows_p;
 };
@@ -103,21 +117,28 @@ __device__ __forceinline__ SoftStat soft_shfl_xor(const SoftStat& x, int o) {
 // owns it, three times per decode iteration; spread over several lines they proceed in parallel.  `round` counts the barriers passed; counter c has seen round * (number of CTAs with i % kBarCounters == c) arrivals.
 constexpr int kBarCounters = 8;
 constexpr int kBarStride = 32;            // unsigned ints between counters
-__device__ __forceinline__ void sp_grid_barrier(unsigned int* counters, unsigned int& round, unsigned int nblocks) {
+// `during` runs CTA-local work between the arrival and the wait: it may touch only shared memory and read-only global data
+// (other CTAs' writes of the phase are not visible to it)
+template <class F>
+__device__ __forceinline__ void sp_grid_barrier_with(unsigned int* counters, unsigned int& round, unsigned int nblocks, F&& during) {
   __syncthreads();
   ++round;
-  if (threadIdx.x == 0)     // release at gpu scope: covers the other threads' writes too (they reached thread 0 through the CTA barrier above)
+  if (threadIdx.x == 0)
     asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counters + (blockIdx.x % kBarCounters) * kBarStride) : "memory");
+  during();
   if (threadIdx.x < kBarCounters) {
     const unsigned int c = threadIdx.x;
-    const unsigned int arrivals = (nblocks + kBarCounters - 1 - c) / kBarCounters;      // CTAs with index % kBarCounters == c
-    const unsigned int target = round * arrivals;
+    const unsigned int target = round * ((nblocks + kBarCounters - 1 - c) / kBarCounters);
     unsigned int v;
     do {
       asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(counters + c * kBarStride) : "memory");
     } while (v < target);
   }
   __syncthreads();
+}
+
+__device__ __forceinline__ void sp_grid_barrier(unsigned int* counters, unsigned int& round, unsigned int nblocks) {
+  sp_grid_barrier_with(counters, round, nblocks, [] {});
 }
 
 __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -170,6 +191,76 @@ __device__ __forceinline__ float best_value(unsigned long long v) {
 // below j0 (<= 3 + 128 + 3 floats copied)
 constexpr int kTileLd = 136;
 
+// n-gram LM lookup of one state over vocabulary columns [j0, jn), jn - j0 <= kTileLd (the slice width rows_j <= 128), by one warp: term[j - j0] = the LM term
+// of token j, next[j - j0] = the state emitting it leads to.  The root row is written first; then the chain levels, lowest
+// first, overwrite the tokens they have arcs for, so the highest level wins (a level's tokens are distinct: no lane conflicts).
+// Each level's arc range is narrowed to <= 32 arcs around the first token >= j0 by 32-wide probe rounds, all levels in the
+// same rounds; then 32-arc chunks are read from there until a token >= jn.  A state outside [0, n_states) counts as the root.
+constexpr int kMaxLmCtx = 5;                 // LM order <= 6
+constexpr int kNoTok = 0x7fffffff;
+__device__ __forceinline__ void lm_fill_row(const NgramLM& lm, int s, int j0, int jn, float* term, int* next, int lane) {
+  const int nctx = lm.order - 1;
+  if (static_cast<unsigned int>(s) >= static_cast<unsigned int>(lm.n_states)) s = 0;
+  const float cb = __ldg(lm.cb + s);
+  const int o = lane < nctx ? __ldg(lm.chain + static_cast<size_t>(s) * nctx + lane) : 0;
+  for (int j = j0 + lane; j < jn; j += 32) { term[j - j0] = cb + __ldg(lm.uni_w + j); next[j - j0] = __ldg(lm.uni_to + j); }
+  int lo = 0, end = 0;
+  if (o > 0) { lo = __ldg(lm.arc_begin + o); end = __ldg(lm.arc_begin + o + 1); }
+  int L[kMaxLmCtx], H[kMaxLmCtx], E[kMaxLmCtx];    // level d (chain[s][d]): the first arc with token >= j0 lies in [L, H]
+#pragma unroll
+  for (int d = 0; d < kMaxLmCtx; ++d) { L[d] = __shfl_sync(0xffffffffu, lo, d); E[d] = __shfl_sync(0xffffffffu, end, d); H[d] = E[d]; }
+  for (;;) {
+    int v[kMaxLmCtx];
+    bool more = false;
+#pragma unroll
+    for (int d = 0; d < kMaxLmCtx; ++d) {                    // the probes of every level first: independent loads
+      v[d] = kNoTok;
+      const int n = H[d] - L[d];
+      if (n > 32) {
+        more = true;
+        const int step = (n + 31) >> 5, q = L[d] + lane * step + step - 1;
+        if (q < H[d]) v[d] = __ldg(lm.arc_tok + q);
+      }
+    }
+    if (!more) break;                                         // warp-uniform
+#pragma unroll
+    for (int d = 0; d < kMaxLmCtx; ++d) {
+      const int n = H[d] - L[d];
+      if (n > 32) {
+        const int step = (n + 31) >> 5, c = __popc(__ballot_sync(0xffffffffu, v[d] < j0));
+        L[d] += c * step;
+        H[d] = min(L[d] + step - 1, H[d]);
+      }
+    }
+  }
+  int t0[kMaxLmCtx], n0[kMaxLmCtx];
+  float w0[kMaxLmCtx];
+#pragma unroll
+  for (int d = 0; d < kMaxLmCtx; ++d) {                      // first chunk of every level
+    const int i = L[d] + lane;
+    const bool ok = i < E[d];
+    t0[d] = ok ? __ldg(lm.arc_tok + i) : kNoTok;
+    w0[d] = ok ? __ldg(lm.arc_w + i) : 0.f;
+    n0[d] = ok ? __ldg(lm.arc_to + i) : 0;
+  }
+  __syncwarp();                                               // the root row is written before any overwrite
+#pragma unroll
+  for (int d = kMaxLmCtx - 1; d >= 0; --d) {
+    int t = t0[d], nx = n0[d];
+    float w = w0[d];
+    for (int base = L[d];; base += 32) {
+      if (t >= j0 && t < jn) { term[t - j0] = cb + w; next[t - j0] = nx; }
+      if (!(__shfl_sync(0xffffffffu, t, 31) < jn && base + 32 < E[d])) break;
+      const int i = base + 32 + lane;
+      const bool ok = i < E[d];
+      t = ok ? __ldg(lm.arc_tok + i) : kNoTok;
+      w = ok ? __ldg(lm.arc_w + i) : 0.f;
+      nx = ok ? __ldg(lm.arc_to + i) : 0;
+    }
+    __syncwarp();
+  }
+}
+
 // The joint window runs on wgmma.  A = the CTA's W_out rows as IEEE half in 128B-swizzled K-major slabs of 64 columns
 // (88 rows stored per slab; the two warpgroups' m64 instructions cover 128 rows and read on into the next slab / region,
 // whose rows land in accumulator rows nobody looks at), B = the 32 (utterance, frame) activation rows as two half planes
@@ -178,7 +269,7 @@ constexpr int kTileLd = 136;
 // is one m64n64k16 per warpgroup and the two halves of D are added in the epilogue.
 static_assert(kSpThreads == 256, "the joint is issued by two warpgroups");
 
-template <int HJ, int HP, bool kConf, bool kBoost>
+template <int HJ, int HP, bool kConf, bool kBoost, bool kLM>
 __global__ void __launch_bounds__(kSpThreads, 1)
 rnnt_greedy_spec_kernel(const SpecDev p) {
   constexpr int KH = HJ / 2;                 // joint k-half staged in shared memory at a time
@@ -240,6 +331,14 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   float* s_tile = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kConf ? s_conf + kPassRows * kSpWarps * 5 : reinterpret_cast<float*>(s_cj)) + 15) & ~static_cast<uintptr_t>(15));
   int* s_state = reinterpret_cast<int*>(s_tile + kPassUtts * kTileLd);
   float* s_le = reinterpret_cast<float*>(s_state + B);
+  // kLM (after the kBoost arrays, which then always exist): [kPassUtts][kTileLd] LM term and next-state tiles, the per-warp
+  // (next state, added term) of each row's best token [kPassRows][kSpWarps] (8-byte aligned), LM state and LM ring slot of the
+  // window's emission (-1: none) per utterance
+  float* s_lmw = reinterpret_cast<float*>(s_le + B);
+  int* s_lmn = reinterpret_cast<int*>(s_lmw + kPassUtts * kTileLd);
+  int2* s_lmb = reinterpret_cast<int2*>((reinterpret_cast<uintptr_t>(s_lmn + kPassUtts * kTileLd) + 7) & ~static_cast<uintptr_t>(7));
+  int* s_lm = reinterpret_cast<int*>(s_lmb + kPassRows * kSpWarps);
+  int* s_lslot = s_lm + B;
 
   {
     const uint32_t zero = 0;
@@ -270,6 +369,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     for (int b = tid; b < B; b += kSpThreads) {
       s_t[b] = 0; s_sym[b] = 0; s_n[b] = 0; s_tok[b] = blank; s_len[b] = p.enc_len[b];
       if constexpr (kBoost) s_state[b] = 0;
+      if constexpr (kLM) { s_lm[b] = p.lm.start_state; s_lslot[b] = -1; }
     }
     if (tid < 12) s_prof[tid] = 0;
   }
@@ -284,8 +384,18 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   // ------------------------------------------------------------------------------------------------
   // LSTM step + joint.pred for the utterances listed in s_emit[0..n_emit), which emitted token s_tok[b]
   // ------------------------------------------------------------------------------------------------
+  // kLM: the LM tile rows of a pass's utterances over the CTA's vocabulary slice, warp e filling the pass's utterance e
+  static_assert(kPassUtts == kSpWarps, "one warp per utterance of a pass fills its LM tile row");
+  auto lm_fill = [&](int pass) {
+    const int ai = grp + kGroups * (pass * kPassUtts + warp);
+    if (ai < s_cnt[1]) lm_fill_row(p.lm, s_lm[s_act[ai]], j0, min(j1, p.V), s_lmw + warp * kTileLd, s_lmn + warp * kTileLd, lane);
+  };
+
   auto lstm_and_pred = [&]() {
     const int n_emit = s_cnt[0];
+    // kLM: the new LM state of utterance tid's emission, requested now and stored after the elementwise work
+    int lm_nx = -1;
+    if constexpr (kLM) if (tid < B && s_lslot[tid] >= 0) lm_nx = __ldcg(&p.lm_ring[s_lslot[tid]].x);
     // ---- phase L: gates = rec + gate_tab[token] per (utterance, unit of the CTA) -> cell -> h.  rec = W_hh . h of the
     // utterance's previous step came from this CTA's phase P (zero before the first step, as h is).
     if (nu > 0) {
@@ -303,8 +413,13 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
         __stcg(p.hbuf + static_cast<size_t>(b) * HP + unit, og * tanhf(c2));
       }
     }
+    if constexpr (kLM) {
+      if (lm_nx >= 0) s_lm[tid] = lm_nx;
+      for (int b = tid + kSpThreads; b < B; b += kSpThreads) if (s_lslot[b] >= 0) s_lm[b] = __ldcg(&p.lm_ring[s_lslot[b]].x);
+    }
     tick(3, tk);
-    sp_grid_barrier(p.counter, target, G);
+    if constexpr (kLM) sp_grid_barrier_with(p.counter, target, G, [&] { if (has_j) lm_fill(0); });   // pass 0's LM tile
+    else sp_grid_barrier(p.counter, target, G);
     tick(4, tk);
     // ---- phase P: one load of the new h of every emitting utterance feeds both products of the CTA, K split over the
     // warps: its rows_p rows of W_pred (-> ppbuf) and its 4 * units rows of W_hh (-> rec, the recurrent half of the
@@ -466,6 +581,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
           cp_async16(s_tile + u * kTileLd + 4 * c, p.boost_bonus + static_cast<size_t>(s_state[s_act[ai]]) * p.boost_pitch + a0 + 4 * c);
       }
     }
+    if constexpr (kLM) if (pass > 0) lm_fill(pass);   // pass 0's tile is filled under the barrier that ends phase L
 #pragma unroll
     for (int i = 0; i < PERU; ++i) {
       int c4, rb[kFrames], rt[kFrames];
@@ -595,19 +711,39 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
                 bon[j][1] = j0 + rr + 8 < p.V ? tr[8] : 0.f;
               }
             }
+            if constexpr (kLM) {                              // the LM terms of the same rows, summed with the bonus
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const float* tr = s_lmw + (2 * j + (tig >> 1)) * kTileLd + rr;
+                const float lm0 = j0 + rr < p.V ? tr[0] : 0.f, lm1 = j0 + rr + 8 < p.V ? tr[8] : 0.f;
+                if constexpr (kBoost) { bon[j][0] += lm0; bon[j][1] += lm1; } else { bon[j][0] = lm0; bon[j][1] = lm1; }
+              }
+            }
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const float l0 = (dj[4 * j + e] + dj[4 * (j + 4) + e]) + bias0, l1 = (dj[4 * j + 2 + e] + dj[4 * (j + 4) + 2 + e]) + bias1;
                 float s0 = l0, s1 = l1;                       // the scores the argmax ranks
-                if constexpr (kBoost) { s0 += bon[j][0]; s1 += bon[j][1]; }
+                if constexpr (kBoost || kLM) { s0 += bon[j][0]; s1 += bon[j][1]; }
                 unsigned long long k0 = v0 ? pack_best(s0, j0 + rr) : 0ull;
                 const unsigned long long k1 = v1 ? pack_best(s1, j0 + rr + 8) : 0ull;
                 k0 = k1 > k0 ? k1 : k0;                       // higher logit first, ties -> lower row
 #pragma unroll
                 for (int o = 4; o < 32; o <<= 1) { const unsigned long long ot = __shfl_xor_sync(0xffffffffu, k0, o); k0 = ot > k0 ? ot : k0; }
                 if (gid == 0) s_best[(8 * j + 2 * tig + e) * kSpWarps + warp] = k0;
+                if constexpr (kLM) {                          // (next LM state, added term) of the warp's best token of the column
+                  if (gid == 0) {
+                    const int k = static_cast<int>(0xffffffffu - static_cast<unsigned int>(k0 & 0xffffffffull)), u = 2 * j + (tig >> 1);
+                    int2 r = make_int2(0, 0);
+                    if (static_cast<unsigned int>(k) < static_cast<unsigned int>(p.V)) {   // k0 == 0 (no row): none
+                      float add = s_lmw[u * kTileLd + k - j0];
+                      if constexpr (kBoost) add = s_tile[u * kTileLd + (j0 & 3) + k - j0] + add;
+                      r = make_int2(s_lmn[u * kTileLd + k - j0], __float_as_int(add));
+                    }
+                    s_lmb[(8 * j + 2 * tig + e) * kSpWarps + warp] = r;
+                  }
+                }
                 if constexpr (kConf) {                        // the same logits and lanes -> the warp's softmax tuple of the column
                   SoftStat c = soft_merge(v0 ? soft_one(l0) : soft_empty(), v1 ? soft_one(l1) : soft_empty(), p.alpha_l2);
 #pragma unroll
@@ -627,6 +763,11 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
 #pragma unroll
           for (int q = 1; q < kSpWarps; ++q) { const unsigned long long o = s_best[lane * kSpWarps + q]; m = o > m ? o : m; }
           asm volatile("red.relaxed.gpu.global.max.u64 [%0], %1;" ::"l"(p.best + (static_cast<size_t>(iter % 3) * B + row_b) * kFrames + (lane % kFrames)), "l"(m) : "memory");
+          if constexpr (kLM) {                                // the slice's best token's (next state, term): its own ring slot
+            int q = 0;
+            while (s_best[lane * kSpWarps + q] != m) ++q;
+            __stcg(p.lm_ring + ((static_cast<size_t>(iter % 3) * B + row_b) * kFrames + (lane % kFrames)) * p.S + slice, s_lmb[lane * kSpWarps + q]);
+          }
           if constexpr (kConf) {                              // the slice's tuple: a plain store into the slot it owns
             const float* sc = s_conf + lane * kSpWarps * 5;
             SoftStat c = {sc[0], sc[1], sc[2], sc[3], sc[4]};
@@ -648,7 +789,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     for (int b = tid; b < B; b += kSpThreads) {
       int t = s_t[b];
       const int len = s_len[b];
-      int tok = -1, cj = -1;
+      int tok = -1, cj = -1, lslot = -1;
       if (t < len) {
         const int nv = min(kFrames, len - t);
         int sym = s_sym[b];
@@ -671,8 +812,12 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
           if constexpr (kBoost) {
             const size_t at = static_cast<size_t>(s_state[b]) * p.boost_pitch + k;
             const int nx = __ldg(p.boost_next + at);
-            if constexpr (kConf) if (n < p.U_max) s_le[b] = best_value(v) - __ldg(p.boost_bonus + at);
+            if constexpr (kConf && !kLM) if (n < p.U_max) s_le[b] = best_value(v) - __ldg(p.boost_bonus + at);
             s_state[b] = static_cast<unsigned int>(nx) < static_cast<unsigned int>(p.boost_states) ? nx : 0;
+          }
+          if constexpr (kLM) {                                // the ring slot of k's slice; read in phase L (the new state)
+            lslot = static_cast<int>(((static_cast<size_t>(iter % 3) * B + b) * kFrames + j) * p.S + k / p.rows_j);
+            if constexpr (kConf) if (n < p.U_max) s_le[b] = best_value(v);   // fused; the term comes from the ring
           }
           s_n[b] = n + 1;
           tok = k;
@@ -683,6 +828,7 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
       }
       s_tok[b] = tok;
       if constexpr (kConf) s_cj[b] = cj;
+      if constexpr (kLM) s_lslot[b] = lslot;
     }
     // the slot that iteration iter+2 will use was last read two barriers ago: clear it now (visible through the
     // next barrier, which precedes that iteration's red.max)
@@ -709,21 +855,23 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
         for (int o = 16; o > 0; o >>= 1) c = soft_merge(c, soft_shfl_xor(c, o), p.alpha_l2);
         if (lane == 0) {                                      // c is relative to the maximum logit m: log p = (l - m) - log s
           const float log_s = logf(c.s), inv_s = 1.f / c.s, s_ma = expf(-p.alpha * log_s), a_alpha = s_ma * c.a;
-          const float lp = kBoost ? (s_le[b] - c.m) - log_s : -log_s;   // unboosted, the emitted token is the maximum
+          float lp = kBoost ? (s_le[b] - c.m) - log_s : -log_s;   // unboosted, the emitted token is the maximum
+          if constexpr (kLM) lp = ((s_le[b] - __int_as_float(__ldcg(&p.lm_ring[s_lslot[b]].y))) - c.m) - log_s;   // unfused
           const float4 st = make_float4(lp, c.g * inv_s - log_s, a_alpha, s_ma * c.ga - log_s * a_alpha);
           __stcg(reinterpret_cast<float4*>(p.stats + (static_cast<size_t>(b) * p.U_max + (s_n[b] - 1)) * 4), st);
         }
       }
     }
     if (s_cnt[0] > 0) lstm_and_pred();
+    if constexpr (kLM) if (s_cnt[0] == 0 && has_j) lm_fill(0);   // no emission: the states stand, the pass's rows may not
     if (n_active == 0) break;
   }
   if (cta == 0) for (int b = tid; b < B; b += kSpThreads) p.n_tok[b] = s_n[b];
   if (cta == 0 && tid == 0) for (int i = 0; i < 12; ++i) p.prof[i] = s_prof[i];
 }
 
-// workspace (SpecDev's global buffers): hbuf | rec | ppbuf | barrier counters (kBarCounters 128-byte lines) | prof | best | conf.
-// Everything before conf is zeroed by the launch; every conf slot that is read was written first.
+// workspace (SpecDev's global buffers): hbuf | rec | ppbuf | barrier counters (kBarCounters 128-byte lines) | prof | best | conf |
+// lm_ring.  Everything before conf is zeroed by the launch; every conf / lm_ring slot that is read was written first.
 SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms) {
   Arena a;
   SpecWorkspace w;
@@ -734,13 +882,14 @@ SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms) {
   w.prof = a.take(12 * 8);
   w.best = a.take(static_cast<size_t>(3) * B * kFrames * 8);
   w.conf = a.take(static_cast<size_t>(3) * B * kFrames * (num_sms / kGroups) * 5 * 4);
+  w.lm_ring = a.take(static_cast<size_t>(3) * B * kFrames * (num_sms / kGroups) * 8);
   w.total = a.off;
   return w;
 }
 
-template <int HJ, int HP, bool kConf, bool kBoost>
+template <int HJ, int HP, bool kConf, bool kBoost, bool kLM>
 static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
-  const auto kernel = rnnt_greedy_spec_kernel<HJ, HP, kConf, kBoost>;
+  const auto kernel = rnnt_greedy_spec_kernel<HJ, HP, kConf, kBoost, kLM>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   int per_sm = 0;
@@ -751,11 +900,26 @@ static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stre
   return cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(kSpThreads), args, smem, stream);
 }
 
-template <int HJ, int HP>
+template <int HJ, int HP, bool kLM>
 static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
   if (p.boost_bonus != nullptr)
-    return p.stats != nullptr ? launch_sp<HJ, HP, true, true>(p, grid, smem, stream) : launch_sp<HJ, HP, false, true>(p, grid, smem, stream);
-  return p.stats != nullptr ? launch_sp<HJ, HP, true, false>(p, grid, smem, stream) : launch_sp<HJ, HP, false, false>(p, grid, smem, stream);
+    return p.stats != nullptr ? launch_sp<HJ, HP, true, true, kLM>(p, grid, smem, stream) : launch_sp<HJ, HP, false, true, kLM>(p, grid, smem, stream);
+  return p.stats != nullptr ? launch_sp<HJ, HP, true, false, kLM>(p, grid, smem, stream) : launch_sp<HJ, HP, false, false, kLM>(p, grid, smem, stream);
+}
+
+template <int HJ, int HP>
+static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
+  return p.lm.order != 0 ? launch_sp<HJ, HP, true>(p, grid, smem, stream) : launch_sp<HJ, HP, false>(p, grid, smem, stream);
+}
+
+// The LM table contract the kernels rely on (rs_set_ngram_lm checks the same before it accepts a table)
+static bool lm_tables_ok(const NgramLM& lm, int V) {
+  const uintptr_t ptrs = reinterpret_cast<uintptr_t>(lm.cb) | reinterpret_cast<uintptr_t>(lm.chain) | reinterpret_cast<uintptr_t>(lm.arc_begin) |
+                         reinterpret_cast<uintptr_t>(lm.arc_tok) | reinterpret_cast<uintptr_t>(lm.arc_to) | reinterpret_cast<uintptr_t>(lm.arc_w) |
+                         reinterpret_cast<uintptr_t>(lm.uni_w) | reinterpret_cast<uintptr_t>(lm.uni_to);
+  return lm.order >= 2 && lm.order <= kMaxLmCtx + 1 && lm.n_states >= 1 && lm.n_arcs >= 0 && lm.pitch >= V && lm.pitch % 4 == 0 &&
+         lm.start_state >= 0 && lm.start_state < lm.n_states && lm.cb && lm.chain && lm.arc_begin && lm.arc_tok && lm.arc_to && lm.arc_w &&
+         lm.uni_w && lm.uni_to && (ptrs & 15u) == 0;
 }
 
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream) {
@@ -785,6 +949,10 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   if (boost && (a.boost_next == nullptr || a.boost_states < 1 || a.boost_pitch < a.V || (a.boost_pitch & 3) ||
                 ((reinterpret_cast<uintptr_t>(a.boost_bonus) | reinterpret_cast<uintptr_t>(a.boost_next)) & 15u)))
     return cudaErrorInvalidValue;                                  // the tile is copied in 16-byte pieces
+  p.lm = a.lm;
+  const bool lm = a.lm.order != 0;
+  if (lm && !lm_tables_ok(a.lm, a.V)) return cudaErrorInvalidValue;
+  p.lm_ring = reinterpret_cast<int2*>(ws + w.lm_ring);
   p.B = a.B; p.T_max = a.T_max; p.V = a.V; p.U_max = a.U_max; p.max_symbols = a.max_symbols;
   p.S = G / kGroups;
   p.rows_j = (a.V + 1 + p.S - 1) / p.S;
@@ -796,9 +964,11 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   const size_t state = ((static_cast<size_t>(a.B) * p.units + 1) & ~static_cast<size_t>(1)) * 4 + (kPassRows * kSpWarps + 12) * 8 + static_cast<size_t>(a.B) * 7 * 4 +
                        (2 + 2 * kSpWarps) * 4 + 64 +
                        (a.stats != nullptr ? static_cast<size_t>(a.B) * 4 + kPassRows * kSpWarps * 5 * 4 : 0) +   // kConf: s_cj, s_conf
-                       (boost ? 16 + kPassUtts * kTileLd * 4 + static_cast<size_t>(a.B) * 4 * (a.stats != nullptr ? 2 : 1) : 0);   // kBoost: align, s_tile, s_state (, s_le)
+                       (boost && !lm ? 16 + kPassUtts * kTileLd * 4 + static_cast<size_t>(a.B) * 4 * (a.stats != nullptr ? 2 : 1) : 0) +   // kBoost: align, s_tile, s_state (, s_le)
+                       (lm ? 16 + kPassUtts * kTileLd * 4 + static_cast<size_t>(a.B) * 8 +                 // kLM: the kBoost arrays,
+                             2 * kPassUtts * kTileLd * 4 + 8 + kPassRows * kSpWarps * 8 + static_cast<size_t>(a.B) * 8 : 0);   // s_lmw, s_lmn, s_lmb, s_lm, s_lslot
   const size_t w_lp = (static_cast<size_t>(4 * p.units) * (a.Hp + 8) + static_cast<size_t>(p.rows_p) * (a.Hp + 8)) * 2;
-  if (p.rows_j > 128) return cudaErrorInvalidValue;
+  if (p.rows_j > 128) return cudaErrorInvalidValue;                // also the LM tile / lm_fill_row's slice bound
   const size_t rows_a8 = (p.rows_j + 7) & ~7;
   const size_t b_bytes = static_cast<size_t>(a.Hj / 2 / 64) * 8192;
   const size_t b_region = b_bytes > 32768 ? b_bytes : 32768;     // also the [8 warps][32][32] fp32 reduction buffer of phase P
@@ -808,6 +978,38 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   if (a.Hj == 640 && a.Hp == 640) return launch_sp<640, 640>(p, G, smem, stream);
   if (a.Hj == 128 && a.Hp == 128) return launch_sp<128, 128>(p, G, smem, stream);
   return cudaErrorInvalidValue;
+}
+
+// rs_ngram_lm_eval: one warp per (state, token) pair runs lm_fill_row over the slice the decode gives the token (S = num_sms /
+// kGroups slices of rows_j columns) and reads the token's term and next state, as the decode's epilogue and ring do
+__global__ void __launch_bounds__(kSpThreads) ngram_lm_eval_kernel(const NgramLM lm, int V, int rows_j, const int32_t* states,
+                                                                   const int32_t* tokens, int n, float* score, int32_t* next) {
+  __shared__ float s_w[kSpWarps][kTileLd];
+  __shared__ int s_n[kSpWarps][kTileLd];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * kSpWarps + warp; i < n; i += gridDim.x * kSpWarps) {
+    const int k = tokens[i];
+    if (static_cast<unsigned int>(k) >= static_cast<unsigned int>(V)) {
+      if (lane == 0) { score[i] = __int_as_float(0x7fc00000); next[i] = -1; }
+      continue;
+    }
+    const int j0 = (k / rows_j) * rows_j;
+    lm_fill_row(lm, states[i], j0, min(j0 + rows_j, V), s_w[warp], s_n[warp], lane);
+    __syncwarp();
+    if (lane == 0) { score[i] = s_w[warp][k - j0]; next[i] = s_n[warp][k - j0]; }
+    __syncwarp();
+  }
+}
+
+cudaError_t launch_ngram_lm_eval(const NgramLM& lm, int V, int num_sms, const int32_t* states, const int32_t* tokens, int n,
+                                 float* score, int32_t* next, cudaStream_t stream) {
+  if (n < 0 || num_sms < kGroups || !lm_tables_ok(lm, V)) return cudaErrorInvalidValue;
+  if (n == 0) return cudaSuccess;
+  const int S = num_sms / kGroups, rows_j = (V + 1 + S - 1) / S;
+  if (rows_j > 128) return cudaErrorInvalidValue;
+  const int grid = min((n + kSpWarps - 1) / kSpWarps, 4096);
+  ngram_lm_eval_kernel<<<grid, kSpThreads, 0, stream>>>(lm, V, rows_j, states, tokens, n, score, next);
+  return cudaGetLastError();
 }
 
 }  // namespace rs

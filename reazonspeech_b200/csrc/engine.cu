@@ -80,6 +80,8 @@ struct rs_engine {
   struct { const void *enc_w, *out_w, *lstm_w, *pred_w; const float *enc_b, *out_b, *embed, *lstm_b, *pred_b, *gate_tab; } dec;
   // phrase boosting (rs_set_phrase_boosting): caller-owned device tables used by every greedy decode while set
   struct { const float* bonus = nullptr; const int32_t* next = nullptr; int n_states = 0, pitch = 0; } boost;
+  // n-gram LM shallow fusion (rs_set_ngram_lm): caller-owned device tables used by every greedy decode while set; order 0: none
+  rs::NgramLM lm;
   void* ws = nullptr;
   size_t ws_bytes = 0;
   mutable char err[512] = "";
@@ -415,7 +417,7 @@ int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_
   mark(e, 4, s);
   rs::DecodeArgs da{at<float>(e, p.encp), enc_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w, e->dec.gate_tab, e->dec.pred_w,
                     e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, c.max_symbols,
-                    stats, alpha, e->boost.bonus, e->boost.next, e->boost.n_states, e->boost.pitch};
+                    stats, alpha, e->boost.bonus, e->boost.next, e->boost.n_states, e->boost.pitch, e->lm};
   // One decode kernel for every batch size (windowed, weights-stationary, joint on wgmma: decode_spec.cu): an utterance's
   // logits are accumulated in the same order whether it is decoded alone or inside a batch, so results do not depend on
   // batch composition.
@@ -496,6 +498,42 @@ int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* 
   if (bonus_dev == nullptr || next_dev == nullptr || ((reinterpret_cast<uintptr_t>(bonus_dev) | reinterpret_cast<uintptr_t>(next_dev)) & 15u))
     return fail(e, RS_ERR_INVALID_ARG, "rs_set_phrase_boosting: bonus and next must be non-null and 16-byte aligned");
   e->boost.bonus = bonus_dev; e->boost.next = next_dev; e->boost.n_states = n_states; e->boost.pitch = pitch;
+  return RS_OK;
+}
+
+int rs_set_ngram_lm(rs_engine* e, const rs_ngram_lm* lm) {
+  if (e == nullptr) return RS_ERR_INVALID_ARG;
+  if (lm == nullptr) {
+    e->lm = {};
+    return RS_OK;
+  }
+  if (lm->order < 2 || lm->order > RS_MAX_LM_ORDER)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_set_ngram_lm: order=%d outside [2, %d]", lm->order, RS_MAX_LM_ORDER);
+  if (lm->n_states < 1 || lm->n_arcs < 0 || lm->start_state < 0 || lm->start_state >= lm->n_states)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_set_ngram_lm: n_states=%d, n_arcs=%d, start_state=%d (need n_states >= 1, n_arcs >= 0, "
+                "0 <= start_state < n_states)", lm->n_states, lm->n_arcs, lm->start_state);
+  if (lm->pitch < e->cfg.vocab_size || lm->pitch % 4 != 0)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_set_ngram_lm: pitch=%d must be >= vocab_size (%d) and a multiple of 4", lm->pitch, e->cfg.vocab_size);
+  const void* arrays[] = {lm->cb, lm->chain, lm->arc_begin, lm->arc_tok, lm->arc_to, lm->arc_w, lm->uni_w, lm->uni_to};
+  for (const void* a : arrays)
+    if (a == nullptr || (reinterpret_cast<uintptr_t>(a) & 15u))
+      return fail(e, RS_ERR_INVALID_ARG, "rs_set_ngram_lm: every array must be non-null and 16-byte aligned");
+  rs::NgramLM t;
+  t.cb = lm->cb; t.chain = lm->chain; t.arc_begin = lm->arc_begin; t.arc_tok = lm->arc_tok; t.arc_to = lm->arc_to; t.arc_w = lm->arc_w;
+  t.uni_w = lm->uni_w; t.uni_to = lm->uni_to;
+  t.order = lm->order; t.n_states = lm->n_states; t.n_arcs = lm->n_arcs; t.pitch = lm->pitch; t.start_state = lm->start_state;
+  e->lm = t;
+  return RS_OK;
+}
+
+int rs_ngram_lm_eval(rs_engine* e, const int32_t* states_dev, const int32_t* tokens_dev, int n, float* score_dev, int32_t* next_dev,
+                     void* stream) {
+  if (e == nullptr || n < 0 || (n > 0 && (!states_dev || !tokens_dev || !score_dev || !next_dev)))
+    return fail(e, RS_ERR_INVALID_ARG, "rs_ngram_lm_eval: bad arguments");
+  if (e->lm.order == 0) return fail(e, RS_ERR_INVALID_ARG, "rs_ngram_lm_eval: no n-gram LM is set (rs_set_ngram_lm)");
+  RS_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  RS_LAUNCH(e, s, 1, rs::launch_ngram_lm_eval(e->lm, e->cfg.vocab_size, e->num_sms, states_dev, tokens_dev, n, score_dev, next_dev, s));
   return RS_OK;
 }
 

@@ -69,6 +69,20 @@ struct AttnArgs {
 bool attention_tc_supported(const AttnArgs& a);
 cudaError_t launch_attention_tc(const AttnArgs& a, cudaStream_t stream);
 
+// n-gram LM of the greedy decode's shallow fusion (reazonspeech_b200/ngram_lm.py builds it; decode_spec.cu describes the
+// layout).  Device arrays, 16-byte aligned; order == 0: no LM.
+struct NgramLM {
+  const float* cb = nullptr;            // [n_states] summed back-off weight of the state's chain (root excluded), nats x alpha
+  const int32_t* chain = nullptr;       // [n_states][order - 1] the state, its back-off state, ... (0 = root pads)
+  const int32_t* arc_begin = nullptr;   // [n_states + 1] CSR of the arcs, sorted by token within a state
+  const int32_t* arc_tok = nullptr;     // [n_arcs]
+  const int32_t* arc_to = nullptr;      // [n_arcs] state reached by emitting arc_tok from the arc's state
+  const float* arc_w = nullptr;         // [n_arcs] LM term of the arc minus cb of its state
+  const float* uni_w = nullptr;         // [pitch] root row: LM term of every token in the empty context
+  const int32_t* uni_to = nullptr;      // [pitch] root row: state reached from the empty context
+  int order = 0, n_states = 0, n_arcs = 0, pitch = 0, start_state = 0;
+};
+
 struct DecodeArgs {
   const float* enc_proj;      // f32 [B*T_max, Hj]  (joint.enc applied to every frame)
   const int32_t* enc_len;
@@ -87,14 +101,20 @@ struct DecodeArgs {
   const float* boost_bonus = nullptr;
   const int32_t* boost_next = nullptr;
   int boost_states = 0, boost_pitch = 0;
+  NgramLM lm;                 // n-gram LM shallow fusion; lm.order == 0: none
 };
 // Byte offsets of the decode workspace's regions and its size (decode_spec.cu describes the regions)
-struct SpecWorkspace { size_t hbuf, rec, ppbuf, counters, prof, best, conf, total; };
+struct SpecWorkspace { size_t hbuf, rec, ppbuf, counters, prof, best, conf, lm_ring, total; };
 SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms);
 // windowed (kFrames per iteration) persistent decode, joint on wgmma (decode_spec.cu); workspace laid out by rnnt_spec_workspace();
 // a.stats != nullptr selects the instance that also reduces the softmax statistics of every emitted token,
-// a.boost_bonus != nullptr the one that adds the phrase-boosting bonus before the argmax
+// a.boost_bonus != nullptr the one that adds the phrase-boosting bonus before the argmax, a.lm.order != 0 the one that adds the
+// n-gram LM term
 cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int num_sms, cudaStream_t stream);
+// The decode kernel's own LM lookup on n arbitrary (state, token) pairs (device arrays): score[i] = the LM term the decode adds to
+// token tokens[i]'s logit in state states[i], next[i] = the state emitting it leads to (decode_spec.cu)
+cudaError_t launch_ngram_lm_eval(const NgramLM& lm, int V, int num_sms, const int32_t* states, const int32_t* tokens, int n,
+                                 float* score, int32_t* next, cudaStream_t stream);
 
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)
 struct ResampleArgs {

@@ -52,7 +52,15 @@ EXPORTS = [
     "rs_enable_kernel_timing", "rs_kernel_timing", "rs_stage_rows",
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
+    "rs_set_ngram_lm", "rs_ngram_lm_eval",
 ]
+
+
+class RsNgramLM(C.Structure):
+    """include/rs_engine.h rs_ngram_lm"""
+    _fields_ = [("order", C.c_int), ("n_states", C.c_int), ("n_arcs", C.c_int), ("pitch", C.c_int), ("start_state", C.c_int),
+                ("cb", C.c_void_p), ("chain", C.c_void_p), ("arc_begin", C.c_void_p), ("arc_tok", C.c_void_p),
+                ("arc_to", C.c_void_p), ("arc_w", C.c_void_p), ("uni_w", C.c_void_p), ("uni_to", C.c_void_p)]
 
 
 def load_library(build_if_missing: bool = True) -> C.CDLL:
@@ -91,6 +99,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_transcribe_device_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
     lib.rs_transcribe_batch_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
     lib.rs_set_phrase_boosting.argtypes = [vp, vp, vp, ip, ip]
+    lib.rs_set_ngram_lm.argtypes = [vp, C.POINTER(RsNgramLM)]
+    lib.rs_ngram_lm_eval.argtypes = [vp, vp, vp, ip, vp, vp, vp]
     lib.rs_rnnt_alsd.argtypes = [vp, vp, vp, ip, ip, ip, C.c_float, ip, ip, vp, vp, vp, vp, ip, vp]
     lib.rs_rnnt_alsd.restype = ip
     lib.rs_resample_mono.argtypes = [vp, vp, ip, vp, ip, ip, ip, vp, ip, ip, ip, ip, ip, vp, ip, vp, vp]
@@ -118,7 +128,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     for fn in ("rs_workspace_bytes", "rs_set_workspace", "rs_mel_frames", "rs_enc_frames", "rs_mel_valid", "rs_enc_valid", "rs_logmel", "rs_encode",
                "rs_rnnt_greedy", "rs_transcribe_device", "rs_transcribe_batch", "rs_transcribe_device_pcm16", "rs_transcribe_batch_pcm16",
                "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
-               "rs_set_phrase_boosting", "rs_gemm_bf16", "rs_layernorm", "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
+               "rs_set_phrase_boosting", "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_gemm_bf16", "rs_layernorm", "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
                "rs_enable_stage_timing", "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing"):
         getattr(lib, fn).restype = ip
     _lib = lib
@@ -284,6 +294,7 @@ class Engine:
         self._ws: Optional[torch.Tensor] = None
         self._ws_key: Tuple[int, int] = (0, 0)
         self._boost: Optional[Tuple[torch.Tensor, torch.Tensor]] = None
+        self._lm: Optional[Dict[str, torch.Tensor]] = None
 
     def __del__(self):
         h = getattr(self, "h", None)
@@ -332,6 +343,32 @@ class Engine:
             self._check(self.lib.rs_set_phrase_boosting(self.h, new[0].data_ptr(), new[1].data_ptr(), new[0].shape[0], new[0].shape[1]),
                         "rs_set_phrase_boosting")
         self._boost = new
+
+    def set_ngram_lm(self, tables) -> None:
+        """n-gram LM shallow fusion of every greedy decode (rs_set_ngram_lm): ``tables`` an ``ngram_lm.NgramLMTables``, or
+        ``None`` to clear.  The engine keeps its device copies alive while they are set; replacing or clearing a table first
+        waits for the work queued on this device's current stream, which may still read the old one."""
+        new = None
+        if tables is not None:
+            dtypes = {"cb": torch.float32, "arc_w": torch.float32, "uni_w": torch.float32}
+            new = {k: torch.as_tensor(v).to(self.device, dtypes.get(k, torch.int32)).contiguous()
+                   for k, v in tables.device_arrays().items()}
+            lm = RsNgramLM(int(tables.order), int(tables.n_states), int(tables.n_arcs), int(tables.pitch), int(tables.start_state),
+                           *[new[k].data_ptr() for k in ("cb", "chain", "arc_begin", "arc_tok", "arc_to", "arc_w", "uni_w", "uni_to")])
+        if self._lm is not None:
+            torch.cuda.current_stream(self.device).synchronize()
+        self._check(self.lib.rs_set_ngram_lm(self.h, None if new is None else C.byref(lm)), "rs_set_ngram_lm")
+        self._lm = new
+
+    def ngram_lm_eval(self, states: torch.Tensor, tokens: torch.Tensor):
+        """The decode kernel's LM lookup on (state, token) pairs (rs_ngram_lm_eval) -> (score f32, next i32) device tensors."""
+        states = states.to(self.device, torch.int32).contiguous()
+        tokens = tokens.to(self.device, torch.int32).contiguous()
+        score = torch.empty(states.shape, dtype=torch.float32, device=self.device)
+        nxt = torch.empty(states.shape, dtype=torch.int32, device=self.device)
+        self._check(self.lib.rs_ngram_lm_eval(self.h, states.data_ptr(), tokens.data_ptr(), states.numel(), score.data_ptr(),
+                                              nxt.data_ptr(), self._stream()), "rs_ngram_lm_eval")
+        return score, nxt
 
     def mel_frames(self, n: int) -> int:
         return self.lib.rs_mel_frames(self.h, n)

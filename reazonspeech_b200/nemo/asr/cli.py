@@ -17,6 +17,11 @@ Second extension, phrase boosting (reazonspeech_b200/boosting.py): the greedy de
   --phrases=FILE       UTF-8 text, one phrase per line (blank lines ignored)
   --phrase-score=L     bonus per phrase token in logit units, L > 0 (default 2.0; alone, without --phrases, it boosts nothing)
 With neither option the output is unchanged.
+Third extension, n-gram LM shallow fusion (reazonspeech_b200/ngram_lm.py): the greedy decode adds alpha * ln(10) * log10 P(k | h)
+of an ARPA LM over BPE token ids (words chr(token id + 100)) to every non-blank logit
+  --lm=FILE            the ARPA file
+  --lm-alpha=A         the LM weight, A > 0; required with --lm (there is no default)
+With neither option the output is unchanged.
 Audio decoding: soundfile when installed, scipy for WAV, librosa for compressed containers, see audio.audio_from_path.
 """
 import dataclasses
@@ -27,7 +32,7 @@ from dataclasses import dataclass, field
 from typing import List, Optional
 
 SHORT_OPTS = "ho:"
-LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=")
+LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=")
 
 
 @dataclass
@@ -38,6 +43,8 @@ class Options:
     audio: List[str] = field(default_factory=list)
     phrases: Optional[str] = None
     phrase_score: Optional[float] = None
+    lm: Optional[str] = None
+    lm_alpha: Optional[float] = None
 
 
 def parse(argv) -> Options:
@@ -55,6 +62,13 @@ def parse(argv) -> Options:
             opt.phrases = value
         if flag == "--phrase-score":
             opt.phrase_score = float(value)
+        if flag == "--lm":
+            opt.lm = value
+        if flag == "--lm-alpha":
+            opt.lm_alpha = float(value)
+    if (opt.lm is None) != (opt.lm_alpha is None):
+        raise ValueError("--lm and --lm-alpha go together: the LM weight has no default (try values around 0.3-0.5 and tune "
+                         "on held-out audio)" if opt.lm is not None else "--lm-alpha needs an LM: --lm=FILE")
     return opt
 
 
@@ -76,7 +90,13 @@ def run(opt: Options) -> None:
         boosting = PhraseBoostingConfig(load_phrases(opt.phrases) if opt.phrases is not None else [])
         if opt.phrase_score is not None:
             boosting.score = opt.phrase_score
-    model = load_model() if boosting is None else load_model(boosting=boosting)
+    extra = {}
+    if boosting is not None:
+        extra["boosting"] = boosting
+    if opt.lm is not None:
+        from ...ngram_lm import NgramLMConfig
+        extra["lm"] = NgramLMConfig(opt.lm, opt.lm_alpha)
+    model = load_model(**extra)
     results = transcribe_batch(model, clips) if len(clips) > 1 else [transcribe(model, clips[0])]
     with sink:
         out = get_writer(sink, opt.fmt)

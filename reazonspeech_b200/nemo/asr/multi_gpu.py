@@ -34,6 +34,15 @@ class MultiGpuRnntModel:
         self.max_batch = self.replicas[0].max_batch
         self.confidence = getattr(self.replicas[0], "confidence", None)
         self.boosting = getattr(self.replicas[0], "boosting", None)
+        self.lm = getattr(self.replicas[0], "lm", None)
+
+    def set_ngram_lm(self, lm) -> None:
+        """``B200RnntModel.set_ngram_lm`` on every replica: the tables are built once and uploaded once per device."""
+        from .transcribe import lm_tables
+        tables = lm_tables(self, lm)
+        for r in self.replicas:
+            r.set_ngram_lm_tables(tables, lm)
+        self.lm = lm
 
     def set_phrase_boosting(self, boosting) -> None:
         """``B200RnntModel.set_phrase_boosting`` on every replica: the tables are built once and uploaded once per device."""

@@ -22,6 +22,7 @@ from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables
 from ...config import ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
 from ...engine import Engine
+from ...ngram_lm import NgramLMConfig, NgramLMTables, build_lm_tables
 from ...tokenizer import PieceTableTokenizer, SentencePieceTokenizer, synthetic_pieces
 from ...weights import load_nemo_archive, random_state_dict
 from .audio import SAMPLERATE, norm_audio, pad_audio
@@ -129,7 +130,8 @@ class B200RnntModel:
     """Engine + tokenizer behind NeMo's model surface."""
 
     def __init__(self, engine: Engine, tokenizer, max_batch: int = 64, decoding: str = "greedy", beam_size: int = 4,
-                 confidence: Optional[ConfidenceConfig] = None, boosting: Optional[PhraseBoostingConfig] = None):
+                 confidence: Optional[ConfidenceConfig] = None, boosting: Optional[PhraseBoostingConfig] = None,
+                 lm: Optional[NgramLMConfig] = None):
         self.engine = engine
         self.cfg = engine.cfg
         self.tokenizer = tokenizer
@@ -143,6 +145,19 @@ class B200RnntModel:
         self.boosting: Optional[PhraseBoostingConfig] = None
         if boosting is not None:
             self.set_phrase_boosting(boosting)
+        self.lm: Optional[NgramLMConfig] = None
+        if lm is not None:
+            self.set_ngram_lm(lm)
+
+    def set_ngram_lm(self, lm: Optional[NgramLMConfig]) -> None:
+        """Fuse the n-gram LM of ``lm`` into every following greedy decode (ngram_lm.py), or stop with None.  Call it between
+        calls, not while one is running."""
+        self.set_ngram_lm_tables(lm_tables(self, lm), lm)
+
+    def set_ngram_lm_tables(self, tables: Optional[NgramLMTables], lm: Optional[NgramLMConfig]) -> None:
+        """Upload tables already built from ``lm`` (the multi-GPU model builds them once for all replicas)."""
+        self.engine.set_ngram_lm(tables)
+        self.lm = lm
 
     def set_phrase_boosting(self, boosting: Optional[PhraseBoostingConfig]) -> None:
         """Boost the phrases of ``boosting`` in every following greedy decode (boosting.py), or stop with None.  Call it
@@ -278,6 +293,15 @@ def boosting_tables(model, boosting: Optional[PhraseBoostingConfig]) -> Optional
     return build_tables(boosting, model.cfg.vocab_size, model.tokenizer)
 
 
+def lm_tables(model, lm: Optional[NgramLMConfig]) -> Optional[NgramLMTables]:
+    """Validated tables of ``lm`` for ``model``'s vocabulary (None: fusion off)."""
+    if lm is None:
+        return None
+    if getattr(model, "decoding", "greedy") != "greedy":
+        raise ValueError("n-gram LM fusion is applied by the greedy decode only (not by ALSD beam search)")
+    return build_lm_tables(lm, model.cfg.vocab_size)
+
+
 def _items(done, B: int):
     """Host outputs of one engine call -> per utterance (tokens, frames), or (tokens, frames, stats) with the statistics."""
     tokens, frames, ntok = done[:3]
@@ -301,7 +325,7 @@ def _find_checkpoint() -> Optional[str]:
 def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Optional[bool] = None,
                config: Optional[ModelConfig] = None, seed: int = 0, max_batch: int = 64, devices: Optional[Sequence] = None,
                decoding: str = "greedy", beam_size: int = 4, confidence: Optional[ConfidenceConfig] = None,
-               boosting: Optional[PhraseBoostingConfig] = None):
+               boosting: Optional[PhraseBoostingConfig] = None, lm: Optional[NgramLMConfig] = None):
     """Load the ReazonSpeech FastConformer-RNNT onto a B200.
 
     ``device``: None / "cuda" / "cuda:N" as in the reference (transcribe.py:9-22, eval.py:26).
@@ -315,7 +339,9 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     architecture are used instead -- the only option offline.  ``confidence``: a ``ConfidenceConfig`` turns on token / word
     confidence and log-probability scores of the greedy decode (``confidence.py``); not available with ``decoding="alsd"``.
     ``boosting``: a ``PhraseBoostingConfig`` boosts its key phrases in the greedy decode (``boosting.py``); change or clear
-    them later with ``model.set_phrase_boosting``; not available with ``decoding="alsd"``."""
+    them later with ``model.set_phrase_boosting``; not available with ``decoding="alsd"``.
+    ``lm``: an ``NgramLMConfig`` fuses its ARPA n-gram LM into the greedy decode (``ngram_lm.py``); change or clear it later
+    with ``model.set_ngram_lm``; not available with ``decoding="alsd"``."""
     if confidence is not None:
         if decoding == "alsd":
             raise ValueError("confidence is computed by the greedy decode only (NeMo offers none for beam search)")
@@ -324,6 +350,10 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
         if decoding == "alsd":
             raise ValueError("phrase boosting is applied by the greedy decode only (not by ALSD beam search)")
         boosting.validate()
+    if lm is not None:
+        if decoding == "alsd":
+            raise ValueError("n-gram LM fusion is applied by the greedy decode only (not by ALSD beam search)")
+        lm.validate()
     if device is None:
         device = "cuda"
     if str(device).startswith("cpu"):
@@ -350,7 +380,7 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
         raise ValueError(f"decoding must be 'greedy' or 'alsd', got {decoding!r}")
     if devices is None:
         return B200RnntModel(Engine(cfg, sd, str(device), alsd=decoding == "alsd"), tokenizer, max_batch=max_batch, decoding=decoding, beam_size=beam_size,
-                             confidence=confidence, boosting=boosting)
+                             confidence=confidence, boosting=boosting, lm=lm)
     if decoding != "greedy":
         raise ValueError("the one-process multi-GPU model decodes greedily; load one model per device for beam search")
     names = [d if isinstance(d, str) else f"cuda:{int(d)}" for d in devices]
@@ -363,6 +393,8 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
                                for n in names])
     if boosting is not None:
         model.set_phrase_boosting(boosting)
+    if lm is not None:
+        model.set_ngram_lm(lm)
     return model
 
 
