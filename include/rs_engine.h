@@ -215,6 +215,26 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev,
                  float u_max_ratio, int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev,
                  int32_t* n_dev, double* score_dev, int U_cap, void* stream);
 
+/* Forced alignment of given label sequences on the standard RNN-T lattice (semantics: reazonspeech_b200/alignment.py):
+ * enc f32[B,T_max,d_model] + enc_len, labels i32[B,U_max] + label_len i32[B] (device) ->
+ * frames i32[B,U_max] (emission frame of each token on the Viterbi path), token_lp f32[B,U_max] (the token's lattice
+ * log-probability lp_emit[frame][u - 1] on that path), viterbi f32[B] (the Viterbi path's log-probability), loglik f32[B]
+ * (log P(y|x) = -RNN-T loss).  Entries at or beyond label_len[b] hold frame -1 and NaN.  An utterance with a label outside
+ * [0, vocab_size), label_len outside [0, U_max] or enc_len outside [1, T_max] gets NaN scores and frames -1; the others are
+ * unaffected.  Scratch (the lattice, 8 bytes + 1 per cell of B x T_max x (U_max + 1), and the predictor rows) is engine-owned
+ * and grown on demand like the ALSD workspace (RS_ERR_WORKSPACE when that allocation fails: a 10-minute clip is about 200 MB;
+ * callers chunk longer inputs); rs_workspace_bytes is unchanged.  U_max <= 14527 (the DP keeps two anti-diagonals in shared
+ * memory; RS_ERR_UNSUPPORTED beyond).  Works with or without the alsd.* tensors, and ignores phrase boosting and the LM.
+ * Asynchronous on stream, except that growing the scratch synchronises it. */
+int rs_rnnt_align(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max,
+                  const int32_t* labels_dev, const int32_t* label_len_dev, int U_max,
+                  int32_t* frames_dev, float* token_lp_dev, float* viterbi_dev, float* loglik_dev, void* stream);
+/* Test seam: the lattice alone -> lp_blank / lp_emit f32[B, T_max, U_max + 1] (cells outside an utterance untouched;
+ * lp_emit[t][label_len] = -inf: no label left to emit). */
+int rs_rnnt_align_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max,
+                          const int32_t* labels_dev, const int32_t* label_len_dev, int U_max,
+                          float* lp_blank_dev, float* lp_emit_dev, void* stream);
+
 /* norm_audio on the device (pkg/nemo-asr/src/audio.py:54-68: resample to 16 kHz, then average the channels) fused with
  * transcribe()'s padding (audio.py:70-83): in [B, channels, L_in_max] f32 or int16 PCM at the native rate ->
  * out f32 [B, L_out_row], row b = pad zeros | resampled mono utterance | zeros, len_out[b] = resampled length + 2 pad;

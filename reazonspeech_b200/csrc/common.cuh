@@ -55,6 +55,26 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t v) {
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
 
+// fp32 pair -> two IEEE-half pairs with hi + lo == x to 22 mantissa bits (11 + 11): the residual x - hi is exact in
+// fp32 and is itself rounded to half.  The number of terms is what the joint costs: two half terms, not three bf16 ones.
+// Magnitudes are clamped to the largest finite half before each conversion, which extends the exactly covered
+// range to |x| <= 2 * 65504; a transducer joint / LSTM input beyond that is outside what NeMo itself runs in fp16 AMP.
+__device__ __forceinline__ void split2(float2 x, uint32_t& hi, uint32_t& lo) {
+  constexpr float kMax = 65504.f;
+  const __half2 h = __floats2half2_rn(fminf(fmaxf(x.x, -kMax), kMax), fminf(fmaxf(x.y, -kMax), kMax));
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(fminf(fmaxf(x.x - hf.x, -kMax), kMax), fminf(fmaxf(x.y - hf.y, -kMax), kMax));
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+// bf16 weight pair -> half pair.  Exact for 2^-14 <= |w| < 65504 (bf16 carries 8 mantissa bits, half 11); smaller
+// magnitudes become half subnormals (absolute error < 2^-25), which is below the fp32 summation noise of a logit.
+__device__ __forceinline__ uint32_t bf16x2_to_f16x2(uint32_t v) { return pack_f16x2(bf16_lo(v), bf16_hi(v)); }
+__device__ __forceinline__ uint4 bf16x8_to_f16x8(uint4 v) {
+  return make_uint4(bf16x2_to_f16x2(v.x), bf16x2_to_f16x2(v.y), bf16x2_to_f16x2(v.z), bf16x2_to_f16x2(v.w));
+}
+
 // 1 / (1 + 2^(-x log2 e)) on the two special-function instructions alone (ex2.approx.ftz, rcp.approx.ftz: 5 instructions
 // with the swish multiply).  __expf / __fdividef wrap the same two in range fix-ups for denormal results (8 instructions);
 // here a denormal e^-x flushes to 0 (sigmoid = 1 exactly) and an overflowing one gives rcp(inf) = 0, both the right limits.

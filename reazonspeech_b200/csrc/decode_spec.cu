@@ -153,26 +153,6 @@ __device__ __forceinline__ void mma_f16_16816(float (&d)[4], const uint32_t (&a)
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// fp32 pair -> two IEEE-half pairs with hi + lo == x to 22 mantissa bits (11 + 11): the residual x - hi is exact in
-// fp32 and is itself rounded to half.  The number of terms is what the joint costs: two half terms, not three bf16 ones.
-// Magnitudes are clamped to the largest finite half before each conversion, which extends the exactly covered
-// range to |x| <= 2 * 65504; a transducer joint / LSTM input beyond that is outside what NeMo itself runs in fp16 AMP.
-__device__ __forceinline__ void split2(float2 x, uint32_t& hi, uint32_t& lo) {
-  constexpr float kMax = 65504.f;
-  const __half2 h = __floats2half2_rn(fminf(fmaxf(x.x, -kMax), kMax), fminf(fmaxf(x.y, -kMax), kMax));
-  const float2 hf = __half22float2(h);
-  const __half2 l = __floats2half2_rn(fminf(fmaxf(x.x - hf.x, -kMax), kMax), fminf(fmaxf(x.y - hf.y, -kMax), kMax));
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
-// bf16 weight pair -> half pair.  Exact for 2^-14 <= |w| < 65504 (bf16 carries 8 mantissa bits, half 11); smaller
-// magnitudes become half subnormals (absolute error < 2^-25), which is below the fp32 summation noise of a logit.
-__device__ __forceinline__ uint32_t bf16x2_to_f16x2(uint32_t v) { return pack_f16x2(bf16_lo(v), bf16_hi(v)); }
-__device__ __forceinline__ uint4 bf16x8_to_f16x8(uint4 v) {
-  return make_uint4(bf16x2_to_f16x2(v.x), bf16x2_to_f16x2(v.y), bf16x2_to_f16x2(v.z), bf16x2_to_f16x2(v.w));
-}
-
 __device__ __forceinline__ float2 ldcg2(const float* p) { return __ldcg(reinterpret_cast<const float2*>(p)); }
 __device__ __forceinline__ float4 ldcg4s(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
 

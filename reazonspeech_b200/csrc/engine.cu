@@ -73,6 +73,9 @@ struct rs_engine {
   void* alsd_ws = nullptr;
   size_t alsd_ws_bytes = 0;
   int* alsd_done_host = nullptr;
+  // forced alignment (align.cu): scratch grown on demand like the ALSD workspace
+  void* align_ws = nullptr;
+  size_t align_ws_bytes = 0;
   unsigned int* lm_tickets = nullptr;   // per-utterance CTA tickets of the log-mel statistics (engine-owned, kept zero between launches)
   static constexpr int kMaxBatch = 1 << 16;
   struct { const float *c0w, *c0b, *d1w, *d1b, *p1b, *d2w, *d2b, *p2b, *ob; const void *p1w, *p2w, *ow; } sub;
@@ -479,6 +482,7 @@ void rs_engine_destroy(rs_engine* e) {
   for (auto& ev : e->log_ev) cudaEventDestroy(ev);
   cudaFree(e->lm_tickets);
   cudaFree(e->alsd_ws);
+  cudaFree(e->align_ws);
   if (e->alsd_done_host) cudaFreeHost(e->alsd_done_host);
   delete e;
 }
@@ -816,6 +820,79 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
   RS_LAUNCH(e, s, 1, rs::alsd_launch_output(st, B, blank, y_dev, step_dev, n_dev, score_dev, U_cap, s));
   RS_CUDA(e, cudaStreamSynchronize(s));
   return RS_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Forced alignment (align.cu; semantics: reazonspeech_b200/alignment.py).  lp_blank / lp_emit set: the lattice seam (the
+// caller's buffers, no DP); otherwise the lattice lives in the scratch and the DP writes frames / token_lp / viterbi / loglik.
+int rnnt_align(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, const int32_t* labels,
+               const int32_t* label_len, int U_max, float* lp_blank, float* lp_emit, int32_t* frames, float* token_lp, float* viterbi,
+               float* loglik, cudaStream_t s) {
+  const bool seam = lp_blank != nullptr;
+  if (!e || !enc || !enc_len || !labels || !label_len || B <= 0 || T_max <= 0 || U_max <= 0 ||
+      (seam ? lp_emit == nullptr : (!frames || !token_lp || !viterbi || !loglik)))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  const rs_model_config& c = e->cfg;
+  char msg[256] = "";
+  if (!rs::align_supported(c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, msg)) return fail(e, RS_ERR_UNSUPPORTED, "%s: %s", fn, msg);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  Nvtx range("rs::rnnt_align");
+  const int M = B * T_max, U1 = U_max + 1, Hj = c.joint_hidden, Hp = c.pred_hidden;
+  const size_t cells = static_cast<size_t>(M) * U1;
+  rs::Arena a;
+  const size_t o_xn = a.take(static_cast<size_t>(M) * c.d_model * 2), o_encp = a.take(static_cast<size_t>(M) * Hj * 4);
+  const size_t o_h = a.take(static_cast<size_t>(B) * U1 * Hp * 4), o_c = a.take(static_cast<size_t>(B) * Hp * 4);
+  const size_t o_pp = a.take(static_cast<size_t>(B) * U1 * Hj * 4);
+  size_t o_lpb = 0, o_lpe = 0, o_ch = 0;
+  if (!seam) { o_lpb = a.take(cells * 4); o_lpe = a.take(cells * 4); o_ch = a.take(cells); }
+  if (a.off > e->align_ws_bytes) {
+    RS_CUDA(e, cudaStreamSynchronize(s));
+    cudaFree(e->align_ws); e->align_ws = nullptr; e->align_ws_bytes = 0;
+    if (cudaMalloc(&e->align_ws, a.off) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(e, RS_ERR_WORKSPACE, "%s: cannot allocate %zu bytes of alignment scratch (chunk long inputs)", fn, a.off);
+    }
+    e->align_ws_bytes = a.off;
+  }
+  char* ws = static_cast<char*>(e->align_ws);
+  rs::AlignArgs g{reinterpret_cast<float*>(ws + o_encp), enc_len, labels, label_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w,
+                  e->dec.gate_tab, e->dec.pred_w, e->dec.pred_b, B, T_max, U_max, Hj, Hp, c.vocab_size,
+                  reinterpret_cast<float*>(ws + o_h), reinterpret_cast<float*>(ws + o_c), reinterpret_cast<float*>(ws + o_pp),
+                  seam ? lp_blank : reinterpret_cast<float*>(ws + o_lpb), seam ? lp_emit : reinterpret_cast<float*>(ws + o_lpe),
+                  reinterpret_cast<uint8_t*>(ws + o_ch), frames, token_lp, viterbi, loglik};
+  // joint.enc over every frame, as in the greedy path
+  RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, ws + o_xn, static_cast<int64_t>(M) * c.d_model, s));
+  RS_TRY(gemm(e, {ws + o_xn, e->dec.enc_w, e->dec.enc_b, nullptr, ws + o_encp, M, Hj, c.d_model, RS_EPI_BIAS_F32, 1.f}, s));
+  for (int u = 0; u <= U_max; ++u) RS_LAUNCH(e, s, 1, rs::launch_align_lstm_step(g, u, s));
+  RS_LAUNCH(e, s, 1, rs::launch_align_pred_proj(g, s));
+  {
+    const int r = launch(e, s, "rnnt_lattice_kernel", 1, 0.0, [&] { return rs::launch_rnnt_lattice(g, s, msg); });
+    if (r != RS_OK && msg[0] != '\0') return fail(e, r, "%s: %s", fn, msg);
+    RS_TRY(r);
+  }
+  if (!seam) RS_LAUNCH(e, s, 1, rs::launch_rnnt_align_dp(g, s));
+  return RS_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rs_rnnt_align(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, const int32_t* labels_dev,
+                  const int32_t* label_len_dev, int U_max, int32_t* frames_dev, float* token_lp_dev, float* viterbi_dev,
+                  float* loglik_dev, void* stream) {
+  return rnnt_align(e, "rs_rnnt_align", enc_dev, enc_len_dev, B, T_max, labels_dev, label_len_dev, U_max, nullptr, nullptr, frames_dev,
+                    token_lp_dev, viterbi_dev, loglik_dev, static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_align_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, const int32_t* labels_dev,
+                          const int32_t* label_len_dev, int U_max, float* lp_blank_dev, float* lp_emit_dev, void* stream) {
+  if (lp_blank_dev == nullptr || lp_emit_dev == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_align_lattice: bad arguments");
+  return rnnt_align(e, "rs_rnnt_align_lattice", enc_dev, enc_len_dev, B, T_max, labels_dev, label_len_dev, U_max, lp_blank_dev, lp_emit_dev,
+                    nullptr, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int rs_resample_mono(rs_engine* e, const void* in_dev, int in_is_pcm16, const int32_t* len_in_dev, int B, int channels, int L_in_max,

@@ -116,6 +116,35 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
 cudaError_t launch_ngram_lm_eval(const NgramLM& lm, int V, int num_sms, const int32_t* states, const int32_t* tokens, int n,
                                  float* score, int32_t* next, cudaStream_t stream);
 
+// Forced alignment on the RNN-T lattice (align.cu; semantics: reazonspeech_b200/alignment.py).  Lattice arrays are
+// [B][T_max][U_max + 1]; labels [B][U_max]; h / pred_proj [B][U_max + 1][Hp / Hj]; c [B][Hp].
+struct AlignArgs {
+  const float* enc_proj;      // f32 [B*T_max, Hj]  (joint.enc applied to every frame)
+  const int32_t* enc_len;
+  const int32_t* labels;
+  const int32_t* label_len;
+  const void* w_out;          // bf16 [V+1, Hj]
+  const float* b_out;         // f32 [V+1]
+  const void* w_lstm;         // bf16 [4*Hp, 2*Hp]  (W_ih | W_hh, gate order i,f,g,o)
+  const float* gate_tab;      // f32 [V+1, 4*Hp]
+  const void* w_pred;         // bf16 [Hj, Hp]
+  const float* b_pred;        // f32 [Hj]
+  int B, T_max, U_max, Hj, Hp, V;
+  float* h; float* c; float* pred_proj;
+  float* lp_blank; float* lp_emit;
+  uint8_t* choice;            // Viterbi predecessor of every cell (1: the emission from (t, u - 1))
+  int32_t* frames; float* token_lp; float* viterbi; float* loglik;
+};
+// shapes the kernels implement (false: err, >= 256 B, says why)
+bool align_supported(int Hj, int Hp, int V, int U_max, char* err);
+// teacher-forced predictor step u (h, c) and then joint.pred of every row
+cudaError_t launch_align_lstm_step(const AlignArgs& a, int u, cudaStream_t stream);
+cudaError_t launch_align_pred_proj(const AlignArgs& a, cudaStream_t stream);
+// lp_blank / lp_emit of every valid cell (err >= 256 B receives a tensor-map failure)
+cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* err);
+// forward + Viterbi recursions and backtrace -> frames, token_lp, viterbi, loglik
+cudaError_t launch_rnnt_align_dp(const AlignArgs& a, cudaStream_t stream);
+
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)
 struct ResampleArgs {
   const void* in; bool in_i16;          // [B, C, L_in_max] f32, or int16 PCM (scaled by 2^-15)

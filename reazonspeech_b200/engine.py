@@ -52,7 +52,7 @@ EXPORTS = [
     "rs_enable_kernel_timing", "rs_kernel_timing", "rs_stage_rows",
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
-    "rs_set_ngram_lm", "rs_ngram_lm_eval",
+    "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice",
 ]
 
 
@@ -103,6 +103,10 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_ngram_lm_eval.argtypes = [vp, vp, vp, ip, vp, vp, vp]
     lib.rs_rnnt_alsd.argtypes = [vp, vp, vp, ip, ip, ip, C.c_float, ip, ip, vp, vp, vp, vp, ip, vp]
     lib.rs_rnnt_alsd.restype = ip
+    lib.rs_rnnt_align.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp]
+    lib.rs_rnnt_align.restype = ip
+    lib.rs_rnnt_align_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp]
+    lib.rs_rnnt_align_lattice.restype = ip
     lib.rs_resample_mono.argtypes = [vp, vp, ip, vp, ip, ip, ip, vp, ip, ip, ip, ip, ip, vp, ip, vp, vp]
     lib.rs_resample_mono.restype = ip
     lib.rs_gemm_bf16.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, ip, ip, C.c_float, vp, ip, ip, vp]
@@ -485,6 +489,39 @@ class Engine:
                                           int(recombine_returns_input), y.data_ptr(), steps.data_ptr(), n.data_ptr(), score.data_ptr(), U,
                                           self._stream()), "rs_rnnt_alsd")
         return y, steps, n, score
+
+    def _align_inputs(self, enc, enc_len, labels, label_len):
+        B, T, _ = enc.shape
+        assert enc.dtype == torch.float32 and enc.is_contiguous() and enc_len.dtype == torch.int32
+        assert labels.dtype == torch.int32 and labels.dim() == 2 and labels.shape[0] == B and label_len.dtype == torch.int32
+        labels = labels.contiguous()
+        if labels.shape[1] == 0:                                 # every utterance has no label: one unused column
+            labels = torch.zeros(B, 1, dtype=torch.int32, device=self.device)
+        return B, T, labels, labels.shape[1]
+
+    def align(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor):
+        """Forced alignment of the label sequences labels[b, :label_len[b]] (rs_rnnt_align; semantics: alignment.py) ->
+        (frames i32 [B, U], token_lp f32 [B, U], viterbi f32 [B], loglik f32 [B]) device tensors."""
+        B, T, labels, U = self._align_inputs(enc, enc_len, labels, label_len)
+        frames = torch.empty(B, U, dtype=torch.int32, device=self.device)
+        token_lp = torch.empty(B, U, dtype=torch.float32, device=self.device)
+        viterbi = torch.empty(B, dtype=torch.float32, device=self.device)
+        loglik = torch.empty(B, dtype=torch.float32, device=self.device)
+        self._check(self.lib.rs_rnnt_align(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, labels.data_ptr(), label_len.data_ptr(), U,
+                                           frames.data_ptr(), token_lp.data_ptr(), viterbi.data_ptr(), loglik.data_ptr(),
+                                           self._stream()), "rs_rnnt_align")
+        return frames, token_lp, viterbi, loglik
+
+    def align_lattice(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor, out=None):
+        """The lattice alone (rs_rnnt_align_lattice) -> (lp_blank, lp_emit) f32 [B, T, U + 1]; cells outside an utterance keep
+        what ``out`` held (NaN for fresh buffers)."""
+        B, T, labels, U = self._align_inputs(enc, enc_len, labels, label_len)
+        if out is None:
+            out = (torch.full((B, T, U + 1), float("nan"), device=self.device), torch.full((B, T, U + 1), float("nan"), device=self.device))
+        lp_blank, lp_emit = out
+        self._check(self.lib.rs_rnnt_align_lattice(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, labels.data_ptr(), label_len.data_ptr(), U,
+                                                   lp_blank.data_ptr(), lp_emit.data_ptr(), self._stream()), "rs_rnnt_align_lattice")
+        return lp_blank, lp_emit
 
     def resample_mono(self, raw: torch.Tensor, lens: torch.Tensor, samplerate: int, pad: int = 0):
         """norm_audio on the device (pkg/nemo-asr/src/audio.py:54-68) + transcribe()'s padding: ``raw`` [B, C, L] float32 or

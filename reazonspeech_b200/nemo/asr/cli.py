@@ -22,6 +22,10 @@ of an ARPA LM over BPE token ids (words chr(token id + 100)) to every non-blank 
   --lm=FILE            the ARPA file
   --lm-alpha=A         the LM weight, A > 0; required with --lm (there is no default)
 With neither option the output is unchanged.
+Fourth extension, forced alignment of known transcripts (reazonspeech_b200/alignment.py): instead of transcribing, each AUDIO is
+aligned to its given transcript and the segments are written through the same writer with the same time offsets
+  --text=FILE          UTF-8 text, one transcript line per AUDIO argument, in order (a count mismatch is an error)
+Without the option the output is unchanged.
 Audio decoding: soundfile when installed, scipy for WAV, librosa for compressed containers, see audio.audio_from_path.
 """
 import dataclasses
@@ -32,7 +36,7 @@ from dataclasses import dataclass, field
 from typing import List, Optional
 
 SHORT_OPTS = "ho:"
-LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=")
+LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=")
 
 
 @dataclass
@@ -45,6 +49,7 @@ class Options:
     phrase_score: Optional[float] = None
     lm: Optional[str] = None
     lm_alpha: Optional[float] = None
+    text: Optional[str] = None
 
 
 def parse(argv) -> Options:
@@ -66,6 +71,8 @@ def parse(argv) -> Options:
             opt.lm = value
         if flag == "--lm-alpha":
             opt.lm_alpha = float(value)
+        if flag == "--text":
+            opt.text = value
     if (opt.lm is None) != (opt.lm_alpha is None):
         raise ValueError("--lm and --lm-alpha go together: the LM weight has no default (try values around 0.3-0.5 and tune "
                          "on held-out audio)" if opt.lm is not None else "--lm-alpha needs an LM: --lm=FILE")
@@ -76,11 +83,21 @@ def usage() -> None:
     print(__doc__, file=sys.stderr)
 
 
+def load_transcripts(path: str, n_audio: int) -> List[str]:
+    """--text: one UTF-8 transcript line per AUDIO argument; ValueError when the counts differ."""
+    with open(path, encoding="utf-8") as f:
+        lines = f.read().splitlines()
+    if len(lines) != n_audio:
+        raise ValueError(f"--text={path}: {len(lines)} transcript lines for {n_audio} AUDIO arguments")
+    return lines
+
+
 def run(opt: Options) -> None:
     from .audio import audio_from_path
-    from .transcribe import load_model, transcribe, transcribe_batch
+    from .transcribe import align_batch, load_model, transcribe, transcribe_batch
     from .writer import get_writer
 
+    texts = load_transcripts(opt.text, len(opt.audio)) if opt.text is not None else None
     sink = sys.stdout if opt.output is None else open(opt.output, "w")
     warnings.simplefilter("ignore")
     clips = [audio_from_path(path) for path in opt.audio]
@@ -97,7 +114,10 @@ def run(opt: Options) -> None:
         from ...ngram_lm import NgramLMConfig
         extra["lm"] = NgramLMConfig(opt.lm, opt.lm_alpha)
     model = load_model(**extra)
-    results = transcribe_batch(model, clips) if len(clips) > 1 else [transcribe(model, clips[0])]
+    if texts is not None:
+        results = align_batch(model, clips, texts)
+    else:
+        results = transcribe_batch(model, clips) if len(clips) > 1 else [transcribe(model, clips[0])]
     with sink:
         out = get_writer(sink, opt.fmt)
         out.write_header()

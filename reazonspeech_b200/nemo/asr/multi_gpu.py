@@ -23,7 +23,7 @@ from ...sharding import shard_indices
 
 class MultiGpuRnntModel:
     """``replicas``: ``B200RnntModel`` objects, one per device, same weights.  Duck-typed like a single replica:
-    ``iter_token_batches`` / ``transcribe_tokens`` / ``transcribe`` / ``tokenizer`` / ``cfg``."""
+    ``iter_token_batches`` / ``transcribe_tokens`` / ``transcribe`` / ``align_tokens`` / ``tokenizer`` / ``cfg``."""
 
     def __init__(self, replicas: Sequence):
         if len(replicas) == 0:
@@ -56,9 +56,10 @@ class MultiGpuRnntModel:
     def devices(self) -> List[str]:
         return [str(r.engine.device) for r in self.replicas]
 
-    def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
-        """Yields ``(indices, [(tokens, frames)])`` per finished engine batch of any device, indices into ``waveforms``
-        (``(tokens, frames, stats)`` items with confidence on, as ``B200RnntModel.iter_token_batches``)."""
+    def _deal(self, waveforms: Sequence[np.ndarray], batches):
+        """Deals the utterances across the replicas by length and yields ``(indices into waveforms, items)`` per finished
+        engine batch of any device; ``batches(replica, mine)`` runs on the replica's worker thread and yields the replica's
+        ``(indices into mine, items)``."""
         if len(waveforms) == 0:
             return
         shards = [s for s in shard_indices([len(w) for w in waveforms], len(self.replicas))]
@@ -66,8 +67,7 @@ class MultiGpuRnntModel:
 
         def work(replica, mine: List[int]):
             try:
-                sub = [waveforms[i] for i in mine]
-                for idx, items in replica.iter_token_batches(sub, pad):
+                for idx, items in batches(replica, mine):
                     out.put(([mine[j] for j in idx], items))
             except BaseException as exc:          # surfaced on the caller's thread: a dead device must not look like a slow one
                 out.put(exc)
@@ -90,6 +90,23 @@ class MultiGpuRnntModel:
             t.join()
         if error is not None:
             raise error
+
+    def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
+        """Yields ``(indices, [(tokens, frames)])`` per finished engine batch of any device, indices into ``waveforms``
+        (``(tokens, frames, stats)`` items with confidence on, as ``B200RnntModel.iter_token_batches``)."""
+        return self._deal(waveforms, lambda replica, mine: replica.iter_token_batches([waveforms[i] for i in mine], pad))
+
+    def align_tokens(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
+        """``B200RnntModel.align_tokens`` over all devices -> [(frames, token_lp, viterbi, loglik)] in input order."""
+        from ...alignment import validate_labels
+        token_lists = validate_labels(token_lists, self.cfg.vocab_size, len(waveforms))
+        results = [None] * len(waveforms)
+        batches = self._deal(waveforms, lambda replica, mine: replica.iter_align_batches([waveforms[i] for i in mine],
+                                                                                          [token_lists[i] for i in mine], pad))
+        for idx, items in batches:
+            for i, item in zip(idx, items):
+                results[i] = item
+        return results
 
     def transcribe_tokens(self, waveforms: Sequence[np.ndarray], pad: int = 0):
         """-> [(tokens, frames)] in input order."""

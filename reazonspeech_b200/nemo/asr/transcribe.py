@@ -18,6 +18,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
+from ...alignment import alignment_hypothesis, pack_labels, validate_labels
 from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables
 from ...config import ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
@@ -44,6 +45,8 @@ class Hypothesis:
     score: float = 0.0
     token_confidence: Optional[List[float]] = None
     word_confidence: Optional[List[float]] = None
+    log_likelihood: Optional[float] = None          # forced alignment: log P(y | x) of the given transcript (alignment.py)
+    token_logprob: Optional[List[float]] = None     # forced alignment: each token's log-probability on the Viterbi path
 
     @staticmethod
     def from_greedy(tokens: Sequence[int], frames: Sequence[int], blank: int) -> "Hypothesis":
@@ -251,6 +254,37 @@ class B200RnntModel:
                                           eng.transcribe_device(wav, wl, alpha=self.confidence.alpha))]
             yield idx, _items(done, len(idx))
 
+    # -- forced alignment of known transcripts (alignment.py)
+    def iter_align_batches(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
+        """16 kHz mono waveforms (``pad`` zero samples on both sides) and their token-id lists -> yields ``(indices, items)``
+        batch by batch, item = (frames, token_lp, viterbi, loglik) of one utterance: log-mel -> encode -> rs_rnnt_align.
+        Utterances are batched by length as in ``transcribe_alsd``; any ``decoding`` works."""
+        token_lists = validate_labels(token_lists, self.cfg.vocab_size, len(waveforms))
+        eng = self.engine
+        order = sorted(range(len(waveforms)), key=lambda i: len(waveforms[i]))
+        for lo in range(0, len(order), self.max_batch):
+            idx = order[lo:lo + self.max_batch]
+            wav, lens = self._staging[0].stage([waveforms[i] for i in idx], pad)
+            labels, label_len = pack_labels([token_lists[i] for i in idx])
+            with torch.cuda.device(eng.device):
+                x = wav.to(eng.device, non_blocking=True)
+                if x.dtype == torch.int16:
+                    x = x.to(torch.float32) * (1.0 / 32768.0)
+                mel, mel_len = eng.log_mel(x, lens.to(eng.device))
+                enc, enc_len = eng.encode(mel, mel_len)
+                frames, token_lp, viterbi, loglik = [a.cpu() for a in eng.align(enc, enc_len, torch.from_numpy(labels).to(eng.device),
+                                                                                 torch.from_numpy(label_len).to(eng.device))]
+            yield idx, [(frames[r, :n].tolist(), token_lp[r, :n].tolist(), float(viterbi[r]), float(loglik[r]))
+                        for r, n in enumerate(label_len.tolist())]
+
+    def align_tokens(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
+        """-> [(frames, token_lp, viterbi, loglik)] in input order (``iter_align_batches``)."""
+        results = [None] * len(waveforms)
+        for idx, items in self.iter_align_batches(waveforms, token_lists, pad):
+            for i, item in zip(idx, items):
+                results[i] = item
+        return results
+
     # -- NeMo's call shape (transcribe.py:48-53): already padded tensors
     def transcribe_alsd(self, waveforms: Sequence[np.ndarray], pad: int = 0) -> List[Hypothesis]:
         """ALSD beam search (NeMo's align_length_sync_decoding, the strategy reazonspeech-nemo-v2 ships with): hypotheses exactly
@@ -453,3 +487,37 @@ def transcribe_batch(model, audios: Sequence[AudioData], config: Optional[Transc
         for i, hyp in enumerate(hyps):
             finish(i, hyp)
     return out
+
+
+def _target_ids(model, text) -> List[int]:
+    """A transcript as token ids: a str is encoded like the model's training targets (``sentence_to_ids``), a sequence of
+    ints is taken as it is."""
+    return model.tokenizer.sentence_to_ids(text) if isinstance(text, str) else [int(k) for k in text]
+
+
+def align_batch(model, audios: Sequence[AudioData], texts: Sequence, config: Optional[TranscribeConfig] = None) -> List[TranscribeResult]:
+    """Forced alignment of known transcripts (alignment.py): ``texts[i]`` (a str, or a sequence of token ids) against
+    ``audios[i]``, results in input order.  The audio is prepared as ``transcribe`` prepares it (norm_audio, 0.5 s of silence
+    on both sides), and each result comes from the unchanged ``decode_hypothesis``: subwords are the given tokens, timed at
+    their Viterbi emission frames exactly as a transcription's tokens are.  ``result.hypothesis`` always carries the
+    alignment: score = the Viterbi path's log-probability, log_likelihood = log P(text | audio), token_logprob per token.
+    Bad token ids or a count mismatch raise ValueError before the GPU is touched."""
+    if config is None:
+        config = TranscribeConfig()
+    if len(texts) != len(audios):
+        raise ValueError(f"{len(texts)} transcripts for {len(audios)} audio inputs")
+    ids = validate_labels([_target_ids(model, t) for t in texts], model.cfg.vocab_size, len(audios))
+    pad = int(PAD_SECONDS * SAMPLERATE)
+    waves = [np.asarray(norm_audio(a).waveform) for a in audios]
+    out: List[TranscribeResult] = []
+    for k, (frames, token_lp, viterbi, loglik) in zip(ids, model.align_tokens(waves, ids, pad=pad)):
+        hyp = alignment_hypothesis(k, frames, token_lp, viterbi, loglik, model.cfg.blank)
+        result = decode_hypothesis(model, hyp)
+        result.hypothesis = hyp
+        out.append(result)
+    return out
+
+
+def align(model, audio: AudioData, text, config: Optional[TranscribeConfig] = None) -> TranscribeResult:
+    """One utterance of ``align_batch``."""
+    return align_batch(model, [audio], [text], config)[0]

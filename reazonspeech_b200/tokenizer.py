@@ -11,7 +11,10 @@ leading space) so a bare U+2581 decodes to the empty string exactly like the rea
 SentencePiece puts in front of a text dropped when it stands alone: a phrase inside a Japanese sentence carries no word
 boundary.  Known limitation: a phrase's segmentation alone may differ from its segmentation inside the sentences the model
 transcribes, and then boosting the phrase's ids favours a spelling the model would not produce; pass token-id sequences
-where that matters."""
+where that matters.
+
+``sentence_to_ids`` (forced alignment's tokenisation, alignment.py) encodes a whole sentence the way the model's training
+targets were encoded: SentencePiece's ``encode`` unchanged, the leading word-boundary piece kept."""
 from __future__ import annotations
 
 from typing import Iterable, List, Sequence
@@ -34,9 +37,9 @@ class PieceTableTokenizer:
     def ids_to_pieces(self, ids: Iterable[int]) -> List[str]:
         return [self.pieces[int(i)] for i in ids]
 
-    def text_to_ids(self, text: str) -> List[int]:
-        """Longest match over the pieces (SentencePiece's space handling: a leading boundary, spaces -> U+2581), a leading lone
-        U+2581 piece dropped.  A character no piece covers raises ValueError."""
+    def sentence_to_ids(self, text: str) -> List[int]:
+        """Longest match over the pieces with SentencePiece's space handling (a leading boundary, spaces -> U+2581), the
+        boundary piece kept.  A character no piece covers raises ValueError."""
         if not hasattr(self, "_index"):
             self._index = {}
             for i, piece in enumerate(self.pieces):
@@ -52,6 +55,12 @@ class PieceTableTokenizer:
                     break
             else:
                 raise ValueError(f"{text!r}: no piece covers {s[i]!r}")
+        return ids
+
+    def text_to_ids(self, text: str) -> List[int]:
+        """Longest match over the pieces (SentencePiece's space handling: a leading boundary, spaces -> U+2581), a leading lone
+        U+2581 piece dropped.  A character no piece covers raises ValueError."""
+        ids = self.sentence_to_ids(text)
         return _drop_lone_boundary(ids, self.pieces[ids[0]] if ids else "")
 
 
@@ -82,6 +91,13 @@ class SentencePieceTokenizer:
 
     def ids_to_pieces(self, ids: Iterable[int]) -> List[str]:
         return [self.sp.id_to_piece(int(i)) for i in ids]
+
+    def sentence_to_ids(self, text: str) -> List[int]:
+        """SentencePiece's ``encode`` unchanged (the leading U+2581 piece kept).  Text no piece covers raises ValueError."""
+        ids = [int(i) for i in self.sp.encode(text)]
+        if self.sp.unk_id() in ids:
+            raise ValueError(f"{text!r}: not covered by the piece table (encodes to <unk>)")
+        return ids
 
     def text_to_ids(self, text: str) -> List[int]:
         """SentencePiece's ``encode``, a leading lone U+2581 piece dropped."""
