@@ -210,10 +210,43 @@ int rs_ngram_lm_eval(rs_engine* e, const int32_t* states_dev, const int32_t* tok
  * Hypothesis.timestamp after NeMo's pack_hypotheses), n i32[B] tokens, score f64[B] (log-probability of the winner).
  * beam 1..8; u_max_ratio = alsd_max_target_len (NeMo: 2.0); score_norm: rank finished hypotheses by score / len(y);
  * recombine_returns_input: NeMo's recombine_hypotheses as recalled (adds duplicate scores, keeps the duplicates).
+ * u_max = int(u_max_ratio * T) is computed in double, as NeMo does (in float, 1.16 * 25 would round to 29 instead of 28).
+ * A finished hypothesis is ranked with the score recombination added into it in the step it finished, as NeMo's `final`
+ * list holds the same object as its beam.  n[b] is the winner's full length even when it exceeds U_cap; y and step then
+ * hold its first U_cap tokens.  enc_len[b] = 0 gives y = [blank], n = 0, score 0.
  * Needs the "alsd.*" weight tensors at rs_engine_create.  Synchronises before returning. */
 int rs_rnnt_alsd(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, int beam,
-                 float u_max_ratio, int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev,
+                 double u_max_ratio, int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev,
                  int32_t* n_dev, double* score_dev, int U_cap, void* stream);
+/* Test seam: rs_rnnt_alsd (the same launches and results) that also copies the search state into caller-owned device
+ * buffers.  R = B * beam rows; row r = b * beam + k is slot k of utterance b.  After the beam update of step i (the
+ * anti-diagonal t + u = i), for i < max_steps (later steps are not recorded; steps the search never ran are untouched):
+ *   n_hyp [i][b], beam_score / beam_u / beam_node [i][r]: the new beam (slot k < n_hyp: its log-probability, token count, back-pointer node);
+ *   row_t [i][r]: frame of the hypothesis in slot k of the previous beam scored at step i (-1: not scored);
+ *   cand_logp [i][r][9]: its log p(blank), then the beam best non-blank log-probabilities; cand_tok [i][r][8]: their classes;
+ *   has_final / final_key / final_score [i][b]: the best finished hypothesis so far (key = score / (u + 1) with score_norm).
+ * Once at the end, the back-pointer tree [B][node_pitch]: node 0 is the leading blank; node n > 0 is a token node_tok[n]
+ * emitted at step node_step[n] after node_parent[n].  node_pitch >= 1 + beam * (T_max + int(u_max_ratio * T_max) + 1);
+ * RS_ERR_INVALID_ARG before any launch otherwise, or when a buffer is NULL or max_steps < 0. */
+typedef struct rs_alsd_trace {
+  int32_t max_steps, node_pitch;
+  int32_t* n_hyp;         /* [max_steps][B] */
+  double* beam_score;     /* [max_steps][R] */
+  int32_t* beam_u;        /* [max_steps][R] */
+  int32_t* beam_node;     /* [max_steps][R] */
+  int32_t* row_t;         /* [max_steps][R] */
+  float* cand_logp;       /* [max_steps][R][9] */
+  int32_t* cand_tok;      /* [max_steps][R][8] */
+  int32_t* has_final;     /* [max_steps][B] */
+  double* final_key;      /* [max_steps][B] */
+  double* final_score;    /* [max_steps][B] */
+  int32_t* node_parent;   /* [B][node_pitch] */
+  int32_t* node_tok;      /* [B][node_pitch] */
+  int32_t* node_step;     /* [B][node_pitch] */
+} rs_alsd_trace;
+int rs_rnnt_alsd_trace(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, int beam,
+                       double u_max_ratio, int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev,
+                       int32_t* n_dev, double* score_dev, int U_cap, const rs_alsd_trace* trace, void* stream);
 
 /* Forced alignment of given label sequences on the standard RNN-T lattice (semantics: reazonspeech_b200/alignment.py):
  * enc f32[B,T_max,d_model] + enc_len, labels i32[B,U_max] + label_len i32[B] (device) ->

@@ -98,25 +98,22 @@ def alsd_beam(enc: torch.Tensor, sd: StateDict, cfg: ModelConfig, beam: int = 4,
         B = [BeamHyp([blank], 0.0, [-1], (torch.zeros(hp), torch.zeros(hp)))]
         final: List[BeamHyp] = []
         for i in range(T + u_max):
-            A: List[BeamHyp] = []
-            live = [(h, i - (len(h.y) - 1)) for h in B]
-            live = [(h, t) for h, t in live if t <= T - 1]
-            if not live:
-                break
-            for h, t in live:
+            rows = []
+            for h in B:
+                t = i - (len(h.y) - 1)
+                if t > T - 1:
+                    rows.append(None)
+                    continue
                 pp, state_after = predictor(h)
                 logp = torch.log_softmax(F.linear(torch.relu(ep[t] + pp), W, b), dim=-1)
-                stay = BeamHyp(h.y[:], h.score + float(logp[blank]), h.timestamp[:], h.state)
-                A.append(stay)
-                if t == T - 1:
-                    final.append(stay)
                 nb = torch.cat((logp[:blank], logp[blank + 1:]))              # beam_logp[:, ids]: every class but the blank
                 top = nb.topk(beam)
-                for lp, k in zip(top.values.tolist(), top.indices.tolist()):
-                    k = k + (1 if k >= blank else 0)                           # index back into the full class list
-                    A.append(BeamHyp(h.y + [k], h.score + lp, h.timestamp + [i], state_after))
-            B = sorted(A, key=lambda x: x.score, reverse=True)[:beam]          # stable, like Python's sorted in NeMo
-            B = _recombine(B, recombine_returns_input)
+                idx = [k + (1 if k >= blank else 0) for k in top.indices.tolist()]   # index back into the full class list
+                rows.append((float(logp[blank]), top.values.tolist(), idx, state_after))
+            B2 = alsd_step(B, rows, i, T, beam, recombine_returns_input, final)
+            if B2 is None:
+                break
+            B = B2
         pool = final if final else B
         key = (lambda x: x.score / len(x.y)) if score_norm else (lambda x: x.score)
         nbest = sorted(pool, key=key, reverse=True)
@@ -125,6 +122,31 @@ def alsd_beam(enc: torch.Tensor, sd: StateDict, cfg: ModelConfig, beam: int = 4,
                           best.score, nbest, from_final=bool(final))
     finally:
         torch.set_num_threads(n_threads)
+
+
+def alsd_step(B: List[BeamHyp], rows, i: int, T: int, beam: int, recombine_returns_input: bool, final: List[BeamHyp],
+              final_aliases_beam: bool = True) -> Optional[List[BeamHyp]]:
+    """One step (the anti-diagonal i = t + u) of align_length_sync_decoding.  rows[k] = (log p(blank), the `beam` best non-blank
+    log-probabilities, their class indices, the predictor state after y[-1]) of B[k] when it is live at step i (t = i - (len(y)
+    - 1) <= T - 1), anything otherwise.  Appends the stays at the last frame to ``final`` and returns the new beam, or None when
+    no hypothesis is live (the search ends).  As in NeMo, an entry of ``final`` is the very object that enters the beam, so
+    recombination in this step adds into it; final_aliases_beam=False records a copy instead, the score before recombination."""
+    A: List[BeamHyp] = []
+    for h, row in zip(B, rows):
+        t = i - (len(h.y) - 1)
+        if t > T - 1:
+            continue
+        lp_blank, values, indices, state_after = row
+        stay = BeamHyp(h.y[:], h.score + lp_blank, h.timestamp[:], h.state)
+        A.append(stay)
+        if t == T - 1:
+            final.append(stay if final_aliases_beam else BeamHyp(stay.y, stay.score, stay.timestamp, stay.state))
+        for lp, k in zip(values, indices):
+            A.append(BeamHyp(h.y + [k], h.score + lp, h.timestamp + [i], state_after))
+    if not A:
+        return None
+    B = sorted(A, key=lambda x: x.score, reverse=True)[:beam]              # stable, like Python's sorted in NeMo
+    return _recombine(B, recombine_returns_input)
 
 
 def _recombine(hyps: List[BeamHyp], returns_input: bool) -> List[BeamHyp]:

@@ -32,7 +32,7 @@ void alsd_layout_state(AlsdState& st, Arena& a, char* base, int B, int beam, int
 cudaError_t alsd_launch_init(const AlsdState& st, int B, int blank, cudaStream_t s);
 cudaError_t alsd_launch_rows(const AlsdState& st, int B, const float* enc_proj, const int32_t* enc_len, int T_max, int Hj, int step, void* planes, cudaStream_t s);
 cudaError_t alsd_launch_reduce(const AlsdState& st, int B, const float* logits, int ld, int V, cudaStream_t s);
-cudaError_t alsd_launch_select(const AlsdState& st, int B, const int32_t* enc_len, int step, float u_max_ratio, bool recombine_returns_input, cudaStream_t s);
+cudaError_t alsd_launch_select(const AlsdState& st, int B, const int32_t* enc_len, int step, double u_max_ratio, bool recombine_returns_input, cudaStream_t s);
 cudaError_t alsd_launch_lstm_in(const AlsdState& st, int B, const float* embed, int Hp, void* planes, cudaStream_t s);
 cudaError_t alsd_launch_cell(const AlsdState& st, int B, const float* gates, int Hp, void* planes, cudaStream_t s);
 cudaError_t alsd_launch_output(const AlsdState& st, int B, int blank, int32_t* y, int32_t* steps, int32_t* n, double* score, int U_cap, cudaStream_t s);

@@ -142,13 +142,14 @@ __device__ __forceinline__ double logaddexp(double a, double b) {
 }
 
 // grid (B), block 32 (lane 0 does the serial work: at most beam * (beam + 1) <= 72 candidates).
+// u_max = int(u_max_ratio * T) in double, as NeMo computes it: in fp32, ratio 1.16 at T = 25 gives 29 instead of 28.
 __global__ void __launch_bounds__(32)
-alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int step, float u_max_ratio, int recombine_returns_input) {
+alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int step, double u_max_ratio, int recombine_returns_input) {
   const int b = blockIdx.x;
   if (threadIdx.x != 0 || st.done[b]) return;
   const int K = st.beam;
   const int T = enc_len[b];
-  const int u_max = static_cast<int>(u_max_ratio * static_cast<float>(T));
+  const int u_max = static_cast<int>(u_max_ratio * static_cast<double>(T));
   const AlsdBeam& cur = st.cur;
   const int n_h = cur.n_hyp[b];
   // the search of utterance b ends: no kernel writes its beam again, so the next beam becomes a copy of the current one and
@@ -170,19 +171,15 @@ alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int 
   double a_score[kMaxBeam * (kMaxBeam + 1)];
   int a_par[kMaxBeam * (kMaxBeam + 1)], a_tok[kMaxBeam * (kMaxBeam + 1)];
   int n_a = 0;
+  bool any_final = false;                              // a stay at the last frame in this step
   for (int k = 0; k < n_h; ++k) {
     const int r = b * K + k;
     const int t = st.row_t[r];
     if (t < 0) continue;                               // past the last frame: dropped (it entered `final` when it got there)
+    any_final |= t == T - 1;
     const double s0 = cur.score[r];
     const double stay = s0 + static_cast<double>(st.cand_logp[r * (kMaxBeam + 1)]);
     a_score[n_a] = stay; a_par[n_a] = k; a_tok[n_a] = -1; ++n_a;
-    if (t == T - 1) {                                  // finished hypothesis: keep the best by score / len(y) (score_norm), first one on ties
-      const double key = st.score_norm ? stay / static_cast<double>(cur.u[r] + 1) : stay;
-      if (!st.has_final[b] || key > st.final_key[b]) {
-        st.has_final[b] = 1; st.final_key[b] = key; st.final_score[b] = stay; st.final_node[b] = cur.node[r]; st.final_u[b] = cur.u[r];
-      }
-    }
     for (int c = 0; c < K; ++c) {
       a_score[n_a] = s0 + static_cast<double>(st.cand_logp[r * (kMaxBeam + 1) + 1 + c]);
       a_par[n_a] = k; a_tok[n_a] = st.cand_tok[r * kMaxBeam + c]; ++n_a;
@@ -216,15 +213,31 @@ alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int 
   }
   // NeMo's recombine_hypotheses: the score of a later duplicate is added (logaddexp) into the first occurrence; as recalled, the
   // reference then returns its INPUT list, duplicates included (oracle/alsd_restated.py `recombine_returns_input`)
-  bool dropped[kMaxBeam];
-  for (int j = 0; j < n_new; ++j) dropped[j] = false;
+  bool dropped[kMaxBeam], later[kMaxBeam];                         // later: a duplicate of an earlier pick (merged into it)
+  for (int j = 0; j < n_new; ++j) dropped[j] = later[j] = false;
   for (int j = 1; j < n_new; ++j)
     for (int f = 0; f < j; ++f)
       if (!dropped[f] && n_hash[f] == n_hash[j] && n_len[f] == n_len[j]) {        // equal token sequences (64-bit sequence hash + length)
         n_score[f] = logaddexp(n_score[f], n_score[j]);
+        later[j] = true;
         if (!recombine_returns_input) dropped[j] = true;
         break;
       }
+  // finished hypotheses: the stays at the last frame, in A order, keep the best by score / len(y) (score_norm), first one on
+  // ties.  In the reference the entry of `final` is the very object that went into the beam, so a stay picked as the first of
+  // its sequence carries the score recombination added into it; any other stay keeps its own.  Only this step can change
+  // them: a stay at T - 1 is not live at the next one.
+  for (int a = 0; any_final && a < n_a; ++a) {
+    const int r = b * K + a_par[a];
+    if (a_tok[a] >= 0 || st.row_t[r] != T - 1) continue;
+    double s = a_score[a];
+    for (int j = 0; j < n_new; ++j)
+      if (pick[j] == a && !later[j]) s = n_score[j];
+    const double key = st.score_norm ? s / static_cast<double>(cur.u[r] + 1) : s;
+    if (!st.has_final[b] || key > st.final_key[b]) {
+      st.has_final[b] = 1; st.final_key[b] = key; st.final_score[b] = s; st.final_node[b] = cur.node[r]; st.final_u[b] = cur.u[r];
+    }
+  }
   int w = 0;
   for (int j = 0; j < n_new; ++j) {
     if (dropped[j]) continue;
@@ -381,7 +394,7 @@ cudaError_t alsd_launch_reduce(const AlsdState& st, int B, const float* logits, 
   alsd_reduce_kernel<<<B * st.beam, 256, 0, s>>>(st, logits, ld, V);
   return cudaGetLastError();
 }
-cudaError_t alsd_launch_select(const AlsdState& st, int B, const int32_t* enc_len, int step, float u_max_ratio, bool recombine_returns_input, cudaStream_t s) {
+cudaError_t alsd_launch_select(const AlsdState& st, int B, const int32_t* enc_len, int step, double u_max_ratio, bool recombine_returns_input, cudaStream_t s) {
   alsd_select_kernel<<<B, 32, 0, s>>>(st, enc_len, step, u_max_ratio, recombine_returns_input ? 1 : 0);
   return cudaGetLastError();
 }

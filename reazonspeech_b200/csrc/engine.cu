@@ -752,22 +752,32 @@ int rs_transcribe_batch_confidence(rs_engine* e, const void* wav_host, int wav_i
                           U_max, stats_host, alpha, static_cast<cudaStream_t>(stream));
 }
 
+}  // extern "C"
+
+namespace {
+
 // ALSD beam search over encoder outputs (decode_alsd.cu; semantics: oracle/alsd_restated.py).  Synchronises: the host checks every
-// 32 steps whether every utterance's search has ended.
-int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, float u_max_ratio, int score_norm,
-                 int recombine_returns_input, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev, int U_cap, void* stream) {
-  if (!e || !enc || !enc_len || !y_dev || !step_dev || !n_dev || !score_dev || B <= 0 || T_max <= 0 || U_cap <= 0 || beam < 1 || beam > 8 || u_max_ratio < 0.f)
-    return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_alsd: bad arguments (beam must be 1..8)");
+// 32 steps whether every utterance's search has ended.  tr set: the trace seam (rs_rnnt_alsd_trace), which copies the state of
+// every step out after the beam update; rs_rnnt_alsd passes nullptr, so the two run the same launches.
+int rnnt_alsd(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, double u_max_ratio,
+              int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev, int U_cap,
+              const rs_alsd_trace* tr, cudaStream_t s) {
+  if (!e || !enc || !enc_len || !y_dev || !step_dev || !n_dev || !score_dev || B <= 0 || T_max <= 0 || U_cap <= 0 || beam < 1 || beam > 8 ||
+      !(u_max_ratio >= 0.0))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments (beam must be 1..8)", fn);
+  const int total_steps = T_max + static_cast<int>(u_max_ratio * static_cast<double>(T_max));
+  const int max_nodes = 1 + beam * (total_steps + 1);
+  if (tr && (tr->max_steps < 0 || tr->node_pitch < max_nodes || !tr->n_hyp || !tr->beam_score || !tr->beam_u || !tr->beam_node || !tr->row_t ||
+             !tr->cand_logp || !tr->cand_tok || !tr->has_final || !tr->final_key || !tr->final_score || !tr->node_parent ||
+             !tr->node_tok || !tr->node_step))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad trace buffers (every pointer set, max_steps >= 0, node_pitch >= %d)", fn, max_nodes);
   if (e->alsd.out_w3 == nullptr)
-    return fail(e, RS_ERR_UNSUPPORTED, "rs_rnnt_alsd: the engine was created without the beam-search weight tensors (alsd.*)");
+    return fail(e, RS_ERR_UNSUPPORTED, "%s: the engine was created without the beam-search weight tensors (alsd.*)", fn);
   RS_CUDA(e, cudaSetDevice(e->device));
   Nvtx range("rs::rnnt_alsd");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
   const rs_model_config& c = e->cfg;
   const int Hj = c.joint_hidden, Hp = c.pred_hidden, d = c.d_model, V = c.vocab_size, blank = c.vocab_size, n_pad = e->alsd.n_pad;
   const int M = B * T_max, R = B * beam;
-  const int total_steps = T_max + static_cast<int>(u_max_ratio * static_cast<float>(T_max));
-  const int max_nodes = 1 + beam * (total_steps + 1);
   // ---- workspace: scratch, then the search state, laid out once to size it and once more to bind it
   rs::Arena a;
   const size_t o_xn = a.take(static_cast<size_t>(M) * d * 2), o_encp = a.take(static_cast<size_t>(M) * Hj * 4);
@@ -810,6 +820,20 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
     RS_TRY(gemm(e, {planes, e->alsd.out_w3, e->alsd.out_b, nullptr, logits, R, n_pad, 3 * Hj, RS_EPI_BIAS_F32, 1.f}, s));
     RS_LAUNCH(e, s, 1, rs::alsd_launch_reduce(st, B, logits, n_pad, V, s));
     RS_LAUNCH(e, s, 1, rs::alsd_launch_select(st, B, enc_len, step, u_max_ratio, recombine_returns_input != 0, s));
+    if (tr && step < tr->max_steps) {                   // the new beam is the `nx` half until the predictor pass swaps it in
+      const size_t o = static_cast<size_t>(step) * R, ob = static_cast<size_t>(step) * B;
+      auto copy = [&](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s); };
+      RS_CUDA(e, copy(tr->n_hyp + ob, st.nx.n_hyp, B * 4));
+      RS_CUDA(e, copy(tr->beam_score + o, st.nx.score, R * 8));
+      RS_CUDA(e, copy(tr->beam_u + o, st.nx.u, R * 4));
+      RS_CUDA(e, copy(tr->beam_node + o, st.nx.node, R * 4));
+      RS_CUDA(e, copy(tr->row_t + o, st.row_t, R * 4));
+      RS_CUDA(e, copy(tr->cand_logp + o * 9, st.cand_logp, R * 9 * 4));
+      RS_CUDA(e, copy(tr->cand_tok + o * 8, st.cand_tok, R * 8 * 4));
+      RS_CUDA(e, copy(tr->has_final + ob, st.has_final, B * 4));
+      RS_CUDA(e, copy(tr->final_key + ob, st.final_key, B * 8));
+      RS_CUDA(e, copy(tr->final_score + ob, st.final_score, B * 8));
+    }
     RS_TRY(predictor());
     if ((step & 31) == 31) {
       RS_CUDA(e, cudaMemcpyAsync(e->alsd_done_host, st.n_done, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -818,8 +842,32 @@ int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, 
     }
   }
   RS_LAUNCH(e, s, 1, rs::alsd_launch_output(st, B, blank, y_dev, step_dev, n_dev, score_dev, U_cap, s));
+  if (tr) {
+    const size_t dp = static_cast<size_t>(tr->node_pitch) * 4, sp = static_cast<size_t>(max_nodes) * 4;
+    RS_CUDA(e, cudaMemcpy2DAsync(tr->node_parent, dp, st.node_parent, sp, sp, B, cudaMemcpyDeviceToDevice, s));
+    RS_CUDA(e, cudaMemcpy2DAsync(tr->node_tok, dp, st.node_tok, sp, sp, B, cudaMemcpyDeviceToDevice, s));
+    RS_CUDA(e, cudaMemcpy2DAsync(tr->node_step, dp, st.node_step, sp, sp, B, cudaMemcpyDeviceToDevice, s));
+  }
   RS_CUDA(e, cudaStreamSynchronize(s));
   return RS_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, double u_max_ratio, int score_norm,
+                 int recombine_returns_input, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev, int U_cap, void* stream) {
+  return rnnt_alsd(e, "rs_rnnt_alsd", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, y_dev, step_dev, n_dev,
+                   score_dev, U_cap, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_alsd_trace(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, double u_max_ratio, int score_norm,
+                       int recombine_returns_input, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev, int U_cap,
+                       const rs_alsd_trace* trace, void* stream) {
+  if (trace == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_alsd_trace: bad arguments (no trace)");
+  return rnnt_alsd(e, "rs_rnnt_alsd_trace", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, y_dev, step_dev,
+                   n_dev, score_dev, U_cap, trace, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

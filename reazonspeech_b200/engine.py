@@ -52,8 +52,16 @@ EXPORTS = [
     "rs_enable_kernel_timing", "rs_kernel_timing", "rs_stage_rows",
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
-    "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice",
+    "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
 ]
+
+
+# per-step buffers of rs_alsd_trace: (name, dtype, trailing shape); then the back-pointer tree, [B, node_pitch] each
+ALSD_TRACE_STEP = [("n_hyp", torch.int32, ()), ("beam_score", torch.float64, ("beam",)), ("beam_u", torch.int32, ("beam",)),
+                   ("beam_node", torch.int32, ("beam",)), ("row_t", torch.int32, ("beam",)), ("cand_logp", torch.float32, ("beam", 9)),
+                   ("cand_tok", torch.int32, ("beam", 8)), ("has_final", torch.int32, ()), ("final_key", torch.float64, ()),
+                   ("final_score", torch.float64, ())]
+ALSD_TRACE_FIELDS = [n for n, _, _ in ALSD_TRACE_STEP] + ["node_parent", "node_tok", "node_step"]
 
 
 class RsNgramLM(C.Structure):
@@ -61,6 +69,11 @@ class RsNgramLM(C.Structure):
     _fields_ = [("order", C.c_int), ("n_states", C.c_int), ("n_arcs", C.c_int), ("pitch", C.c_int), ("start_state", C.c_int),
                 ("cb", C.c_void_p), ("chain", C.c_void_p), ("arc_begin", C.c_void_p), ("arc_tok", C.c_void_p),
                 ("arc_to", C.c_void_p), ("arc_w", C.c_void_p), ("uni_w", C.c_void_p), ("uni_to", C.c_void_p)]
+
+
+class RsAlsdTrace(C.Structure):
+    """include/rs_engine.h rs_alsd_trace"""
+    _fields_ = [("max_steps", C.c_int32), ("node_pitch", C.c_int32)] + [(n, C.c_void_p) for n in ALSD_TRACE_FIELDS]
 
 
 def load_library(build_if_missing: bool = True) -> C.CDLL:
@@ -101,8 +114,10 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_set_phrase_boosting.argtypes = [vp, vp, vp, ip, ip]
     lib.rs_set_ngram_lm.argtypes = [vp, C.POINTER(RsNgramLM)]
     lib.rs_ngram_lm_eval.argtypes = [vp, vp, vp, ip, vp, vp, vp]
-    lib.rs_rnnt_alsd.argtypes = [vp, vp, vp, ip, ip, ip, C.c_float, ip, ip, vp, vp, vp, vp, ip, vp]
+    lib.rs_rnnt_alsd.argtypes = [vp, vp, vp, ip, ip, ip, C.c_double, ip, ip, vp, vp, vp, vp, ip, vp]
     lib.rs_rnnt_alsd.restype = ip
+    lib.rs_rnnt_alsd_trace.argtypes = [vp, vp, vp, ip, ip, ip, C.c_double, ip, ip, vp, vp, vp, vp, ip, C.POINTER(RsAlsdTrace), vp]
+    lib.rs_rnnt_alsd_trace.restype = ip
     lib.rs_rnnt_align.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp]
     lib.rs_rnnt_align.restype = ip
     lib.rs_rnnt_align_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp]
@@ -489,6 +504,38 @@ class Engine:
                                           int(recombine_returns_input), y.data_ptr(), steps.data_ptr(), n.data_ptr(), score.data_ptr(), U,
                                           self._stream()), "rs_rnnt_alsd")
         return y, steps, n, score
+
+    def alsd_trace(self, enc: torch.Tensor, enc_len: torch.Tensor, beam: int = 4, u_max_ratio: float = 2.0, score_norm: bool = True,
+                   recombine_returns_input: bool = True, U_cap: Optional[int] = None, max_steps: Optional[int] = None):
+        """``alsd`` through the trace seam (rs_rnnt_alsd_trace) -> dict of CPU tensors: y, steps, n, score as ``alsd`` returns
+        them; per recorded step i: n_hyp [S, B], beam_score / beam_u / beam_node / row_t [S, B, beam], cand_logp [S, B, beam, 9], cand_tok
+        [S, B, beam, 8], has_final / final_key / final_score [S, B]; the back-pointer tree node_parent / node_tok / node_step
+        [B, node_pitch].  S = the steps the search ran (at most ``max_steps``, default all it may run)."""
+        B, T, _ = enc.shape
+        assert enc.dtype == torch.float32 and enc.is_contiguous() and enc_len.dtype == torch.int32
+        total_steps = T + int(u_max_ratio * T)
+        S = total_steps + 1 if max_steps is None else int(max_steps)
+        U = U_cap or (total_steps + 1)
+        node_pitch = 1 + beam * (total_steps + 1)
+        dims = {"beam": beam}
+        buf = {n: torch.full((max(S, 1), B) + tuple(dims.get(d, d) for d in shape), -1, dtype=dt, device=self.device)
+               for n, dt, shape in ALSD_TRACE_STEP}
+        for n in ("node_parent", "node_tok", "node_step"):
+            buf[n] = torch.full((B, node_pitch), -1, dtype=torch.int32, device=self.device)
+        tr = RsAlsdTrace(S, node_pitch, *[buf[n].data_ptr() for n in ALSD_TRACE_FIELDS])
+        y = torch.zeros(B, U + 1, dtype=torch.int32, device=self.device)
+        steps = torch.zeros(B, U, dtype=torch.int32, device=self.device)
+        n = torch.zeros(B, dtype=torch.int32, device=self.device)
+        score = torch.zeros(B, dtype=torch.float64, device=self.device)
+        self._check(self.lib.rs_rnnt_alsd_trace(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, int(beam), float(u_max_ratio), int(score_norm),
+                                                int(recombine_returns_input), y.data_ptr(), steps.data_ptr(), n.data_ptr(), score.data_ptr(), U,
+                                                C.byref(tr), self._stream()), "rs_rnnt_alsd_trace")
+        out = {k: v.cpu() for k, v in buf.items()}
+        ran = int((out["n_hyp"][:, 0] >= 0).sum())               # steps never run keep the -1 fill
+        for k, _, _ in ALSD_TRACE_STEP:
+            out[k] = out[k][:ran]
+        out.update(y=y.cpu(), steps=steps.cpu(), n=n.cpu(), score=score.cpu())
+        return out
 
     def _align_inputs(self, enc, enc_len, labels, label_len):
         B, T, _ = enc.shape
