@@ -161,6 +161,30 @@ int rs_transcribe_batch_confidence(rs_engine* e, const void* wav_host, int wav_i
                                    int B, int L_max, int32_t* tokens_host, int32_t* frames_host,
                                    int32_t* n_tok_host, int U_max, float alpha, float* stats_host, void* stream);
 
+/* Streaming: the greedy decode resumed from, and returning, a per-stream decoder state (semantics, frame grid and chunk
+ * schedule: reazonspeech_b200/streaming.py).  A stream's state is one record of rs_stream_state_bytes() bytes in caller-owned
+ * device memory (about 15 KB at the production size; records 16-byte aligned).  The record is opaque apart from its three
+ * leading int32 words: started, boost_state, lm_state.  An all-zero record is a stream that has not started: its first call
+ * runs the start (SOS) step, exactly as rs_rnnt_greedy does.  A boost_state / lm_state outside the current table counts as
+ * the root / the LM's start_state: writing -1 there makes a stream start over in a table set while it was open.
+ *
+ * rs_rnnt_greedy_resume: enc f32[B,T_max,d_model] (device); row b decodes its frames [dec_begin[b], dec_end[b]) from record
+ * slot[b] of `states` (device arrays i32[B]) and stores its state there.  Slots must be distinct (not checked: they are on
+ * the device).  tokens / frames / n_tok / stats as rs_rnnt_greedy_confidence, for this call's emissions only; frames are
+ * frames of `enc`.  stats may be NULL (alpha is then ignored).  Asynchronous on stream.
+ * rs_stream_step: the whole path with HOST buffers, shaped like rs_transcribe_batch_confidence: H2D, log-mel, encoder,
+ * joint.enc, the resumed decode, D2H; synchronises.  Row b is a buffer of len_host[b] samples; dec_begin / dec_end / slot are
+ * host arrays.  Checks on the host that the slots are distinct and >= 0 and that 0 <= dec_begin <= dec_end <=
+ * rs_enc_valid(len) (and len <= L_max), RS_ERR_INVALID_ARG before any launch otherwise.  stats_host may be NULL.
+ * Phrase boosting and the n-gram LM apply to both as to every greedy entry point. */
+size_t rs_stream_state_bytes(const rs_engine* e);
+int rs_rnnt_greedy_resume(rs_engine* e, const float* enc_dev, const int32_t* dec_begin_dev, const int32_t* dec_end_dev,
+                          const int32_t* slot_dev, void* states_dev, int B, int T_max, int32_t* tokens_dev, int32_t* frames_dev,
+                          int32_t* n_tok_dev, int U_max, float alpha, float* stats_dev, void* stream);
+int rs_stream_step(rs_engine* e, const void* wav_host, int wav_is_pcm16, const int32_t* len_host, const int32_t* dec_begin_host,
+                   const int32_t* dec_end_host, const int32_t* slot_host, void* states_dev, int B, int L_max, int32_t* tokens_host,
+                   int32_t* frames_host, int32_t* n_tok_host, int U_max, float alpha, float* stats_host, void* stream);
+
 /* Phrase boosting (context biasing) of the greedy decode.  bonus f32 and next i32, both [n_states, pitch] in device memory
  * and 16-byte aligned, are the tables of a phrase automaton (reazonspeech_b200/boosting.py builds them): emitting non-blank
  * token k from state n adds bonus[n][k] to token k's logit before the argmax and moves the utterance to next[n][k] (a value

@@ -56,10 +56,21 @@
 // ([3][B][kFrames][S], like conf); after the consume step the ring slot of the emitted token's slice holds the new state, which
 // phase L reads.  Pass 0's tile is filled between the arrival at and the release from the grid barrier that ends phase L,
 // i.e. under the barrier's latency.  With kConf the emitted token's unfused logit is its fused value - the added term.
+//
+// Resume (streaming; semantics: reazonspeech_b200/streaming.py), rnnt_greedy_resume_kernel: the same body with the load at the
+// start and the store at the end compiled in (kResume), its own 16 instances: as a runtime branch the same code moved the
+// register allocation of the offline instances.  With p.states set, row b
+// decodes frames [dec_begin[b], enc_len[b]) from record slot[b]: int32 started, boost_state, lm_state, reserved, then f32 c[HP],
+// rec[HP][4], pp[HJ].  h itself is not needed: the next LSTM step reads only rec = W_hh . h, c and the token's gate_tab row, and
+// pp feeds the joint.  sym is not needed either: a row leaves the loop only at t == enc_len, reached by a blank or a max_symbols
+// advance, both of which reset it.  An unstarted record (all zero) runs the SOS step exactly as a fresh decode does.
 #include "common.cuh"
 #include "kernels.h"
 
 namespace rs {
+
+constexpr int kStateHead = 16;                   // bytes of a stream record's header (three documented int32 words + one reserved)
+size_t stream_state_bytes(int Hj, int Hp) { return (kStateHead + (static_cast<size_t>(Hp) * 5 + Hj) * 4 + 15) & ~static_cast<size_t>(15); }
 
 constexpr int kSpThreads = 256;
 constexpr int kSpWarps = kSpThreads / 32;
@@ -89,6 +100,9 @@ struct SpecDev {
   int2* lm_ring;              // [3][B][kFrames][S] (next LM state, added term bits) of each slice's best token (kLM)
   int B, T_max, V, U_max, max_symbols;
   int S, rows_j, units, rows_p;
+  // resume (rnnt_greedy_resume_kernel): row b decodes frames [dec_begin[b], enc_len[b]) from record slot[b] of `states` and
+  // writes its state back there
+  const int32_t* dec_begin; const int32_t* slot; uint8_t* states; int state_bytes;
 };
 
 // Softmax statistics of a set of logits relative to its maximum m (an empty set: m = -inf, all sums zero):
@@ -249,9 +263,8 @@ __device__ __forceinline__ void lm_fill_row(const NgramLM& lm, int s, int j0, in
 // is one m64n64k16 per warpgroup and the two halves of D are added in the epilogue.
 static_assert(kSpThreads == 256, "the joint is issued by two warpgroups");
 
-template <int HJ, int HP, bool kConf, bool kBoost, bool kLM>
-__global__ void __launch_bounds__(kSpThreads, 1)
-rnnt_greedy_spec_kernel(const SpecDev p) {
+template <int HJ, int HP, bool kConf, bool kBoost, bool kLM, bool kResume>
+__device__ __forceinline__ void greedy_spec_body(const SpecDev& p) {
   constexpr int KH = HJ / 2;                 // joint k-half staged in shared memory at a time
   constexpr int LS = HP + 8;                 // W_hh row stride in halves
   constexpr int KSW = (HP / 16) / kSpWarps;  // k16 steps per warp of phase P
@@ -350,6 +363,35 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
       s_t[b] = 0; s_sym[b] = 0; s_n[b] = 0; s_tok[b] = blank; s_len[b] = p.enc_len[b];
       if constexpr (kBoost) s_state[b] = 0;
       if constexpr (kLM) { s_lm[b] = p.lm.start_state; s_lslot[b] = -1; }
+    }
+    if constexpr (kResume) {
+      // resume: a started row continues from its record (no SOS step: s_tok = -1), an unstarted one starts as above.  Each CTA
+      // loads what it owns -- the cell state and rec of its units, the pred_proj rows of joint.pred it computes -- and every
+      // CTA the automaton and LM states.  Out-of-range states count as the root / start_state.
+      for (int b = tid; b < B; b += kSpThreads) {
+        const int32_t* hd = reinterpret_cast<const int32_t*>(p.states + static_cast<size_t>(p.slot[b]) * p.state_bytes);
+        if (p.dec_begin != nullptr) s_t[b] = p.dec_begin[b];
+        if (hd[0] != 0) {
+          s_tok[b] = -1;
+          if constexpr (kBoost) s_state[b] = static_cast<unsigned int>(hd[1]) < static_cast<unsigned int>(p.boost_states) ? hd[1] : 0;
+          if constexpr (kLM) s_lm[b] = static_cast<unsigned int>(hd[2]) < static_cast<unsigned int>(p.lm.n_states) ? hd[2] : p.lm.start_state;
+        }
+      }
+      for (int i = tid; i < B * p.units; i += kSpThreads) {
+        const int b = i / p.units, u = i % p.units;
+        const uint8_t* r = p.states + static_cast<size_t>(p.slot[b]) * p.state_bytes;
+        if (u < nu && reinterpret_cast<const int32_t*>(r)[0] != 0) {
+          s_c[i] = reinterpret_cast<const float*>(r + kStateHead)[u0 + u];
+          __stcg(reinterpret_cast<float4*>(p.rec + (static_cast<size_t>(b) * HP + u0 + u) * 4),
+                 reinterpret_cast<const float4*>(r + kStateHead + HP * 4)[u0 + u]);
+        }
+      }
+      for (int i = tid; i < B * np; i += kSpThreads) {
+        const int b = i / np, r = i % np;
+        const uint8_t* rc = p.states + static_cast<size_t>(p.slot[b]) * p.state_bytes;
+        if (reinterpret_cast<const int32_t*>(rc)[0] != 0)
+          __stcg(p.ppbuf + static_cast<size_t>(b) * HJ + p0 + r, reinterpret_cast<const float*>(rc + kStateHead + HP * 20)[p0 + r]);
+      }
     }
     if (tid < 12) s_prof[tid] = 0;
   }
@@ -605,9 +647,18 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
     }
   };
 
-  compact();                                      // SOS: every utterance steps once on the blank (zero) embedding
+  compact();                                      // SOS: every unstarted utterance steps once on the blank (zero) embedding
   if (has_j) fetch_enc(0);
-  lstm_and_pred();
+  if constexpr (kResume) {
+    if (s_cnt[0] > 0) {
+      lstm_and_pred();
+    } else {                                      // every row resumes (same decision in every CTA): one barrier publishes the loaded ppbuf
+      if constexpr (kLM) sp_grid_barrier_with(p.counter, target, G, [&] { if (has_j) lm_fill(0); });
+      else sp_grid_barrier(p.counter, target, G);
+    }
+  } else {
+    lstm_and_pred();
+  }
 
   for (;;) {
     // ---- phase J
@@ -848,7 +899,41 @@ rnnt_greedy_spec_kernel(const SpecDev p) {
   }
   if (cta == 0) for (int b = tid; b < B; b += kSpThreads) p.n_tok[b] = s_n[b];
   if (cta == 0 && tid == 0) for (int i = 0; i < 12; ++i) p.prof[i] = s_prof[i];
+  if constexpr (kResume) {
+    // store back what this CTA owns.  The last lstm_and_pred ran for the last emissions, so the record holds the state after
+    // the last token's step; rec / ppbuf of the CTA's units / rows were written by this CTA (before the barrier that ended it).
+    for (int i = tid; i < B * p.units; i += kSpThreads) {
+      const int b = i / p.units, u = i % p.units;
+      uint8_t* r = p.states + static_cast<size_t>(p.slot[b]) * p.state_bytes;
+      if (u < nu) {
+        reinterpret_cast<float*>(r + kStateHead)[u0 + u] = s_c[i];
+        reinterpret_cast<float4*>(r + kStateHead + HP * 4)[u0 + u] = __ldcg(reinterpret_cast<const float4*>(p.rec + (static_cast<size_t>(b) * HP + u0 + u) * 4));
+      }
+    }
+    for (int i = tid; i < B * np; i += kSpThreads) {
+      const int b = i / np, r = i % np;
+      uint8_t* rc = p.states + static_cast<size_t>(p.slot[b]) * p.state_bytes;
+      reinterpret_cast<float*>(rc + kStateHead + HP * 20)[p0 + r] = __ldcg(p.ppbuf + static_cast<size_t>(b) * HJ + p0 + r);
+    }
+    if (cta == 0) {                               // every CTA read the headers before the first grid barrier
+      for (int b = tid; b < B; b += kSpThreads) {
+        int32_t* hd = reinterpret_cast<int32_t*>(p.states + static_cast<size_t>(p.slot[b]) * p.state_bytes);
+        hd[0] = 1;
+        if constexpr (kBoost) hd[1] = s_state[b];
+        if constexpr (kLM) hd[2] = s_lm[b];
+      }
+    }
+  }
 }
+
+template <int HJ, int HP, bool kConf, bool kBoost, bool kLM>
+__global__ void __launch_bounds__(kSpThreads, 1)
+rnnt_greedy_spec_kernel(const SpecDev p) { greedy_spec_body<HJ, HP, kConf, kBoost, kLM, false>(p); }
+
+// the resumed decode: its own instances, so that the offline ones compile from unchanged code (same registers, same results)
+template <int HJ, int HP, bool kConf, bool kBoost, bool kLM>
+__global__ void __launch_bounds__(kSpThreads, 1)
+rnnt_greedy_resume_kernel(const SpecDev p) { greedy_spec_body<HJ, HP, kConf, kBoost, kLM, true>(p); }
 
 // workspace (SpecDev's global buffers): hbuf | rec | ppbuf | barrier counters (kBarCounters 128-byte lines) | prof | best | conf |
 // lm_ring.  Everything before conf is zeroed by the launch; every conf / lm_ring slot that is read was written first.
@@ -869,7 +954,7 @@ SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms) {
 
 template <int HJ, int HP, bool kConf, bool kBoost, bool kLM>
 static cudaError_t launch_sp(SpecDev p, int grid, size_t smem, cudaStream_t stream) {
-  const auto kernel = rnnt_greedy_spec_kernel<HJ, HP, kConf, kBoost, kLM>;
+  const auto kernel = p.states != nullptr ? rnnt_greedy_resume_kernel<HJ, HP, kConf, kBoost, kLM> : rnnt_greedy_spec_kernel<HJ, HP, kConf, kBoost, kLM>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   int per_sm = 0;
@@ -933,6 +1018,9 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   const bool lm = a.lm.order != 0;
   if (lm && !lm_tables_ok(a.lm, a.V)) return cudaErrorInvalidValue;
   p.lm_ring = reinterpret_cast<int2*>(ws + w.lm_ring);
+  p.dec_begin = a.dec_begin; p.slot = a.slot; p.states = static_cast<uint8_t*>(a.states);
+  p.state_bytes = static_cast<int>(stream_state_bytes(a.Hj, a.Hp));
+  if (a.states != nullptr && (a.slot == nullptr || (reinterpret_cast<uintptr_t>(a.states) & 15u))) return cudaErrorInvalidValue;
   p.B = a.B; p.T_max = a.T_max; p.V = a.V; p.U_max = a.U_max; p.max_symbols = a.max_symbols;
   p.S = G / kGroups;
   p.rows_j = (a.V + 1 + p.S - 1) / p.S;

@@ -9,6 +9,7 @@
 #include <cstdlib>
 #include <cstdio>
 #include <cstring>
+#include <algorithm>
 #include <map>
 #include <string>
 #include <utility>
@@ -76,6 +77,9 @@ struct rs_engine {
   // forced alignment (align.cu): scratch grown on demand like the ALSD workspace
   void* align_ws = nullptr;
   size_t align_ws_bytes = 0;
+  // rs_stream_step: device copies of the step's dec_begin | dec_end | slot, grown on demand
+  void* stream_args = nullptr;
+  size_t stream_args_bytes = 0;
   unsigned int* lm_tickets = nullptr;   // per-utterance CTA tickets of the log-mel statistics (engine-owned, kept zero between launches)
   static constexpr int kMaxBatch = 1 << 16;
   struct { const float *c0w, *c0b, *d1w, *d1b, *p1b, *d2w, *d2b, *p2b, *ob; const void *p1w, *p2w, *ow; } sub;
@@ -409,18 +413,24 @@ int do_encode(rs_engine* e, const Plan& p, const int32_t* mel_len, float* enc, i
   return RS_OK;
 }
 
-// stats == nullptr: tokens only; otherwise stats f32 [B, U_max, 4] receives (lp, H1, A_alpha, G_alpha) of every stored token
+// The resumed decode of streaming (rs_rnnt_greedy_resume, rs_stream_step): device arrays; the decode runs frames
+// [dec_begin[b], dec_end[b]) of row b from record slot[b] of states
+struct Resume { const int32_t* dec_begin; const int32_t* dec_end; const int32_t* slot; void* states; };
+
+// stats == nullptr: tokens only; otherwise stats f32 [B, U_max, 4] receives (lp, H1, A_alpha, G_alpha) of every stored token.
+// rs != nullptr: the resumed decode (enc_len stays the encoder's valid length; the decode ends at rs->dec_end)
 int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_len, int T_max, int32_t* tokens,
-              int32_t* frames, int32_t* ntok, int U_max, float* stats, float alpha, cudaStream_t s) {
+              int32_t* frames, int32_t* ntok, int U_max, float* stats, float alpha, cudaStream_t s, const Resume* rs = nullptr) {
   Nvtx range("rs::rnnt_greedy (joint.enc projection + persistent decode)");
   const rs_model_config& c = e->cfg;
   const int M = p.B * T_max;
   RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, at<void>(e, p.xn), static_cast<int64_t>(M) * c.d_model, s));
   RS_TRY(gemm(e, {at<void>(e, p.xn), e->dec.enc_w, e->dec.enc_b, nullptr, at<void>(e, p.encp), M, c.joint_hidden, c.d_model, RS_EPI_BIAS_F32, 1.f}, s));
   mark(e, 4, s);
-  rs::DecodeArgs da{at<float>(e, p.encp), enc_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w, e->dec.gate_tab, e->dec.pred_w,
+  rs::DecodeArgs da{at<float>(e, p.encp), rs ? rs->dec_end : enc_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w, e->dec.gate_tab, e->dec.pred_w,
                     e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, c.max_symbols,
                     stats, alpha, e->boost.bonus, e->boost.next, e->boost.n_states, e->boost.pitch, e->lm};
+  if (rs) { da.dec_begin = rs->dec_begin; da.slot = rs->slot; da.states = rs->states; }
   // One decode kernel for every batch size (windowed, weights-stationary, joint on wgmma: decode_spec.cu): an utterance's
   // logits are accumulated in the same order whether it is decoded alone or inside a batch, so results do not depend on
   // batch composition.
@@ -483,6 +493,7 @@ void rs_engine_destroy(rs_engine* e) {
   cudaFree(e->lm_tickets);
   cudaFree(e->alsd_ws);
   cudaFree(e->align_ws);
+  cudaFree(e->stream_args);
   if (e->alsd_done_host) cudaFreeHost(e->alsd_done_host);
   delete e;
 }
@@ -589,7 +600,7 @@ namespace {
 bool alpha_ok(float alpha) { return alpha > 0.f && std::isfinite(alpha); }
 
 int rnnt_greedy(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, int32_t* tokens,
-                int32_t* frames, int32_t* n_tok, int U_max, float* stats, float alpha, cudaStream_t s) {
+                int32_t* frames, int32_t* n_tok, int U_max, float* stats, float alpha, cudaStream_t s, const Resume* rs = nullptr) {
   if (!e || !enc || !enc_len || !tokens || !frames || !n_tok || B <= 0 || T_max <= 0 || U_max <= 0)
     return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
   RS_CUDA(e, cudaSetDevice(e->device));
@@ -602,7 +613,7 @@ int rnnt_greedy(rs_engine* e, const char* fn, const float* enc, const int32_t* e
   p.dec_ws = a.take(dec_ws(e, B).total);
   p.total = a.off;
   RS_TRY(check_ws(e, p));
-  return do_greedy(e, p, enc, enc_len, T_max, tokens, frames, n_tok, U_max, stats, alpha, s);
+  return do_greedy(e, p, enc, enc_len, T_max, tokens, frames, n_tok, U_max, stats, alpha, s, rs);
 }
 
 }  // namespace
@@ -619,6 +630,21 @@ int rs_rnnt_greedy_confidence(rs_engine* e, const float* enc, const int32_t* enc
   if (!stats || !alpha_ok(alpha)) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_greedy_confidence: bad arguments (stats must be set, alpha > 0 and finite)");
   return rnnt_greedy(e, "rs_rnnt_greedy_confidence", enc, enc_len, B, T_max, tokens, frames, n_tok, U_max, stats, alpha,
                      static_cast<cudaStream_t>(stream));
+}
+
+size_t rs_stream_state_bytes(const rs_engine* e) {
+  return e ? rs::stream_state_bytes(e->cfg.joint_hidden, e->cfg.pred_hidden) : 0;
+}
+
+int rs_rnnt_greedy_resume(rs_engine* e, const float* enc, const int32_t* dec_begin, const int32_t* dec_end, const int32_t* slot,
+                          void* states, int B, int T_max, int32_t* tokens, int32_t* frames, int32_t* n_tok, int U_max, float alpha,
+                          float* stats, void* stream) {
+  if (!dec_begin || !dec_end || !slot || !states || (stats && !alpha_ok(alpha)))
+    return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_greedy_resume: bad arguments (dec_begin, dec_end, slot and states must be set; with stats, alpha > 0 and finite)");
+  if (reinterpret_cast<uintptr_t>(states) & 15u) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_greedy_resume: states must be 16-byte aligned");
+  const Resume rs{dec_begin, dec_end, slot, states};
+  return rnnt_greedy(e, "rs_rnnt_greedy_resume", enc, dec_end, B, T_max, tokens, frames, n_tok, U_max, stats, alpha,
+                     static_cast<cudaStream_t>(stream), &rs);
 }
 
 }  // extern "C"
@@ -638,7 +664,8 @@ int check_transcribe_args(rs_engine* e, const char* fn, const void* wav, const i
 // landed[c] (when not null) is recorded once chunk c's samples have been copied in.  `wav` holds f32 samples, or int16 PCM
 // (scaled by 2^-15 inside the log-mel kernel) when i16.
 int run_pipeline(rs_engine* e, const Plan& p, const void* wav, bool i16, const int32_t* len, int n_chunks, const cudaEvent_t* landed,
-                 int32_t* tokens, int32_t* frames, int32_t* n_tok, int U_max, float* conf_stats, float alpha, cudaStream_t s) {
+                 int32_t* tokens, int32_t* frames, int32_t* n_tok, int U_max, float* conf_stats, float alpha, cudaStream_t s,
+                 const Resume* rs = nullptr) {
   const int B = p.B, per = (B + n_chunks - 1) / n_chunks;
   const size_t row_bytes = static_cast<size_t>(p.L_max) * (i16 ? 2 : 4);
   float* mel = at<float>(e, p.mel);
@@ -655,7 +682,7 @@ int run_pipeline(rs_engine* e, const Plan& p, const void* wav, bool i16, const i
   }
   RS_TRY(do_encode(e, p, mel_len, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), -1, s));
   mark(e, 3, s);
-  RS_TRY(do_greedy(e, p, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), p.T3, tokens, frames, n_tok, U_max, conf_stats, alpha, s));
+  RS_TRY(do_greedy(e, p, at<float>(e, p.enc), at<int32_t>(e, p.enc_len), p.T3, tokens, frames, n_tok, U_max, conf_stats, alpha, s, rs));
   mark(e, 5, s);
   return RS_OK;
 }
@@ -671,12 +698,29 @@ int transcribe_device(rs_engine* e, const char* fn, const void* wav, bool i16, c
 // Host buffers in, host buffers out (the model.transcribe seam): H2D in utterance chunks on the copy stream, overlapped with
 // the frontend of the chunks that have landed; D2H of the tokens (and of the statistics when stats_host is set); synchronises
 // before returning.
+// rs (host arrays dec_begin / dec_end / slot, device states): the resumed decode of rs_stream_step; the three arrays are copied
+// into an engine-owned device buffer first.
 int transcribe_batch(rs_engine* e, const char* fn, const void* wav_host, bool i16, const int32_t* len_host, int B, int L_max,
                      int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, float* stats_host, float alpha,
-                     cudaStream_t s) {
+                     cudaStream_t s, const Resume* rs_host = nullptr) {
   RS_TRY(check_transcribe_args(e, fn, wav_host, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max));
   Plan p = make_plan(e, B, L_max, U_max);
   RS_TRY(check_ws(e, p));
+  Resume rs_dev{};
+  if (rs_host) {
+    const size_t need_bytes = static_cast<size_t>(3) * B * 4;
+    if (need_bytes > e->stream_args_bytes) {
+      RS_CUDA(e, cudaStreamSynchronize(s));
+      cudaFree(e->stream_args); e->stream_args = nullptr; e->stream_args_bytes = 0;
+      RS_CUDA(e, cudaMalloc(&e->stream_args, need_bytes));
+      e->stream_args_bytes = need_bytes;
+    }
+    int32_t* d = static_cast<int32_t*>(e->stream_args);
+    RS_CUDA(e, cudaMemcpyAsync(d, rs_host->dec_begin, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, s));
+    RS_CUDA(e, cudaMemcpyAsync(d + B, rs_host->dec_end, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, s));
+    RS_CUDA(e, cudaMemcpyAsync(d + 2 * B, rs_host->slot, static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, s));
+    rs_dev = {d, d + B, d + 2 * B, rs_host->states};
+  }
   const size_t row_bytes = static_cast<size_t>(L_max) * (i16 ? 2 : 4);   // the waveform region of the workspace is sized for f32
   char* wav = at<char>(e, p.wav);
   const char* wav_h = static_cast<const char*>(wav_host);
@@ -700,7 +744,8 @@ int transcribe_batch(rs_engine* e, const char* fn, const void* wav_host, bool i1
     }
   }
   RS_TRY(run_pipeline(e, p, wav, i16, len, n_chunks, n_chunks > 1 ? e->copy_ev : nullptr, at<int32_t>(e, p.tokens),
-                      at<int32_t>(e, p.frames), at<int32_t>(e, p.ntok), U_max, stats_host ? at<float>(e, p.stats) : nullptr, alpha, s));
+                      at<int32_t>(e, p.frames), at<int32_t>(e, p.ntok), U_max, stats_host ? at<float>(e, p.stats) : nullptr, alpha, s,
+                      rs_host ? &rs_dev : nullptr));
   RS_CUDA(e, cudaMemcpyAsync(tokens_host, at<int32_t>(e, p.tokens), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(frames_host, at<int32_t>(e, p.frames), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(n_tok_host, at<int32_t>(e, p.ntok), static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
@@ -750,6 +795,28 @@ int rs_transcribe_batch_confidence(rs_engine* e, const void* wav_host, int wav_i
   if (!stats_host || !alpha_ok(alpha)) return fail(e, RS_ERR_INVALID_ARG, "rs_transcribe_batch_confidence: bad arguments (stats must be set, alpha > 0 and finite)");
   return transcribe_batch(e, "rs_transcribe_batch_confidence", wav_host, wav_is_pcm16 != 0, len_host, B, L_max, tokens_host, frames_host, n_tok_host,
                           U_max, stats_host, alpha, static_cast<cudaStream_t>(stream));
+}
+
+int rs_stream_step(rs_engine* e, const void* wav_host, int wav_is_pcm16, const int32_t* len_host, const int32_t* dec_begin_host,
+                   const int32_t* dec_end_host, const int32_t* slot_host, void* states, int B, int L_max, int32_t* tokens_host,
+                   int32_t* frames_host, int32_t* n_tok_host, int U_max, float alpha, float* stats_host, void* stream) {
+  const char* fn = "rs_stream_step";
+  if (!e || !dec_begin_host || !dec_end_host || !slot_host || !states || !len_host || B <= 0 || (stats_host && !alpha_ok(alpha)))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments (dec_begin, dec_end, slot, len and states must be set; with stats, alpha > 0 and finite)", fn);
+  if (reinterpret_cast<uintptr_t>(states) & 15u) return fail(e, RS_ERR_INVALID_ARG, "%s: states must be 16-byte aligned", fn);
+  std::vector<int32_t> seen(slot_host, slot_host + B);
+  std::sort(seen.begin(), seen.end());
+  if (seen[0] < 0 || std::adjacent_find(seen.begin(), seen.end()) != seen.end())
+    return fail(e, RS_ERR_INVALID_ARG, "%s: slots must be distinct and >= 0", fn);
+  for (int b = 0; b < B; ++b) {
+    const int n = len_host[b] < 0 || len_host[b] > L_max ? -1 : rs_enc_valid(e, len_host[b]);
+    if (n < 0 || dec_begin_host[b] < 0 || dec_begin_host[b] > dec_end_host[b] || dec_end_host[b] > n)
+      return fail(e, RS_ERR_INVALID_ARG, "%s: row %d: need 0 <= dec_begin (%d) <= dec_end (%d) <= rs_enc_valid(len = %d) = %d and len <= L_max",
+                  fn, b, dec_begin_host[b], dec_end_host[b], len_host[b], n);
+  }
+  const Resume rs{dec_begin_host, dec_end_host, slot_host, states};
+  return transcribe_batch(e, fn, wav_host, wav_is_pcm16 != 0, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max,
+                          stats_host, alpha, static_cast<cudaStream_t>(stream), &rs);
 }
 
 }  // extern "C"

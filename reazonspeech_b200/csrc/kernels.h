@@ -102,7 +102,15 @@ struct DecodeArgs {
   const int32_t* boost_next = nullptr;
   int boost_states = 0, boost_pitch = 0;
   NgramLM lm;                 // n-gram LM shallow fusion; lm.order == 0: none
+  // resume (streaming): states != nullptr makes row b decode frames [dec_begin[b] (nullptr: 0), enc_len[b]) from the record
+  // slot[b] of states (stream_state_bytes each, 16-byte aligned, distinct slots) and store its state there; nullptr: every row
+  // starts fresh at frame 0
+  const int32_t* dec_begin = nullptr;
+  const int32_t* slot = nullptr;
+  void* states = nullptr;
 };
+// Bytes of one stream record of the resumed decode (decode_spec.cu describes the layout)
+size_t stream_state_bytes(int Hj, int Hp);
 // Byte offsets of the decode workspace's regions and its size (decode_spec.cu describes the regions)
 struct SpecWorkspace { size_t hbuf, rec, ppbuf, counters, prof, best, conf, lm_ring, total; };
 SpecWorkspace rnnt_spec_workspace(int B, int Hj, int Hp, int num_sms);

@@ -53,6 +53,7 @@ EXPORTS = [
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
+    "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step",
 ]
 
 
@@ -122,6 +123,12 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_align.restype = ip
     lib.rs_rnnt_align_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp]
     lib.rs_rnnt_align_lattice.restype = ip
+    lib.rs_stream_state_bytes.argtypes = [vp]
+    lib.rs_stream_state_bytes.restype = C.c_size_t
+    lib.rs_rnnt_greedy_resume.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
+    lib.rs_rnnt_greedy_resume.restype = ip
+    lib.rs_stream_step.argtypes = [vp, vp, ip, vp, vp, vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
+    lib.rs_stream_step.restype = ip
     lib.rs_resample_mono.argtypes = [vp, vp, ip, vp, ip, ip, ip, vp, ip, ip, ip, ip, ip, vp, ip, vp, vp]
     lib.rs_resample_mono.restype = ip
     lib.rs_gemm_bf16.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, ip, ip, C.c_float, vp, ip, ip, vp]
@@ -443,6 +450,50 @@ class Engine:
         self._check(self.lib.rs_rnnt_greedy_confidence(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, tokens.data_ptr(), frames.data_ptr(),
                                                        ntok.data_ptr(), U, float(alpha), stats.data_ptr(), self._stream()), "rs_rnnt_greedy_confidence")
         return tokens, frames, ntok, stats
+
+    @property
+    def stream_state_bytes(self) -> int:
+        """Bytes of one stream's decoder-state record (rs_stream_state_bytes; streaming.py)."""
+        return int(self.lib.rs_stream_state_bytes(self.h))
+
+    def greedy_resume(self, enc: torch.Tensor, dec_begin: torch.Tensor, dec_end: torch.Tensor, slot: torch.Tensor, states: torch.Tensor,
+                      U_max: Optional[int] = None, alpha: Optional[float] = None):
+        """The resumed greedy decode (rs_rnnt_greedy_resume): row b decodes frames [dec_begin[b], dec_end[b]) of ``enc`` from record
+        ``states[slot[b]]`` (device uint8 [n_records, stream_state_bytes]) and stores its state there -> (tokens, frames, n_tok),
+        plus stats [B, U, 4] with ``alpha``.  Slots must be distinct."""
+        B, T, _ = enc.shape
+        assert enc.dtype == torch.float32 and enc.is_contiguous()
+        assert states.dtype == torch.uint8 and states.is_contiguous() and states.shape[-1] == self.stream_state_bytes
+        args = [a.to(self.device, torch.int32).contiguous() for a in (dec_begin, dec_end, slot)]
+        self.ensure_workspace(B, (T * 8 + 8) * self.cfg.n_window_stride)
+        U = U_max or T * self.cfg.max_symbols
+        tokens = torch.zeros(B, U, dtype=torch.int32, device=self.device)
+        frames = torch.zeros(B, U, dtype=torch.int32, device=self.device)
+        ntok = torch.zeros(B, dtype=torch.int32, device=self.device)
+        stats = torch.zeros(B, U, 4, dtype=torch.float32, device=self.device) if alpha is not None else None
+        self._check(self.lib.rs_rnnt_greedy_resume(self.h, enc.data_ptr(), args[0].data_ptr(), args[1].data_ptr(), args[2].data_ptr(),
+                                                   states.data_ptr(), B, T, tokens.data_ptr(), frames.data_ptr(), ntok.data_ptr(), U,
+                                                   float(alpha or 0.0), None if stats is None else stats.data_ptr(), self._stream()),
+                    "rs_rnnt_greedy_resume")
+        return (tokens, frames, ntok) if stats is None else (tokens, frames, ntok, stats)
+
+    def stream_step(self, wav: torch.Tensor, lens: torch.Tensor, dec_begin: torch.Tensor, dec_end: torch.Tensor, slot: torch.Tensor,
+                    states: torch.Tensor, U_max: int, out, alpha: Optional[float] = None):
+        """One streaming step over host buffers (rs_stream_step): ``wav`` host float32 or int16 [B, L] (the rows' buffers), ``lens``,
+        ``dec_begin``, ``dec_end``, ``slot`` host int32 [B], ``states`` the device records -> ``out`` (host tokens [B, U],
+        frames [B, U], n_tok [B], and stats [B, U, 4] with ``alpha``) filled; synchronises."""
+        B, L = wav.shape
+        assert wav.device.type == "cpu" and wav.dtype in (torch.float32, torch.int16) and wav.is_contiguous()
+        assert states.dtype == torch.uint8 and states.is_contiguous() and states.shape[-1] == self.stream_state_bytes
+        host = [a.to(torch.int32).contiguous() for a in (lens, dec_begin, dec_end, slot)]
+        assert all(a.device.type == "cpu" for a in host)
+        self.ensure_workspace(B, L)
+        tokens, frames, ntok = out[:3]
+        self._check(self.lib.rs_stream_step(self.h, wav.data_ptr(), int(wav.dtype == torch.int16), host[0].data_ptr(), host[1].data_ptr(),
+                                            host[2].data_ptr(), host[3].data_ptr(), states.data_ptr(), B, L, tokens.data_ptr(),
+                                            frames.data_ptr(), ntok.data_ptr(), U_max, float(alpha or 0.0),
+                                            out[3].data_ptr() if alpha is not None else None, self._stream()), "rs_stream_step")
+        return out
 
     def transcribe_device(self, wav: torch.Tensor, lens: torch.Tensor, U_max: Optional[int] = None, out=None, alpha: Optional[float] = None):
         """With ``alpha``: also the confidence statistics (``greedy``), ``out`` then holds four tensors."""

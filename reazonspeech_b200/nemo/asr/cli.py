@@ -26,6 +26,12 @@ Fourth extension, forced alignment of known transcripts (reazonspeech_b200/align
 aligned to its given transcript and the segments are written through the same writer with the same time offsets
   --text=FILE          UTF-8 text, one transcript line per AUDIO argument, in order (a count mismatch is an error)
 Without the option the output is unchanged.
+Fifth extension, streaming (reazonspeech_b200/streaming.py): the one AUDIO argument is decoded chunk by chunk as a live stream
+  --stream             AUDIO is a file, or - for raw 16-bit little-endian 16 kHz mono PCM on stdin; every chunk's final
+                       text goes to stderr as "[start seconds] text" as soon as it is decoded, and at the end the usual
+                       output (--to, -o) is written from the whole stream
+  --chunk=S --left=S --right=S   chunk and context seconds (multiples of 0.08; default 1.6, 1.2, 1.2)
+Without the option the output is unchanged.
 Audio decoding: soundfile when installed, scipy for WAV, librosa for compressed containers, see audio.audio_from_path.
 """
 import dataclasses
@@ -36,7 +42,7 @@ from dataclasses import dataclass, field
 from typing import List, Optional
 
 SHORT_OPTS = "ho:"
-LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=")
+LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=", "stream", "chunk=", "left=", "right=")
 
 
 @dataclass
@@ -50,6 +56,10 @@ class Options:
     lm: Optional[str] = None
     lm_alpha: Optional[float] = None
     text: Optional[str] = None
+    stream: bool = False
+    chunk: float = 1.6
+    left: float = 1.2
+    right: float = 1.2
 
 
 def parse(argv) -> Options:
@@ -73,9 +83,15 @@ def parse(argv) -> Options:
             opt.lm_alpha = float(value)
         if flag == "--text":
             opt.text = value
+        if flag == "--stream":
+            opt.stream = True
+        if flag in ("--chunk", "--left", "--right"):
+            setattr(opt, flag[2:], float(value))
     if (opt.lm is None) != (opt.lm_alpha is None):
         raise ValueError("--lm and --lm-alpha go together: the LM weight has no default (try values around 0.3-0.5 and tune "
                          "on held-out audio)" if opt.lm is not None else "--lm-alpha needs an LM: --lm=FILE")
+    if opt.stream and len(opt.audio) > 1:
+        raise ValueError("--stream decodes one AUDIO argument (a file, or - for PCM on stdin)")
     return opt
 
 
@@ -100,7 +116,7 @@ def run(opt: Options) -> None:
     texts = load_transcripts(opt.text, len(opt.audio)) if opt.text is not None else None
     sink = sys.stdout if opt.output is None else open(opt.output, "w")
     warnings.simplefilter("ignore")
-    clips = [audio_from_path(path) for path in opt.audio]
+    clips = [audio_from_path(path) for path in opt.audio] if not (opt.stream and opt.audio == ["-"]) else []
     boosting = None
     if opt.phrases is not None or opt.phrase_score is not None:
         from ...boosting import PhraseBoostingConfig, load_phrases
@@ -114,7 +130,9 @@ def run(opt: Options) -> None:
         from ...ngram_lm import NgramLMConfig
         extra["lm"] = NgramLMConfig(opt.lm, opt.lm_alpha)
     model = load_model(**extra)
-    if texts is not None:
+    if opt.stream:
+        results = [stream(model, opt, clips[0] if clips else None)]
+    elif texts is not None:
         results = align_batch(model, clips, texts)
     else:
         results = transcribe_batch(model, clips) if len(clips) > 1 else [transcribe(model, clips[0])]
@@ -122,11 +140,47 @@ def run(opt: Options) -> None:
         out = get_writer(sink, opt.fmt)
         out.write_header()
         offset = 0.0
-        for clip, result in zip(clips, results):
+        for k, result in enumerate(results):
             for segment in result.segments:
                 out.write(segment if offset == 0.0 else
                           dataclasses.replace(segment, start_seconds=segment.start_seconds + offset, end_seconds=segment.end_seconds + offset))
-            offset += clip.seconds
+            offset += clips[k].seconds if k < len(clips) else 0.0
+
+
+def stream(model, opt: Options, clip=None):
+    """--stream: ``clip`` (a decoded file), or 16-bit PCM from stdin when None, fed to a StreamingTranscriber in 0.16 s pieces;
+    each step's final text goes to stderr with its start time -> the stream's TranscribeResult."""
+    import numpy as np
+    from .audio import norm_audio
+    from .streaming import StreamingTranscriber
+    from ...streaming import StreamingConfig
+    st = StreamingTranscriber(model, StreamingConfig(opt.chunk, opt.left, opt.right), max_streams=1)
+    sid = st.open()
+    piece = 2560
+
+    def show(new):
+        for subs in new.values():
+            if subs:
+                print(f"[{subs[0].seconds:.2f}] {''.join(s.token for s in subs)}", file=sys.stderr, flush=True)
+
+    if clip is not None:
+        wave = np.asarray(norm_audio(clip).waveform)
+        wave = wave if wave.dtype == np.int16 else wave.astype(np.float32)
+        for lo in range(0, len(wave), piece):
+            st.feed(sid, wave[lo:lo + piece])
+            show(st.step())
+    else:
+        raw = sys.stdin.buffer
+        while True:
+            data = raw.read(2 * piece)
+            if not data:
+                break
+            st.feed(sid, np.frombuffer(data[: len(data) // 2 * 2], dtype="<i2").astype(np.int16))
+            show(st.step())
+    st.close(sid)
+    while not st.done(sid):
+        show(st.step())
+    return st.result(sid)
 
 
 def main(argv=None):

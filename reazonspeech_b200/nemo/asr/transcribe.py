@@ -161,6 +161,14 @@ class B200RnntModel:
         """Upload tables already built from ``lm`` (the multi-GPU model builds them once for all replicas)."""
         self.engine.set_ngram_lm(tables)
         self.lm = lm
+        self._notify_tables(2)
+
+    def _notify_tables(self, word: int) -> None:
+        """Open streams (``StreamingTranscriber``) restart their boosting (word 1) or LM (word 2) state from the root."""
+        for ref in list(self.__dict__.get("_table_listeners", ())):
+            fn = ref()
+            if fn is not None:
+                fn(word)
 
     def set_phrase_boosting(self, boosting: Optional[PhraseBoostingConfig]) -> None:
         """Boost the phrases of ``boosting`` in every following greedy decode (boosting.py), or stop with None.  Call it
@@ -171,6 +179,7 @@ class B200RnntModel:
         """Upload tables already built from ``boosting`` (the multi-GPU model builds them once for all replicas)."""
         self.engine.set_phrase_boosting(None if tables is None else tables.bonus, None if tables is None else tables.next)
         self.boosting = boosting
+        self._notify_tables(1)
 
     # -- token-level batched path
     def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
