@@ -188,14 +188,28 @@ int rs_stream_step(rs_engine* e, const void* wav_host, int wav_is_pcm16, const i
 /* Phrase boosting (context biasing) of the greedy decode.  bonus f32 and next i32, both [n_states, pitch] in device memory
  * and 16-byte aligned, are the tables of a phrase automaton (reazonspeech_b200/boosting.py builds them): emitting non-blank
  * token k from state n adds bonus[n][k] to token k's logit before the argmax and moves the utterance to next[n][k] (a value
- * outside [0, n_states) counts as the root, state 0).  Every utterance starts at the root in every call; blank is never
- * boosted.  pitch >= vocab_size and a multiple of 4; 1 <= n_states <= RS_MAX_BOOST_STATES; otherwise RS_ERR_INVALID_ARG and
+ * outside [0, n_states) counts as the root: state 0, or the row's root with rs_set_boost_roots).  Every utterance starts at
+ * the root in every call; blank is never boosted.  pitch >= vocab_size and a multiple of 4; 1 <= n_states <= RS_MAX_BOOST_STATES; otherwise RS_ERR_INVALID_ARG and
  * the previous setting stays.  n_states = 0 clears the setting (the pointers are then ignored).  While a table is set, every
  * greedy entry point (rs_rnnt_greedy, rs_transcribe_device / _batch and their _pcm16 / _confidence forms) decodes with it; the
  * confidence statistics stay those of the unboosted softmax at the boosted decisions.  The tables stay owned by the caller
  * and must outlive every call that uses them; the engine keeps only the pointers.  rs_rnnt_alsd ignores them. */
 #define RS_MAX_BOOST_STATES 8192
 int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* next_dev, int n_states, int pitch);
+
+/* Phrase boosting per row: each row of a greedy batch decodes against its own phrase list.  The table set by
+ * rs_set_phrase_boosting then holds several automata laid one after another, each with its next entries offset to its own
+ * region (reazonspeech_b200/boosting.py combine_tables builds it); a row's root is the first state of its region.
+ * roots_host is a HOST array of n entries; each must lie in [0, n_states) of the current table, and a table must be set,
+ * otherwise RS_ERR_INVALID_ARG and the previous roots stay.  The engine keeps a copy and stages it into an engine-owned
+ * device buffer on each decode's stream, ordered like the workspace (the call waits for the device only when that buffer
+ * has to grow).  From then on row b of every greedy
+ * entry point (rs_rnnt_greedy, rs_transcribe_device / _batch in their _pcm16 / _confidence forms, rs_rnnt_greedy_resume and
+ * rs_stream_step) starts at roots[b] instead of state 0, and a state outside [0, n_states) -- a transition or a stream
+ * record's boost_state -- counts as roots[b].  A call with more rows than roots (B > n) returns RS_ERR_INVALID_ARG before any
+ * launch.  n = 0 clears the roots (every row starts at 0 again); setting or clearing a table with rs_set_phrase_boosting also
+ * clears them. */
+int rs_set_boost_roots(rs_engine* e, const int32_t* roots_host, int n);
 
 /* n-gram language-model shallow fusion of the greedy decode (reazonspeech_b200/ngram_lm.py builds the tables from an ARPA file
  * over BPE token ids and states the semantics).  The decision of every (utterance, frame) is the argmax of

@@ -21,7 +21,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
-from typing import List, Sequence, Union
+from typing import Hashable, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -124,6 +124,52 @@ def build_tables(cfg: PhraseBoostingConfig, vocab_size: int, tokenizer=None) -> 
     bonus = np.zeros((S, pitch), np.float32)
     bonus[:, :vocab_size] = (g[nxt[:, :vocab_size]] - f[:, None]).astype(np.float32) * np.float32(cfg.score)
     return PhraseBoostingTables(bonus, nxt, f, g)
+
+
+def config_key(cfg: Optional[PhraseBoostingConfig]) -> Hashable:
+    """A hashable identity of a phrase list: configs with equal phrases (in order) and score build equal tables."""
+    if cfg is None:
+        return None
+    return (tuple(p if isinstance(p, str) else tuple(int(i) for i in p) for p in cfg.phrases), float(cfg.score))
+
+
+def combine_tables(lists: Sequence[Optional[PhraseBoostingConfig]], vocab_size: int, tokenizer=None,
+                   base: Optional[PhraseBoostingConfig] = None) -> Tuple[PhraseBoostingTables, List[int]]:
+    """Several phrase lists in one table, for decoding each row of a batch against its own list (rs_set_boost_roots) ->
+    (tables, one root per entry of ``lists``).
+
+    Region 0 holds ``base`` (the model's global list; with none, the 1-state empty automaton, whose bonus is zero).  Each
+    distinct list follows in its own region: ``build_tables(list)`` with ``next`` offset by the region's start in the columns
+    below vocab_size.  A row starting at its region's root never leaves that region, so it decodes exactly as it would with
+    its list set alone.  Identical lists (``config_key``) share a region; a ``None`` entry means the global list, root 0.
+
+    Memory: 8 * pitch bytes per state on the device (bonus f32 + next i32), about 24 KB at vocab_size 3000; the whole table
+    may hold at most MAX_STATES states and raises ValueError beyond (there is no silent splitting)."""
+    distinct = {config_key(c): c for c in lists if c is not None}
+    regions = [build_tables(base if base is not None else PhraseBoostingConfig(), vocab_size, tokenizer)]
+    regions += [build_tables(c, vocab_size, tokenizer) for c in distinct.values()]
+    tables, starts = stack_tables(regions, vocab_size, len(distinct))
+    start = dict(zip(distinct, starts[1:]))
+    return tables, [0 if c is None else start[config_key(c)] for c in lists]
+
+
+def stack_tables(regions: Sequence[PhraseBoostingTables], vocab_size: int, n_lists: Optional[int] = None
+                 ) -> Tuple[PhraseBoostingTables, List[int]]:
+    """Tables already built by ``build_tables`` laid one after another, ``next`` of each offset by its start in the columns
+    below vocab_size (the inputs are not modified) -> (tables, start of every region).  Raises ValueError beyond MAX_STATES
+    (``n_lists``: the number of distinct lists named in the message, default all regions but the first)."""
+    sizes = [t.n_states for t in regions]
+    if sum(sizes) > MAX_STATES:
+        n = len(regions) - 1 if n_lists is None else n_lists
+        raise ValueError(f"the {n} distinct phrase lists need {sum(sizes)} automaton states together with the "
+                         f"global list's region, more than {MAX_STATES}; pass fewer or shorter lists per call")
+    starts = np.cumsum([0] + sizes[:-1]).tolist()
+    nxt = np.concatenate([t.next for t in regions])
+    for at, size in zip(starts[1:], sizes[1:]):
+        nxt[at:at + size, :vocab_size] += at
+    tables = PhraseBoostingTables(np.concatenate([t.bonus for t in regions]), nxt, np.concatenate([t.f for t in regions]),
+                                  np.concatenate([t.g for t in regions]))
+    return tables, starts
 
 
 def _pitch(vocab_size: int) -> int:

@@ -38,7 +38,10 @@
 //
 // Phrase boosting (kBoost = true; tables built by reazonspeech_b200/boosting.py).  Every utterance carries a state of the
 // phrase automaton, s_state[b], advanced identically by every CTA in the consume step: s_state = next[s_state][token] on
-// every emission (a value outside [0, n_states) becomes the root).  The decision for a (utterance, frame) is the argmax of
+// every emission (a value outside [0, n_states) becomes the row's root).  Row b starts at its root boost_root[b] (0 without
+// roots): with several automata laid one after another in one table, each with next offset to its own region, each row
+// decodes against its own phrase list.  The root is re-read from global memory where it is needed (the start, and the
+// out-of-range case), which keeps it out of the register budget.  The decision for a (utterance, frame) is the argmax of
 // logit_k + bonus[s_state][k], blank never boosted.  The four frames of a window share the utterance's state, so a pass needs
 // the bonus rows of its <= 8 utterances over the CTA's vocabulary slice: cp.async'd into a shared tile when the pass's
 // rows are fetched (pass 0: under phases L and P) and added to the logits in the argmax epilogue.  With kConf as well, the
@@ -103,7 +106,13 @@ struct SpecDev {
   // resume (rnnt_greedy_resume_kernel): row b decodes frames [dec_begin[b], enc_len[b]) from record slot[b] of `states` and
   // writes its state back there
   const int32_t* dec_begin; const int32_t* slot; uint8_t* states; int state_bytes;
+  // kBoost: root state of each row ([B]; nullptr: state 0 for every row).  Last, so that the other fields keep their offsets
+  // and the instances without kBoost their code.
+  const int32_t* boost_root;
 };
+
+// Row b's root of the phrase automaton: where it starts, and where a state outside the table sends it (kBoost)
+__device__ __forceinline__ int boost_root_of(const SpecDev& p, int b) { return p.boost_root != nullptr ? __ldg(p.boost_root + b) : 0; }
 
 // Softmax statistics of a set of logits relative to its maximum m (an empty set: m = -inf, all sums zero):
 // s = sum e^(l-m), g = sum e^(l-m) (l-m), a = sum e^(alpha (l-m)), ga = sum e^(alpha (l-m)) (l-m).
@@ -361,19 +370,19 @@ __device__ __forceinline__ void greedy_spec_body(const SpecDev& p) {
     for (int i = tid; i < B * p.units; i += kSpThreads) s_c[i] = 0.f;
     for (int b = tid; b < B; b += kSpThreads) {
       s_t[b] = 0; s_sym[b] = 0; s_n[b] = 0; s_tok[b] = blank; s_len[b] = p.enc_len[b];
-      if constexpr (kBoost) s_state[b] = 0;
+      if constexpr (kBoost) s_state[b] = boost_root_of(p, b);
       if constexpr (kLM) { s_lm[b] = p.lm.start_state; s_lslot[b] = -1; }
     }
     if constexpr (kResume) {
       // resume: a started row continues from its record (no SOS step: s_tok = -1), an unstarted one starts as above.  Each CTA
       // loads what it owns -- the cell state and rec of its units, the pred_proj rows of joint.pred it computes -- and every
-      // CTA the automaton and LM states.  Out-of-range states count as the root / start_state.
+      // CTA the automaton and LM states.  Out-of-range states count as the row's root / start_state.
       for (int b = tid; b < B; b += kSpThreads) {
         const int32_t* hd = reinterpret_cast<const int32_t*>(p.states + static_cast<size_t>(p.slot[b]) * p.state_bytes);
         if (p.dec_begin != nullptr) s_t[b] = p.dec_begin[b];
         if (hd[0] != 0) {
           s_tok[b] = -1;
-          if constexpr (kBoost) s_state[b] = static_cast<unsigned int>(hd[1]) < static_cast<unsigned int>(p.boost_states) ? hd[1] : 0;
+          if constexpr (kBoost) s_state[b] = static_cast<unsigned int>(hd[1]) < static_cast<unsigned int>(p.boost_states) ? hd[1] : boost_root_of(p, b);
           if constexpr (kLM) s_lm[b] = static_cast<unsigned int>(hd[2]) < static_cast<unsigned int>(p.lm.n_states) ? hd[2] : p.lm.start_state;
         }
       }
@@ -844,7 +853,7 @@ __device__ __forceinline__ void greedy_spec_body(const SpecDev& p) {
             const size_t at = static_cast<size_t>(s_state[b]) * p.boost_pitch + k;
             const int nx = __ldg(p.boost_next + at);
             if constexpr (kConf && !kLM) if (n < p.U_max) s_le[b] = best_value(v) - __ldg(p.boost_bonus + at);
-            s_state[b] = static_cast<unsigned int>(nx) < static_cast<unsigned int>(p.boost_states) ? nx : 0;
+            s_state[b] = static_cast<unsigned int>(nx) < static_cast<unsigned int>(p.boost_states) ? nx : boost_root_of(p, b);
           }
           if constexpr (kLM) {                                // the ring slot of k's slice; read in phase L (the new state)
             lslot = static_cast<int>(((static_cast<size_t>(iter % 3) * B + b) * kFrames + j) * p.S + k / p.rows_j);
@@ -1010,6 +1019,7 @@ cudaError_t launch_rnnt_greedy_spec(const DecodeArgs& a, void* workspace, int nu
   if (a.stats != nullptr && !(a.alpha > 0.f && a.alpha < INFINITY)) return cudaErrorInvalidValue;
   p.alpha = a.alpha; p.alpha_l2 = a.alpha * kLog2e;
   p.boost_bonus = a.boost_bonus; p.boost_next = a.boost_next; p.boost_states = a.boost_states; p.boost_pitch = a.boost_pitch;
+  p.boost_root = a.boost_root;
   const bool boost = a.boost_bonus != nullptr;
   if (boost && (a.boost_next == nullptr || a.boost_states < 1 || a.boost_pitch < a.V || (a.boost_pitch & 3) ||
                 ((reinterpret_cast<uintptr_t>(a.boost_bonus) | reinterpret_cast<uintptr_t>(a.boost_next)) & 15u)))

@@ -87,6 +87,11 @@ struct rs_engine {
   struct { const void *enc_w, *out_w, *lstm_w, *pred_w; const float *enc_b, *out_b, *embed, *lstm_b, *pred_b, *gate_tab; } dec;
   // phrase boosting (rs_set_phrase_boosting): caller-owned device tables used by every greedy decode while set
   struct { const float* bonus = nullptr; const int32_t* next = nullptr; int n_states = 0, pitch = 0; } boost;
+  // per-row roots of that table (rs_set_boost_roots): n_roots host entries, copied on the call's stream into an engine-owned
+  // device buffer (grown on demand) before each decode; 0: none
+  std::vector<int32_t> roots_host;
+  int32_t* boost_roots = nullptr;
+  int n_roots = 0, roots_cap = 0;
   // n-gram LM shallow fusion (rs_set_ngram_lm): caller-owned device tables used by every greedy decode while set; order 0: none
   rs::NgramLM lm;
   void* ws = nullptr;
@@ -431,6 +436,10 @@ int do_greedy(rs_engine* e, const Plan& p, const float* enc, const int32_t* enc_
                     e->dec.pred_b, tokens, frames, ntok, p.B, T_max, c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, c.max_symbols,
                     stats, alpha, e->boost.bonus, e->boost.next, e->boost.n_states, e->boost.pitch, e->lm};
   if (rs) { da.dec_begin = rs->dec_begin; da.slot = rs->slot; da.states = rs->states; }
+  if (e->n_roots > 0) {             // ordered on s like the workspace: the previous decode has read the previous roots
+    RS_CUDA(e, cudaMemcpyAsync(e->boost_roots, e->roots_host.data(), static_cast<size_t>(p.B) * 4, cudaMemcpyHostToDevice, s));
+    da.boost_root = e->boost_roots;
+  }
   // One decode kernel for every batch size (windowed, weights-stationary, joint on wgmma: decode_spec.cu): an utterance's
   // logits are accumulated in the same order whether it is decoded alone or inside a batch, so results do not depend on
   // batch composition.
@@ -494,6 +503,7 @@ void rs_engine_destroy(rs_engine* e) {
   cudaFree(e->alsd_ws);
   cudaFree(e->align_ws);
   cudaFree(e->stream_args);
+  cudaFree(e->boost_roots);
   if (e->alsd_done_host) cudaFreeHost(e->alsd_done_host);
   delete e;
 }
@@ -504,6 +514,7 @@ int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* 
   if (e == nullptr) return RS_ERR_INVALID_ARG;
   if (n_states == 0) {
     e->boost = {};
+    e->n_roots = 0;
     return RS_OK;
   }
   if (n_states < 1 || n_states > RS_MAX_BOOST_STATES)
@@ -513,6 +524,30 @@ int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* 
   if (bonus_dev == nullptr || next_dev == nullptr || ((reinterpret_cast<uintptr_t>(bonus_dev) | reinterpret_cast<uintptr_t>(next_dev)) & 15u))
     return fail(e, RS_ERR_INVALID_ARG, "rs_set_phrase_boosting: bonus and next must be non-null and 16-byte aligned");
   e->boost.bonus = bonus_dev; e->boost.next = next_dev; e->boost.n_states = n_states; e->boost.pitch = pitch;
+  e->n_roots = 0;                         // roots index the table they were set for
+  return RS_OK;
+}
+
+int rs_set_boost_roots(rs_engine* e, const int32_t* roots_host, int n) {
+  if (e == nullptr) return RS_ERR_INVALID_ARG;
+  if (n == 0) {
+    e->n_roots = 0;
+    return RS_OK;
+  }
+  if (n < 0 || roots_host == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_set_boost_roots: n=%d must be >= 0 and roots non-null", n);
+  if (e->boost.bonus == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_set_boost_roots: no phrase-boosting table is set (rs_set_phrase_boosting)");
+  for (int b = 0; b < n; ++b)
+    if (roots_host[b] < 0 || roots_host[b] >= e->boost.n_states)
+      return fail(e, RS_ERR_INVALID_ARG, "rs_set_boost_roots: roots[%d] = %d outside [0, %d)", b, roots_host[b], e->boost.n_states);
+  if (n > e->roots_cap) {                 // growing: a decode still queued may read the old buffer
+    RS_CUDA(e, cudaSetDevice(e->device));
+    RS_CUDA(e, cudaDeviceSynchronize());
+    cudaFree(e->boost_roots); e->boost_roots = nullptr; e->roots_cap = 0; e->n_roots = 0;
+    RS_CUDA(e, cudaMalloc(&e->boost_roots, static_cast<size_t>(n) * 4));
+    e->roots_cap = n;
+  }
+  e->roots_host.assign(roots_host, roots_host + n);
+  e->n_roots = n;
   return RS_OK;
 }
 
@@ -599,10 +634,18 @@ namespace {
 
 bool alpha_ok(float alpha) { return alpha > 0.f && std::isfinite(alpha); }
 
+// Per-row boosting roots, when set, must cover every row of the batch
+int check_roots(rs_engine* e, const char* fn, int B) {
+  if (e->n_roots > 0 && B > e->n_roots)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: B=%d rows but only %d boosting roots are set (rs_set_boost_roots)", fn, B, e->n_roots);
+  return RS_OK;
+}
+
 int rnnt_greedy(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, int32_t* tokens,
                 int32_t* frames, int32_t* n_tok, int U_max, float* stats, float alpha, cudaStream_t s, const Resume* rs = nullptr) {
   if (!e || !enc || !enc_len || !tokens || !frames || !n_tok || B <= 0 || T_max <= 0 || U_max <= 0)
     return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  RS_TRY(check_roots(e, fn, B));
   RS_CUDA(e, cudaSetDevice(e->device));
   Plan p{};
   // only xn / encp / dec_ws are touched: size them for M = B*T_max rows
@@ -655,6 +698,7 @@ int check_transcribe_args(rs_engine* e, const char* fn, const void* wav, const i
                           const int32_t* frames, const int32_t* n_tok, int U_max) {
   if (!e || !wav || !len || !tokens || !frames || !n_tok || B <= 0 || L_max <= 0 || U_max <= 0)
     return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  RS_TRY(check_roots(e, fn, B));
   RS_CUDA(e, cudaSetDevice(e->device));
   return RS_OK;
 }

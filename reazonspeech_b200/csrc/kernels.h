@@ -108,6 +108,8 @@ struct DecodeArgs {
   const int32_t* dec_begin = nullptr;
   const int32_t* slot = nullptr;
   void* states = nullptr;
+  // phrase boosting per row: [B] row b's root state, in [0, boost_states) (checked by the caller); nullptr: the root is 0
+  const int32_t* boost_root = nullptr;
 };
 // Bytes of one stream record of the resumed decode (decode_spec.cu describes the layout)
 size_t stream_state_bytes(int Hj, int Hp);

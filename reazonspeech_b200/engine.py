@@ -53,7 +53,7 @@ EXPORTS = [
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
-    "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step",
+    "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots",
 ]
 
 
@@ -113,6 +113,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_transcribe_device_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
     lib.rs_transcribe_batch_confidence.argtypes = [vp, vp, ip, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
     lib.rs_set_phrase_boosting.argtypes = [vp, vp, vp, ip, ip]
+    lib.rs_set_boost_roots.argtypes = [vp, vp, ip]
     lib.rs_set_ngram_lm.argtypes = [vp, C.POINTER(RsNgramLM)]
     lib.rs_ngram_lm_eval.argtypes = [vp, vp, vp, ip, vp, vp, vp]
     lib.rs_rnnt_alsd.argtypes = [vp, vp, vp, ip, ip, ip, C.c_double, ip, ip, vp, vp, vp, vp, ip, vp]
@@ -154,7 +155,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     for fn in ("rs_workspace_bytes", "rs_set_workspace", "rs_mel_frames", "rs_enc_frames", "rs_mel_valid", "rs_enc_valid", "rs_logmel", "rs_encode",
                "rs_rnnt_greedy", "rs_transcribe_device", "rs_transcribe_batch", "rs_transcribe_device_pcm16", "rs_transcribe_batch_pcm16",
                "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
-               "rs_set_phrase_boosting", "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_gemm_bf16", "rs_layernorm", "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
+               "rs_set_phrase_boosting", "rs_set_boost_roots", "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_gemm_bf16", "rs_layernorm", "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw",
                "rs_enable_stage_timing", "rs_stage_times_ms", "rs_enable_gemm_timing", "rs_gemm_timing"):
         getattr(lib, fn).restype = ip
     _lib = lib
@@ -369,6 +370,13 @@ class Engine:
             self._check(self.lib.rs_set_phrase_boosting(self.h, new[0].data_ptr(), new[1].data_ptr(), new[0].shape[0], new[0].shape[1]),
                         "rs_set_phrase_boosting")
         self._boost = new
+
+    def set_boost_roots(self, roots) -> None:
+        """Per-row roots of the phrase-boosting table (rs_set_boost_roots): row b of every following greedy call starts at
+        ``roots[b]`` (a table from ``boosting.combine_tables``), or ``None`` / empty to clear.  A host-side setting: the roots are
+        copied to the device on each decode's stream."""
+        r = np.ascontiguousarray(np.asarray([] if roots is None else roots, dtype=np.int32).reshape(-1))
+        self._check(self.lib.rs_set_boost_roots(self.h, r.ctypes.data if r.size else None, int(r.size)), "rs_set_boost_roots")
 
     def set_ngram_lm(self, tables) -> None:
         """n-gram LM shallow fusion of every greedy decode (rs_set_ngram_lm): ``tables`` an ``ngram_lm.NgramLMTables``, or

@@ -12,6 +12,7 @@ peer-to-peer traffic: an utterance never leaves its device.  The engine's C call
 """
 from __future__ import annotations
 
+import contextlib
 import queue
 import threading
 from typing import List, Sequence
@@ -59,16 +60,21 @@ class MultiGpuRnntModel:
     def _deal(self, waveforms: Sequence[np.ndarray], batches):
         """Deals the utterances across the replicas by length and yields ``(indices into waveforms, items)`` per finished
         engine batch of any device; ``batches(replica, mine)`` runs on the replica's worker thread and yields the replica's
-        ``(indices into mine, items)``."""
+        ``(indices into mine, items)``.  A caller that stops early (closes the generator) waits for every replica to finish
+        its engine batch in flight: the replicas' engines are idle when this generator has ended."""
         if len(waveforms) == 0:
             return
         shards = [s for s in shard_indices([len(w) for w in waveforms], len(self.replicas))]
         out: "queue.Queue" = queue.Queue()
+        stop = threading.Event()
 
         def work(replica, mine: List[int]):
             try:
-                for idx, items in batches(replica, mine):
-                    out.put(([mine[j] for j in idx], items))
+                with contextlib.closing(batches(replica, mine)) as it:      # closing waits for the batch in flight
+                    for idx, items in it:
+                        out.put(([mine[j] for j in idx], items))
+                        if stop.is_set():
+                            break
             except BaseException as exc:          # surfaced on the caller's thread: a dead device must not look like a slow one
                 out.put(exc)
             finally:
@@ -78,23 +84,45 @@ class MultiGpuRnntModel:
         for t in threads:
             t.start()
         running, error = len(threads), None
-        while running:
-            item = out.get()
-            if item is None:
-                running -= 1
-            elif isinstance(item, BaseException):
-                error = error or item
-            elif error is None:
-                yield item
-        for t in threads:
-            t.join()
+        try:
+            while running:
+                item = out.get()
+                if item is None:
+                    running -= 1
+                elif isinstance(item, BaseException):
+                    error = error or item
+                elif error is None:
+                    yield item
+        finally:
+            stop.set()
+            for t in threads:
+                t.join()
         if error is not None:
             raise error
 
-    def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
+    def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0, *, phrases=None):
         """Yields ``(indices, [(tokens, frames)])`` per finished engine batch of any device, indices into ``waveforms``
-        (``(tokens, frames, stats)`` items with confidence on, as ``B200RnntModel.iter_token_batches``)."""
-        return self._deal(waveforms, lambda replica, mine: replica.iter_token_batches([waveforms[i] for i in mine], pad))
+        (``(tokens, frames, stats)`` items with confidence on, as ``B200RnntModel.iter_token_batches``).  ``phrases``: one
+        list or None per waveform, as there; the combined table is built once and uploaded once per device, and each replica
+        sets the roots of its own batches."""
+        if phrases is None:
+            return self._deal(waveforms, lambda replica, mine: replica.iter_token_batches([waveforms[i] for i in mine], pad))
+        return self._phrase_batches(waveforms, pad, phrases)
+
+    def _phrase_batches(self, waveforms, pad, phrases):
+        from ...boosting import combine_tables
+        from .transcribe import check_phrases, phrases_key
+        phrases = check_phrases(self, phrases, len(waveforms))
+        key, combined = phrases_key(self, phrases), None
+        if any(r._phrase_cache is None or r._phrase_cache[0] != key for r in self.replicas):
+            combined = combine_tables(phrases, self.cfg.vocab_size, self.tokenizer, base=self.boosting)
+        setups = [r.phrase_setup(phrases, combined) for r in self.replicas]
+        roots = setups[0][1]                                  # the same table on every device
+        with contextlib.ExitStack() as stack:
+            for r, (dev, _) in zip(self.replicas, setups):
+                stack.enter_context(r.phrase_tables_set(dev))
+            yield from self._deal(waveforms, lambda replica, mine: replica._token_batches([waveforms[i] for i in mine], pad,
+                                                                                          [roots[i] for i in mine]))
 
     def align_tokens(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
         """``B200RnntModel.align_tokens`` over all devices -> [(frames, token_lp, viterbi, loglik)] in input order."""
@@ -108,10 +136,10 @@ class MultiGpuRnntModel:
                 results[i] = item
         return results
 
-    def transcribe_tokens(self, waveforms: Sequence[np.ndarray], pad: int = 0):
+    def transcribe_tokens(self, waveforms: Sequence[np.ndarray], pad: int = 0, *, phrases=None):
         """-> [(tokens, frames)] in input order."""
         results = [None] * len(waveforms)
-        for idx, items in self.iter_token_batches(waveforms, pad):
+        for idx, items in self.iter_token_batches(waveforms, pad, phrases=phrases):
             for i, item in zip(idx, items):
                 results[i] = item
         return results

@@ -9,6 +9,7 @@ exactly the three points the reference touches it (SURVEY.md section 8b):
 transcribe()/decode_hypothesis() therefore run unmodified on it (see INTEGRATION.md)."""
 from __future__ import annotations
 
+import contextlib
 import glob
 import os
 from dataclasses import dataclass
@@ -19,7 +20,7 @@ import numpy as np
 import torch
 
 from ...alignment import alignment_hypothesis, pack_labels, validate_labels
-from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables
+from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables, combine_tables, config_key
 from ...config import ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
 from ...engine import Engine
@@ -145,7 +146,9 @@ class B200RnntModel:
         self.confidence = confidence.validate() if confidence is not None else None
         pin = torch.cuda.is_available()
         self._staging = (HostStaging(pin), HostStaging(pin))      # double buffer: stage batch k+1 while batch k runs
+        self._phrase_cache = None                                 # (key, device tables, {list key: root}) of the last phrases= call
         self.boosting: Optional[PhraseBoostingConfig] = None
+        self.boosting_tables: Optional[PhraseBoostingTables] = None   # host tables of the global list (streams build on them)
         if boosting is not None:
             self.set_phrase_boosting(boosting)
         self.lm: Optional[NgramLMConfig] = None
@@ -176,20 +179,65 @@ class B200RnntModel:
         self.set_phrase_boosting_tables(boosting_tables(self, boosting), boosting)
 
     def set_phrase_boosting_tables(self, tables: Optional[PhraseBoostingTables], boosting: Optional[PhraseBoostingConfig]) -> None:
-        """Upload tables already built from ``boosting`` (the multi-GPU model builds them once for all replicas)."""
+        """Upload tables already built from ``boosting`` (the multi-GPU model builds them once for all replicas).  Raises
+        ValueError, changing nothing, when open streams with their own lists (``StreamingTranscriber``) could not share one
+        table with the new global list."""
+        for ref in list(self.__dict__.get("_boost_checks", ())):
+            fn = ref()
+            if fn is not None:
+                fn(tables)
         self.engine.set_phrase_boosting(None if tables is None else tables.bonus, None if tables is None else tables.next)
-        self.boosting = boosting
+        self.boosting, self.boosting_tables = boosting, tables
         self._notify_tables(1)
 
+    # -- phrase boosting per utterance (phrases=)
+    def phrase_setup(self, phrases: Sequence[Optional[PhraseBoostingConfig]], combined=None):
+        """The combined table of ``phrases`` (one list or None per input; ``boosting.combine_tables`` with the model's global
+        list in region 0) on this device -> (device tables, one root per input).  The upload is cached, keyed by the lists, so
+        a repeated call does not upload again.  ``combined``: the result of ``combine_tables`` for the same lists, already built
+        (the multi-GPU model builds it once for all replicas)."""
+        key = phrases_key(self, phrases)
+        if self._phrase_cache is None or self._phrase_cache[0] != key:
+            tables, roots = combined if combined is not None else combine_tables(phrases, self.cfg.vocab_size, self.tokenizer, base=self.boosting)
+            dev = tuple(torch.as_tensor(a).to(self.engine.device).contiguous() for a in (tables.bonus, tables.next))
+            self._phrase_cache = (key, dev, {config_key(c): r for c, r in zip(phrases, roots) if c is not None})
+        _, dev, root_of = self._phrase_cache
+        return dev, [0 if c is None else root_of[config_key(c)] for c in phrases]
+
+    @contextlib.contextmanager
+    def phrase_tables_set(self, dev):
+        """Decodes inside use the combined device tables ``dev`` (``phrase_setup``); afterwards the model's global setting is
+        back (its tables' pointers only: nothing is uploaded) and the roots are cleared."""
+        eng = self.engine
+        prev = eng._boost
+        eng.set_phrase_boosting(*dev)
+        try:
+            yield
+        finally:
+            eng.set_phrase_boosting(*(prev if prev is not None else (None,)))
+
     # -- token-level batched path
-    def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0):
+    def iter_token_batches(self, waveforms: Sequence[np.ndarray], pad: int = 0, *, phrases=None):
         """16 kHz mono waveforms (each gets ``pad`` zero samples on both sides) -> yields ``(indices, [(tokens, frames)])``
         batch by batch; with confidence on, ``(tokens, frames, stats)``, stats float32 [n_tokens, 4] (lp, H1, A_alpha, G_alpha).
 
         Utterances are sorted by length and cut into batches of at most ``max_batch`` so padding waste stays small.
         The engine call of batch k runs on a worker thread (ctypes drops the GIL) while this thread stages batch k+1
         into the other staging set and the caller post-processes batch k-1: on a long list the host work hides behind
-        the GPU.  One engine call is in flight at a time (an engine is not re-entrant)."""
+        the GPU.  One engine call is in flight at a time (an engine is not re-entrant).
+
+        ``phrases``: one ``PhraseBoostingConfig`` or None (the model's global list) per waveform; each utterance is decoded
+        against its own list, exactly as it would be alone with that list set by ``set_phrase_boosting``."""
+        if phrases is None:
+            yield from self._token_batches(waveforms, pad, None)
+            return
+        phrases = check_phrases(self, phrases, len(waveforms))
+        dev, roots = self.phrase_setup(phrases)
+        with self.phrase_tables_set(dev):
+            yield from self._token_batches(waveforms, pad, roots)
+
+    def _token_batches(self, waveforms: Sequence[np.ndarray], pad: int, roots: Optional[List[int]]):
+        """``iter_token_batches``; ``roots``: the boosting root of every waveform in the table that is set, or None."""
         from concurrent.futures import ThreadPoolExecutor
         if len(waveforms) == 0:
             return
@@ -198,7 +246,12 @@ class B200RnntModel:
         eng = self.engine
         eng.ensure_workspace(len(batches[0]), (len(waveforms[order[-1]]) + 2 * pad + 3) & ~3)   # once, on this thread (stage() rounds rows up to 4 samples)
         alpha = self.confidence.alpha if self.confidence is not None else None
-        call = eng.transcribe_host if alpha is None else partial(eng.transcribe_host, alpha=alpha)
+        host_call = eng.transcribe_host if alpha is None else partial(eng.transcribe_host, alpha=alpha)
+
+        def call(wav, lens, U, out, idx):
+            if roots is not None:                                     # the batch's roots in its sorted row order, set on the thread that runs it
+                eng.set_boost_roots([roots[i] for i in idx])
+            return host_call(wav, lens, U, out)
 
         def run(staging, idx):
             wav, lens = staging.stage([waveforms[i] for i in idx], pad)
@@ -211,32 +264,42 @@ class B200RnntModel:
 
         if len(batches) == 1:                                         # nothing to overlap: skip the thread hand-off (one-clip calls)
             wav, lens, out = run(self._staging[0], batches[0])
-            yield collect(call(wav, lens, out[0].shape[1], out), batches[0])
+            yield collect(call(wav, lens, out[0].shape[1], out, batches[0]), batches[0])
             return
         with ThreadPoolExecutor(max_workers=1) as pool:
             in_flight = None
             for k, idx in enumerate(batches):
                 wav, lens, out = run(self._staging[k & 1], idx)
-                nxt = (pool.submit(call, wav, lens, out[0].shape[1], out), idx)
+                nxt = (pool.submit(call, wav, lens, out[0].shape[1], out, idx), idx)
                 if in_flight is not None:
                     yield collect(in_flight[0].result(), in_flight[1])
                 in_flight = nxt
             yield collect(in_flight[0].result(), in_flight[1])
 
-    def transcribe_tokens(self, waveforms: Sequence[np.ndarray], pad: int = 0):
-        """-> [(tokens, frames)] in input order."""
+    def transcribe_tokens(self, waveforms: Sequence[np.ndarray], pad: int = 0, *, phrases=None):
+        """-> [(tokens, frames)] in input order (``phrases``: as ``iter_token_batches``)."""
         results = [None] * len(waveforms)
-        for idx, items in self.iter_token_batches(waveforms, pad):
+        for idx, items in self.iter_token_batches(waveforms, pad, phrases=phrases):
             for i, item in zip(idx, items):
                 results[i] = item
         return results
 
-    def iter_token_batches_raw(self, waves: Sequence[np.ndarray], samplerate: int, pad: int = 0):
+    def iter_token_batches_raw(self, waves: Sequence[np.ndarray], samplerate: int, pad: int = 0, *, phrases=None):
         """Like ``iter_token_batches`` for audio that still needs ``norm_audio`` (pkg/nemo-asr/src/audio.py:54-68): waveforms
         at ``samplerate`` (any rate), mono [n] or channels-first [c, n] with the SAME channel count, float or int16 PCM.  They
         are staged as they are (pinned), copied to the GPU and resampled / down-mixed / padded there (rs_resample_mono)
         straight into the buffer the engine transcribes from: the host never touches a sample arithmetically.  (scipy's
-        resample_poly, which this kernel restates, costs the host ~10 ms per 30 s 48 kHz clip -- more than the whole engine.)"""
+        resample_poly, which this kernel restates, costs the host ~10 ms per 30 s 48 kHz clip -- more than the whole engine.)
+        ``phrases``: as ``iter_token_batches``."""
+        if phrases is None:
+            yield from self._token_batches_raw(waves, samplerate, pad, None)
+            return
+        phrases = check_phrases(self, phrases, len(waves))
+        dev, roots = self.phrase_setup(phrases)
+        with self.phrase_tables_set(dev):
+            yield from self._token_batches_raw(waves, samplerate, pad, roots)
+
+    def _token_batches_raw(self, waves: Sequence[np.ndarray], samplerate: int, pad: int, roots: Optional[List[int]]):
         if len(waves) == 0:
             return
         eng = self.engine
@@ -257,6 +320,8 @@ class B200RnntModel:
                 w = waves[i]
                 rows[r, :, : w.shape[1]] = w if (pcm or w.dtype != np.int16) else w.astype(np.float32) * np.float32(1.0 / 32768.0)
             lens = torch.tensor([waves[i].shape[1] for i in idx], dtype=torch.int32)
+            if roots is not None:
+                eng.set_boost_roots([roots[i] for i in idx])
             with torch.cuda.device(eng.device):
                 wav, wl = eng.resample_mono(raw.to(eng.device, non_blocking=True), lens.to(eng.device, non_blocking=True), samplerate, pad)
                 done = [a.cpu() for a in (eng.transcribe_device(wav, wl) if self.confidence is None else
@@ -334,6 +399,24 @@ def boosting_tables(model, boosting: Optional[PhraseBoostingConfig]) -> Optional
     if getattr(model, "decoding", "greedy") != "greedy":
         raise ValueError("phrase boosting is applied by the greedy decode only (not by ALSD beam search)")
     return build_tables(boosting, model.cfg.vocab_size, model.tokenizer)
+
+
+def check_phrases(model, phrases, n: int) -> List[Optional[PhraseBoostingConfig]]:
+    """``phrases=`` of a call with ``n`` inputs, validated: one ``PhraseBoostingConfig`` or None per input, greedy decoding."""
+    if getattr(model, "decoding", "greedy") != "greedy":
+        raise ValueError("phrase boosting is applied by the greedy decode only (not by ALSD beam search)")
+    phrases = list(phrases)
+    if len(phrases) != n:
+        raise ValueError(f"phrases= has {len(phrases)} entries for {n} inputs (one PhraseBoostingConfig or None per input)")
+    for c in phrases:
+        if c is not None and not isinstance(c, PhraseBoostingConfig):
+            raise ValueError(f"phrases= entries must be PhraseBoostingConfig or None, got {type(c).__name__}")
+    return phrases
+
+
+def phrases_key(model, phrases) -> tuple:
+    """The identity of the combined table of ``phrases`` on ``model``: its global list and the distinct lists, in order."""
+    return config_key(model.boosting), tuple(dict.fromkeys(config_key(c) for c in phrases if c is not None))
 
 
 def lm_tables(model, lm: Optional[NgramLMConfig]) -> Optional[NgramLMTables]:
@@ -458,15 +541,23 @@ def transcribe(model, audio: AudioData, config: Optional[TranscribeConfig] = Non
     return result
 
 
-def transcribe_batch(model, audios: Sequence[AudioData], config: Optional[TranscribeConfig] = None) -> List[TranscribeResult]:
+def transcribe_batch(model, audios: Sequence[AudioData], config: Optional[TranscribeConfig] = None, *,
+                     phrases: Optional[Sequence[Optional[PhraseBoostingConfig]]] = None) -> List[TranscribeResult]:
     """Many utterances through one or a few engine launches; results in input order.
 
     Same per-utterance semantics as ``transcribe`` (norm_audio, 0.5 s of silence on both sides, greedy decode,
     decode_hypothesis); the padding is written straight into the staging buffer and the post-processing of one batch
     overlaps the engine call of the next.  A model object without ``iter_token_batches`` (e.g. a real NeMo model)
-    is driven through its ``transcribe`` method instead."""
+    is driven through its ``transcribe`` method instead.
+
+    ``phrases``: one ``PhraseBoostingConfig`` or None (the model's global list) per audio: utterances with different key
+    phrases share the batches, each decoded against its own list (greedy decoding only)."""
     if config is None:
         config = TranscribeConfig()
+    if phrases is not None:
+        phrases = check_phrases(model, phrases, len(audios))
+        if not hasattr(model, "iter_token_batches"):
+            raise ValueError("phrases= needs a model of this package (load_model)")
     out: List[Optional[TranscribeResult]] = [None] * len(audios)
 
     def finish(i, hyp):
@@ -484,9 +575,9 @@ def transcribe_batch(model, audios: Sequence[AudioData], config: Optional[Transc
                        for a in audios}) == 1 and
                   (audios[0].samplerate != SAMPLERATE or np.asarray(audios[0].waveform).ndim == 2))
         if raw_ok:
-            batches = model.iter_token_batches_raw([np.asarray(a.waveform) for a in audios], audios[0].samplerate, pad=pad)
+            batches = model.iter_token_batches_raw([np.asarray(a.waveform) for a in audios], audios[0].samplerate, pad=pad, phrases=phrases)
         else:
-            batches = model.iter_token_batches([np.asarray(norm_audio(a).waveform) for a in audios], pad=pad)
+            batches = model.iter_token_batches([np.asarray(norm_audio(a).waveform) for a in audios], pad=pad, phrases=phrases)
         for idx, items in batches:
             for i, item in zip(idx, items):
                 finish(i, greedy_hypothesis(model, item))

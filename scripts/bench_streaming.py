@@ -32,12 +32,13 @@ def card():
         return f"unknown ({exc})"
 
 
-def run(model, N, config, clips, timed):
+def run(model, N, config, clips, timed, lists=None):
+    """``lists``: stream k is opened with its own phrase list ``lists[k % len(lists)]`` (None: the model's global list)."""
     from reazonspeech_b200.nemo.asr import StreamingTranscriber
     C = config.frames()[0]
     piece = C * 1280
     st = StreamingTranscriber(model, config, max_streams=N)
-    ids = [st.open() for _ in range(N)]
+    ids = [st.open(boosting=None if lists is None else lists[k % len(lists)]) for k in range(N)]
     pos = [0] * N
     eng = model.engine
     wall, dev, dec = [], [], []
