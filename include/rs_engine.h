@@ -256,13 +256,39 @@ int rs_ngram_lm_eval(rs_engine* e, const int32_t* states_dev, const int32_t* tok
 int rs_rnnt_alsd(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, int beam,
                  double u_max_ratio, int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev,
                  int32_t* n_dev, double* score_dev, int U_cap, void* stream);
+/* The N-best list of the same search (NeMo's BeamRNNTInfer with return_best_hypothesis=False): the same launches as
+ * rs_rnnt_alsd, and every beam, scored row and winner bit-identical to it.  The N-best list of an utterance is the first
+ * n_best entries of Python's stable sorted(pool, key, reverse=True), where
+ *   pool = NeMo's `final`: every stay at the last frame, in append order (A order within a step, steps ascending),
+ *          duplicates included; if nothing finished, the last beam in slot order;
+ *   key  = score / len(y) with score_norm (len(y) counts the leading blank), else score; equal keys keep pool order.
+ * A finished entry carries the score recombination added into it in the step it finished, as for rs_rnnt_alsd.  Entry 0 is
+ * always what rs_rnnt_alsd returns.  Entry e of utterance b is row b * n_best + e of y [B][n_best][U_cap + 1] (leading
+ * blank), step [B][n_best][U_cap], n [B][n_best] (its full token count; y and step hold the first U_cap tokens) and
+ * score [B][n_best].  count[b] = min(n_best, pool[b]) entries are written, and entries at or past count[b] are left
+ * untouched; pool[b] is the size of NeMo's whole list; from_final[b] is 0 when nothing finished and the last beam was ranked.
+ * enc_len[b] = 0 gives one entry: [blank], n 0, score 0, pool 1, from_final 0.  n_best outside 1..RS_MAX_NBEST, or any
+ * argument rs_rnnt_alsd rejects, gives RS_ERR_INVALID_ARG before any launch.  The list lives in the engine-owned ALSD
+ * workspace (24 bytes per entry); rs_workspace_bytes is unchanged.  Synchronises before returning. */
+#define RS_MAX_NBEST 64
+int rs_rnnt_alsd_nbest(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, int beam,
+                       double u_max_ratio, int score_norm, int recombine_returns_input, int n_best,
+                       int32_t* y_dev,          /* [B][n_best][U_cap + 1] */
+                       int32_t* step_dev,       /* [B][n_best][U_cap]     */
+                       int32_t* n_dev,          /* [B][n_best] full token count */
+                       double* score_dev,       /* [B][n_best]            */
+                       int32_t* count_dev,      /* [B] entries written = min(n_best, pool) */
+                       int32_t* pool_dev,       /* [B] size of NeMo's whole list */
+                       int32_t* from_final_dev, /* [B] 0: nothing finished, the last beam was ranked */
+                       int U_cap, void* stream);
 /* Test seam: rs_rnnt_alsd (the same launches and results) that also copies the search state into caller-owned device
  * buffers.  R = B * beam rows; row r = b * beam + k is slot k of utterance b.  After the beam update of step i (the
  * anti-diagonal t + u = i), for i < max_steps (later steps are not recorded; steps the search never ran are untouched):
  *   n_hyp [i][b], beam_score / beam_u / beam_node [i][r]: the new beam (slot k < n_hyp: its log-probability, token count, back-pointer node);
  *   row_t [i][r]: frame of the hypothesis in slot k of the previous beam scored at step i (-1: not scored);
  *   cand_logp [i][r][9]: its log p(blank), then the beam best non-blank log-probabilities; cand_tok [i][r][8]: their classes;
- *   has_final / final_key / final_score [i][b]: the best finished hypothesis so far (key = score / (u + 1) with score_norm).
+ *   has_final / final_key / final_score [i][b]: the best finished hypothesis so far (key = score / (u + 1) with score_norm),
+ *   entry 0 of rs_rnnt_alsd_nbest's list.
  * Once at the end, the back-pointer tree [B][node_pitch]: node 0 is the leading blank; node n > 0 is a token node_tok[n]
  * emitted at step node_step[n] after node_parent[n].  node_pitch >= 1 + beam * (T_max + int(u_max_ratio * T_max) + 1);
  * RS_ERR_INVALID_ARG before any launch otherwise, or when a buffer is NULL or max_steps < 0. */

@@ -14,7 +14,8 @@
 //   alsd_reduce_kernel   per row: log-sum-exp, log p(blank), the `beam` best non-blank classes (ties: lower index)
 //   alsd_select_kernel   per utterance: A = [stay, extensions ...] per live hypothesis in beam order, the `beam` best by score
 //                        (stable: ties keep A's order, as Python's sorted does), NeMo's recombine_hypotheses, the finished
-//                        list (hypotheses that took the blank at the last frame), back-pointer nodes of the extensions
+//                        list (hypotheses that took the blank at the last frame; its n_best best kept sorted), back-pointer
+//                        nodes of the extensions
 //   alsd_lstm_in_kernel  extended hypotheses: [embed[token] | h_parent] -> three bf16 planes
 //   [GEMM]               gates = planes . [W_lstm x3]^T + b
 //   alsd_cell_kernel     LSTM cell, new (h, c) (kept hypotheses: copied from the parent); h -> three bf16 planes
@@ -223,10 +224,19 @@ alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int 
         if (!recombine_returns_input) dropped[j] = true;
         break;
       }
-  // finished hypotheses: the stays at the last frame, in A order, keep the best by score / len(y) (score_norm), first one on
-  // ties.  In the reference the entry of `final` is the very object that went into the beam, so a stay picked as the first of
-  // its sequence carries the score recombination added into it; any other stay keeps its own.  Only this step can change
-  // them: a stay at T - 1 is not live at the next one.
+  // finished hypotheses: the stays at the last frame, appended to `final` in A order and kept sorted by score / len(y)
+  // (score_norm) as Python's stable sorted(reverse=True) orders them: a new entry goes after every held entry whose key is >=
+  // its own, and the list keeps its first n_best.  In the reference the entry of `final` is the very object that went into
+  // the beam, so a stay picked as the first of its sequence carries the score recombination added into it; any other stay
+  // keeps its own.  Only this step can change them: a stay at T - 1 is not live at the next one.
+  // The held keys are sorted, so the entries whose key is >= the new one are a prefix: counting them over the whole list
+  // (independent loads) finds the position without a scan that stops at each load.
+  const int N = st.n_best;
+  const size_t fo = static_cast<size_t>(b) * N;
+  double* __restrict__ f_key = st.fin_key + fo;
+  double* __restrict__ f_score = st.fin_score + fo;
+  int* __restrict__ f_node = st.fin_node + fo;
+  int* __restrict__ f_u = st.fin_u + fo;
   for (int a = 0; any_final && a < n_a; ++a) {
     const int r = b * K + a_par[a];
     if (a_tok[a] >= 0 || st.row_t[r] != T - 1) continue;
@@ -234,9 +244,16 @@ alsd_select_kernel(const AlsdState st, const int32_t* __restrict__ enc_len, int 
     for (int j = 0; j < n_new; ++j)
       if (pick[j] == a && !later[j]) s = n_score[j];
     const double key = st.score_norm ? s / static_cast<double>(cur.u[r] + 1) : s;
-    if (!st.has_final[b] || key > st.final_key[b]) {
-      st.has_final[b] = 1; st.final_key[b] = key; st.final_score[b] = s; st.final_node[b] = cur.node[r]; st.final_u[b] = cur.u[r];
+    ++st.fin_pool[b];
+    const int cnt = st.fin_count[b];
+    int pos = 0;
+    for (int e = 0; e < cnt; ++e) pos += f_key[e] >= key;
+    if (pos == N) continue;                            // full, and no held key is below it
+    for (int e = cnt < N ? cnt : N - 1; e > pos; --e) {
+      f_key[e] = f_key[e - 1]; f_score[e] = f_score[e - 1]; f_node[e] = f_node[e - 1]; f_u[e] = f_u[e - 1];
     }
+    f_key[pos] = key; f_score[pos] = s; f_node[pos] = cur.node[r]; f_u[pos] = cur.u[r];
+    st.fin_count[b] = cnt < N ? cnt + 1 : N;
   }
   int w = 0;
   for (int j = 0; j < n_new; ++j) {
@@ -323,48 +340,71 @@ __global__ void alsd_init_kernel(const AlsdState st, int blank) {
   st.nx.hash[r] = 1469598103934665603ull; st.nx_tok[r] = blank;
 }
 
-// grid (B), block 32: walk the back-pointers of the winning hypothesis (best finished one; with none, the best of the last
-// beam by the same key) and write y_sequence (leading blank) and the alignment steps of its tokens.
-__global__ void alsd_output_kernel(const AlsdState st, int blank, int32_t* __restrict__ y_out, int32_t* __restrict__ step_out,
-                                   int32_t* __restrict__ n_out, double* __restrict__ score_out, int U_cap) {
-  const int b = blockIdx.x;
-  if (threadIdx.x != 0) return;
-  int node, u;
-  double score;
-  if (st.has_final[b]) { node = st.final_node[b]; u = st.final_u[b]; score = st.final_score[b]; }
-  else {
-    int best = 0;
-    double bk = -DBL_MAX;
-    const AlsdBeam& cur = st.cur;
-    for (int k = 0; k < cur.n_hyp[b]; ++k) {
-      const int r = b * st.beam + k;
-      const double key = st.score_norm ? cur.score[r] / static_cast<double>(cur.u[r] + 1) : cur.score[r];
-      if (key > bk) { bk = key; best = k; }
-    }
-    const int r = b * st.beam + best;
-    node = cur.node[r]; u = cur.u[r]; score = cur.score[r];
-  }
-  n_out[b] = u;
-  score_out[b] = score;
-  y_out[static_cast<size_t>(b) * (U_cap + 1)] = blank;
+// Entry e of utterance b: y_sequence (leading blank) and the alignment steps of its tokens from the back-pointers of `node`;
+// n is the full token count u, y / steps hold the first U_cap tokens.
+__device__ void alsd_write_entry(const AlsdState& st, int b, int e, int node, int u, double score, int blank, int32_t* __restrict__ y_out,
+                                 int32_t* __restrict__ step_out, int32_t* __restrict__ n_out, double* __restrict__ score_out, int U_cap) {
+  const size_t i = static_cast<size_t>(b) * st.n_best + e;
+  n_out[i] = u;
+  score_out[i] = score;
+  int32_t* y = y_out + i * (U_cap + 1);
+  int32_t* steps = step_out + i * U_cap;
+  const size_t tree = static_cast<size_t>(b) * st.max_nodes;
+  y[0] = blank;
   int pos = u;
   while (node > 0 && pos > 0) {
     if (pos <= U_cap) {
-      y_out[static_cast<size_t>(b) * (U_cap + 1) + pos] = st.node_tok[static_cast<size_t>(b) * st.max_nodes + node];
-      step_out[static_cast<size_t>(b) * U_cap + pos - 1] = st.node_step[static_cast<size_t>(b) * st.max_nodes + node];
+      y[pos] = st.node_tok[tree + node];
+      steps[pos - 1] = st.node_step[tree + node];
     }
-    node = st.node_parent[static_cast<size_t>(b) * st.max_nodes + node];
+    node = st.node_parent[tree + node];
     --pos;
+  }
+}
+
+// grid (B), block 32: the N-best list of every utterance, one entry per lane.  With a finished hypothesis, the held entries
+// of the list; with none, the last beam ranked by the same key, stable in slot order (entry 0 is the winner either way).
+__global__ void __launch_bounds__(32)
+alsd_output_kernel(const AlsdState st, int blank, int32_t* __restrict__ y_out, int32_t* __restrict__ step_out, int32_t* __restrict__ n_out,
+                   double* __restrict__ score_out, int32_t* __restrict__ count_out, int32_t* __restrict__ pool_out,
+                   int32_t* __restrict__ from_final_out, int U_cap) {
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const int N = st.n_best;
+  const int pool = st.fin_pool[b];
+  if (pool > 0) {
+    const size_t fo = static_cast<size_t>(b) * N;
+    for (int e = lane; e < st.fin_count[b]; e += 32)
+      alsd_write_entry(st, b, e, st.fin_node[fo + e], st.fin_u[fo + e], st.fin_score[fo + e], blank, y_out, step_out, n_out, score_out, U_cap);
+  } else if (lane < st.cur.n_hyp[b]) {                 // slot `lane` of the last beam goes to entry `rank`
+    const AlsdBeam& cur = st.cur;
+    auto key = [&](int k) {
+      const int r = b * st.beam + k;
+      return st.score_norm ? cur.score[r] / static_cast<double>(cur.u[r] + 1) : cur.score[r];
+    };
+    const double mine = key(lane);
+    int rank = 0;
+    for (int k = 0; k < cur.n_hyp[b]; ++k) {
+      const double other = key(k);
+      rank += other > mine || (other == mine && k < lane);
+    }
+    const int r = b * st.beam + lane;
+    if (rank < N) alsd_write_entry(st, b, rank, cur.node[r], cur.u[r], cur.score[r], blank, y_out, step_out, n_out, score_out, U_cap);
+  }
+  if (lane == 0 && count_out != nullptr) {
+    const int n_pool = pool > 0 ? pool : st.cur.n_hyp[b];
+    count_out[b] = n_pool < N ? n_pool : N;
+    pool_out[b] = n_pool;
+    from_final_out[b] = pool > 0 ? 1 : 0;
   }
 }
 
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ host side
-void alsd_layout_state(AlsdState& st, Arena& a, char* base, int B, int beam, int Hp, int Hj, int max_nodes, bool score_norm) {
-  const size_t R = static_cast<size_t>(B) * beam;
+void alsd_layout_state(AlsdState& st, Arena& a, char* base, int B, int beam, int Hp, int Hj, int max_nodes, bool score_norm, int n_best) {
+  const size_t R = static_cast<size_t>(B) * beam, F = static_cast<size_t>(B) * n_best;
   auto take = [&](size_t bytes) { return reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(base) + a.take(bytes)); };
-  st.beam = beam; st.max_nodes = max_nodes; st.score_norm = score_norm ? 1 : 0;
+  st.beam = beam; st.max_nodes = max_nodes; st.score_norm = score_norm ? 1 : 0; st.n_best = n_best;
   for (AlsdBeam* m : {&st.cur, &st.nx}) {
     m->score = static_cast<double*>(take(R * 8)); m->hash = static_cast<unsigned long long*>(take(R * 8));
     m->u = static_cast<int*>(take(R * 4)); m->node = static_cast<int*>(take(R * 4));
@@ -373,10 +413,10 @@ void alsd_layout_state(AlsdState& st, Arena& a, char* base, int B, int beam, int
   }
   st.nx_parent = static_cast<int*>(take(R * 4)); st.nx_tok = static_cast<int*>(take(R * 4)); st.row_t = static_cast<int*>(take(R * 4));
   st.cand_logp = static_cast<float*>(take(R * (kMaxBeam + 1) * 4)); st.cand_tok = static_cast<int*>(take(R * kMaxBeam * 4));
-  int* ints = static_cast<int*>(take(static_cast<size_t>(B) * 4 * 5));
-  st.done = ints; st.has_final = ints + B; st.n_nodes = ints + 2 * B; st.final_node = ints + 3 * B; st.final_u = ints + 4 * B;
-  double* dbl = static_cast<double*>(take(static_cast<size_t>(B) * 8 * 2));
-  st.final_key = dbl; st.final_score = dbl + B;
+  int* ints = static_cast<int*>(take(static_cast<size_t>(B) * 4 * 4));
+  st.done = ints; st.n_nodes = ints + B; st.fin_count = ints + 2 * B; st.fin_pool = ints + 3 * B;
+  st.fin_key = static_cast<double*>(take(F * 8)); st.fin_score = static_cast<double*>(take(F * 8));
+  st.fin_node = static_cast<int*>(take(F * 4)); st.fin_u = static_cast<int*>(take(F * 4));
   int* tree = static_cast<int*>(take(static_cast<size_t>(B) * max_nodes * 4 * 3));
   st.node_parent = tree; st.node_tok = tree + static_cast<size_t>(B) * max_nodes; st.node_step = tree + 2 * static_cast<size_t>(B) * max_nodes;
   st.n_done = static_cast<int*>(take(4));
@@ -406,8 +446,9 @@ cudaError_t alsd_launch_cell(const AlsdState& st, int B, const float* gates, int
   alsd_cell_kernel<<<B * st.beam, 128, 0, s>>>(st, gates, Hp, static_cast<__nv_bfloat16*>(planes));
   return cudaGetLastError();
 }
-cudaError_t alsd_launch_output(const AlsdState& st, int B, int blank, int32_t* y, int32_t* steps, int32_t* n, double* score, int U_cap, cudaStream_t s) {
-  alsd_output_kernel<<<B, 32, 0, s>>>(st, blank, y, steps, n, score, U_cap);
+cudaError_t alsd_launch_output(const AlsdState& st, int B, int blank, int32_t* y, int32_t* steps, int32_t* n, double* score, int32_t* count,
+                               int32_t* pool, int32_t* from_final, int U_cap, cudaStream_t s) {
+  alsd_output_kernel<<<B, 32, 0, s>>>(st, blank, y, steps, n, score, count, pool, from_final, U_cap);
   return cudaGetLastError();
 }
 

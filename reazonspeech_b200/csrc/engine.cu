@@ -868,14 +868,17 @@ int rs_stream_step(rs_engine* e, const void* wav_host, int wav_is_pcm16, const i
 namespace {
 
 // ALSD beam search over encoder outputs (decode_alsd.cu; semantics: oracle/alsd_restated.py).  Synchronises: the host checks every
-// 32 steps whether every utterance's search has ended.  tr set: the trace seam (rs_rnnt_alsd_trace), which copies the state of
-// every step out after the beam update; rs_rnnt_alsd passes nullptr, so the two run the same launches.
+// 32 steps whether every utterance's search has ended.  The search keeps the n_best best finished hypotheses and writes them
+// all; rs_rnnt_alsd and the trace seam run it with n_best = 1 and without the per-utterance list sizes (count == nullptr).
+// tr set: the trace seam (rs_rnnt_alsd_trace), which copies the state of every step out after the beam update; rs_rnnt_alsd
+// passes nullptr, so the two run the same launches.
 int rnnt_alsd(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, double u_max_ratio,
-              int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev, int U_cap,
-              const rs_alsd_trace* tr, cudaStream_t s) {
+              int score_norm, int recombine_returns_input, int n_best, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev,
+              int32_t* count_dev, int32_t* pool_dev, int32_t* from_final_dev, int U_cap, const rs_alsd_trace* tr, cudaStream_t s) {
   if (!e || !enc || !enc_len || !y_dev || !step_dev || !n_dev || !score_dev || B <= 0 || T_max <= 0 || U_cap <= 0 || beam < 1 || beam > 8 ||
-      !(u_max_ratio >= 0.0))
-    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments (beam must be 1..8)", fn);
+      !(u_max_ratio >= 0.0) || n_best < 1 || n_best > RS_MAX_NBEST || (count_dev != nullptr) != (pool_dev != nullptr) ||
+      (count_dev != nullptr) != (from_final_dev != nullptr))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments (beam must be 1..8, n_best 1..%d)", fn, RS_MAX_NBEST);
   const int total_steps = T_max + static_cast<int>(u_max_ratio * static_cast<double>(T_max));
   const int max_nodes = 1 + beam * (total_steps + 1);
   if (tr && (tr->max_steps < 0 || tr->node_pitch < max_nodes || !tr->n_hyp || !tr->beam_score || !tr->beam_u || !tr->beam_node || !tr->row_t ||
@@ -898,7 +901,7 @@ int rnnt_alsd(rs_engine* e, const char* fn, const float* enc, const int32_t* enc
   const size_t o_state = a.off;
   rs::AlsdState st{};
   rs::Arena state_plan = a;
-  rs::alsd_layout_state(st, state_plan, nullptr, B, beam, Hp, Hj, max_nodes, score_norm != 0);
+  rs::alsd_layout_state(st, state_plan, nullptr, B, beam, Hp, Hj, max_nodes, score_norm != 0, n_best);
   const size_t need_bytes = state_plan.off;
   if (need_bytes > e->alsd_ws_bytes) {
     RS_CUDA(e, cudaStreamSynchronize(s));
@@ -911,7 +914,7 @@ int rnnt_alsd(rs_engine* e, const char* fn, const float* enc, const int32_t* enc
   void* xn = ws + o_xn; float* encp = reinterpret_cast<float*>(ws + o_encp); void* planes = ws + o_planes;
   float* logits = reinterpret_cast<float*>(ws + o_logits); float* gates = reinterpret_cast<float*>(ws + o_gates);
   RS_CUDA(e, cudaMemsetAsync(ws + o_state, 0, need_bytes - o_state, s));
-  rs::alsd_layout_state(st, a, ws, B, beam, Hp, Hj, max_nodes, score_norm != 0);
+  rs::alsd_layout_state(st, a, ws, B, beam, Hp, Hj, max_nodes, score_norm != 0, n_best);
   // ---- joint.enc over every frame (as in the greedy path)
   RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, xn, static_cast<int64_t>(M) * d, s));
   RS_TRY(gemm(e, {xn, e->dec.enc_w, e->dec.enc_b, nullptr, encp, M, Hj, d, RS_EPI_BIAS_F32, 1.f}, s));
@@ -941,9 +944,11 @@ int rnnt_alsd(rs_engine* e, const char* fn, const float* enc, const int32_t* enc
       RS_CUDA(e, copy(tr->row_t + o, st.row_t, R * 4));
       RS_CUDA(e, copy(tr->cand_logp + o * 9, st.cand_logp, R * 9 * 4));
       RS_CUDA(e, copy(tr->cand_tok + o * 8, st.cand_tok, R * 8 * 4));
-      RS_CUDA(e, copy(tr->has_final + ob, st.has_final, B * 4));
-      RS_CUDA(e, copy(tr->final_key + ob, st.final_key, B * 8));
-      RS_CUDA(e, copy(tr->final_score + ob, st.final_score, B * 8));
+      // entry 0 of each utterance's finished list (n_best = 1 here, so fin_count is 0 or 1)
+      RS_CUDA(e, copy(tr->has_final + ob, st.fin_count, B * 4));
+      const size_t fp = static_cast<size_t>(n_best) * 8;
+      RS_CUDA(e, cudaMemcpy2DAsync(tr->final_key + ob, 8, st.fin_key, fp, 8, B, cudaMemcpyDeviceToDevice, s));
+      RS_CUDA(e, cudaMemcpy2DAsync(tr->final_score + ob, 8, st.fin_score, fp, 8, B, cudaMemcpyDeviceToDevice, s));
     }
     RS_TRY(predictor());
     if ((step & 31) == 31) {
@@ -952,7 +957,7 @@ int rnnt_alsd(rs_engine* e, const char* fn, const float* enc, const int32_t* enc
       if (*e->alsd_done_host >= B) break;
     }
   }
-  RS_LAUNCH(e, s, 1, rs::alsd_launch_output(st, B, blank, y_dev, step_dev, n_dev, score_dev, U_cap, s));
+  RS_LAUNCH(e, s, 1, rs::alsd_launch_output(st, B, blank, y_dev, step_dev, n_dev, score_dev, count_dev, pool_dev, from_final_dev, U_cap, s));
   if (tr) {
     const size_t dp = static_cast<size_t>(tr->node_pitch) * 4, sp = static_cast<size_t>(max_nodes) * 4;
     RS_CUDA(e, cudaMemcpy2DAsync(tr->node_parent, dp, st.node_parent, sp, sp, B, cudaMemcpyDeviceToDevice, s));
@@ -969,16 +974,25 @@ extern "C" {
 
 int rs_rnnt_alsd(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, double u_max_ratio, int score_norm,
                  int recombine_returns_input, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev, int U_cap, void* stream) {
-  return rnnt_alsd(e, "rs_rnnt_alsd", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, y_dev, step_dev, n_dev,
-                   score_dev, U_cap, nullptr, static_cast<cudaStream_t>(stream));
+  return rnnt_alsd(e, "rs_rnnt_alsd", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, 1, y_dev, step_dev, n_dev,
+                   score_dev, nullptr, nullptr, nullptr, U_cap, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_alsd_nbest(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, double u_max_ratio, int score_norm,
+                       int recombine_returns_input, int n_best, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev,
+                       int32_t* count_dev, int32_t* pool_dev, int32_t* from_final_dev, int U_cap, void* stream) {
+  if (!count_dev || !pool_dev || !from_final_dev)
+    return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_alsd_nbest: bad arguments (count, pool and from_final are required)");
+  return rnnt_alsd(e, "rs_rnnt_alsd_nbest", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, n_best, y_dev,
+                   step_dev, n_dev, score_dev, count_dev, pool_dev, from_final_dev, U_cap, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int rs_rnnt_alsd_trace(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, int beam, double u_max_ratio, int score_norm,
                        int recombine_returns_input, int32_t* y_dev, int32_t* step_dev, int32_t* n_dev, double* score_dev, int U_cap,
                        const rs_alsd_trace* trace, void* stream) {
   if (trace == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_alsd_trace: bad arguments (no trace)");
-  return rnnt_alsd(e, "rs_rnnt_alsd_trace", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, y_dev, step_dev,
-                   n_dev, score_dev, U_cap, trace, static_cast<cudaStream_t>(stream));
+  return rnnt_alsd(e, "rs_rnnt_alsd_trace", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, 1, y_dev, step_dev,
+                   n_dev, score_dev, nullptr, nullptr, nullptr, U_cap, trace, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

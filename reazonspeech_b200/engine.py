@@ -53,8 +53,10 @@ EXPORTS = [
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
-    "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots",
+    "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots", "rs_rnnt_alsd_nbest",
 ]
+
+MAX_NBEST = 64                          # include/rs_engine.h RS_MAX_NBEST
 
 
 # per-step buffers of rs_alsd_trace: (name, dtype, trailing shape); then the back-pointer tree, [B, node_pitch] each
@@ -120,6 +122,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_alsd.restype = ip
     lib.rs_rnnt_alsd_trace.argtypes = [vp, vp, vp, ip, ip, ip, C.c_double, ip, ip, vp, vp, vp, vp, ip, C.POINTER(RsAlsdTrace), vp]
     lib.rs_rnnt_alsd_trace.restype = ip
+    lib.rs_rnnt_alsd_nbest.argtypes = [vp, vp, vp, ip, ip, ip, C.c_double, ip, ip, ip, vp, vp, vp, vp, vp, vp, vp, ip, vp]
+    lib.rs_rnnt_alsd_nbest.restype = ip
     lib.rs_rnnt_align.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp]
     lib.rs_rnnt_align.restype = ip
     lib.rs_rnnt_align_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp]
@@ -563,6 +567,23 @@ class Engine:
                                           int(recombine_returns_input), y.data_ptr(), steps.data_ptr(), n.data_ptr(), score.data_ptr(), U,
                                           self._stream()), "rs_rnnt_alsd")
         return y, steps, n, score
+
+    def alsd_nbest(self, enc: torch.Tensor, enc_len: torch.Tensor, n_best: int, beam: int = 4, u_max_ratio: float = 2.0,
+                   score_norm: bool = True, recombine_returns_input: bool = True, U_cap: Optional[int] = None):
+        """The N-best list of the ALSD search (rs_rnnt_alsd_nbest), best first -> (y [B, N, U_cap + 1] with the leading blank,
+        steps [B, N, U_cap], n [B, N], score [B, N], count [B], pool [B], from_final [B]) device tensors; entries at or past
+        count[b] stay zero.  Entry 0 is what ``alsd`` returns."""
+        B, T, _ = enc.shape
+        assert enc.dtype == torch.float32 and enc.is_contiguous() and enc_len.dtype == torch.int32
+        N = int(n_best)
+        U = U_cap or (T + int(u_max_ratio * T) + 1)
+        y, steps, n, count, pool, from_final = [torch.zeros(*shape, dtype=torch.int32, device=self.device)
+                                                for shape in ((B, N, U + 1), (B, N, U), (B, N), (B,), (B,), (B,))]
+        score = torch.zeros(B, N, dtype=torch.float64, device=self.device)
+        self._check(self.lib.rs_rnnt_alsd_nbest(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, int(beam), float(u_max_ratio), int(score_norm),
+                                                int(recombine_returns_input), N, y.data_ptr(), steps.data_ptr(), n.data_ptr(), score.data_ptr(),
+                                                count.data_ptr(), pool.data_ptr(), from_final.data_ptr(), U, self._stream()), "rs_rnnt_alsd_nbest")
+        return y, steps, n, score, count, pool, from_final
 
     def alsd_trace(self, enc: torch.Tensor, enc_len: torch.Tensor, beam: int = 4, u_max_ratio: float = 2.0, score_norm: bool = True,
                    recombine_returns_input: bool = True, U_cap: Optional[int] = None, max_steps: Optional[int] = None):

@@ -23,7 +23,7 @@ from ...alignment import alignment_hypothesis, pack_labels, validate_labels
 from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables, combine_tables, config_key
 from ...config import ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
-from ...engine import Engine
+from ...engine import MAX_NBEST, Engine
 from ...ngram_lm import NgramLMConfig, NgramLMTables, build_lm_tables
 from ...tokenizer import PieceTableTokenizer, SentencePieceTokenizer, synthetic_pieces
 from ...weights import load_nemo_archive, random_state_dict
@@ -381,6 +381,47 @@ class B200RnntModel:
                 out[i] = Hypothesis(y[r, : k + 1].to(torch.long), steps[r, :k].tolist(), float(score[r]))
         return out
 
+    def transcribe_alsd_nbest(self, waveforms: Sequence[np.ndarray], n_best: int, pad: int = 0,
+                              log_likelihood: bool = False) -> List[List[Hypothesis]]:
+        """The N-best lists of ``transcribe_alsd``'s search (NeMo's return_best_hypothesis=False), best first, one list per
+        waveform: at most ``n_best`` ALSD-shaped hypotheses each, ``score`` the candidate's beam score.  Entry 0 is
+        ``transcribe_alsd``'s hypothesis.  ``log_likelihood``: every candidate is also force-aligned (``Engine.align``) on its
+        batch's encoder output, so ``hypothesis.log_likelihood`` = log P(tokens | audio) (alignment.py), the score for
+        rescoring the list; the log-mel and the encoder do not run again."""
+        eng = self.engine
+        out: List[Optional[List[Hypothesis]]] = [None] * len(waveforms)
+        order = sorted(range(len(waveforms)), key=lambda i: len(waveforms[i]))
+        for lo in range(0, len(order), self.max_batch):
+            idx = order[lo:lo + self.max_batch]
+            wav, lens = self._staging[0].stage([waveforms[i] for i in idx], pad)
+            with torch.cuda.device(eng.device):
+                x = wav.to(eng.device, non_blocking=True)
+                if x.dtype == torch.int16:
+                    x = x.to(torch.float32) * (1.0 / 32768.0)
+                mel, mel_len = eng.log_mel(x, lens.to(eng.device))
+                enc, enc_len = eng.encode(mel, mel_len)
+                res = [a.cpu() for a in eng.alsd_nbest(enc, enc_len, n_best, beam=self.beam_size)]
+                lists = nbest_hypotheses(*res[:5])
+                if log_likelihood:
+                    self._candidate_log_likelihoods(enc, enc_len, lists)
+            for r, i in enumerate(idx):
+                out[i] = lists[r]
+        return out
+
+    def _candidate_log_likelihoods(self, enc: torch.Tensor, enc_len: torch.Tensor, lists: List[List[Hypothesis]]) -> None:
+        """Fills ``log_likelihood`` of every candidate of one batch: its encoder rows gathered with index_select and aligned in
+        chunks of at most ``max_batch`` rows."""
+        eng = self.engine
+        cands = [(r, h) for r, hyps in enumerate(lists) for h in hyps]
+        for lo in range(0, len(cands), self.max_batch):
+            chunk = cands[lo:lo + self.max_batch]
+            rows = torch.tensor([r for r, _ in chunk], dtype=torch.long, device=eng.device)
+            labels, label_len = pack_labels([h.y_sequence.tolist()[1:] for _, h in chunk])
+            loglik = eng.align(enc.index_select(0, rows).contiguous(), enc_len.index_select(0, rows).contiguous(),
+                               torch.from_numpy(labels).to(eng.device), torch.from_numpy(label_len).to(eng.device))[3].cpu()
+            for j, (_, h) in enumerate(chunk):
+                h.log_likelihood = float(loglik[j])
+
     def transcribe(self, audio, batch_size: int = 1, return_hypotheses: bool = True, verbose: bool = True, **_):
         waves = [a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a) for a in audio]
         if self.decoding == "alsd":
@@ -426,6 +467,20 @@ def lm_tables(model, lm: Optional[NgramLMConfig]) -> Optional[NgramLMTables]:
     if getattr(model, "decoding", "greedy") != "greedy":
         raise ValueError("n-gram LM fusion is applied by the greedy decode only (not by ALSD beam search)")
     return build_lm_tables(lm, model.cfg.vocab_size)
+
+
+def nbest_hypotheses(y: torch.Tensor, steps: torch.Tensor, n: torch.Tensor, score: torch.Tensor, count: torch.Tensor) -> List[List[Hypothesis]]:
+    """Host outputs of ``Engine.alsd_nbest`` (y [B, N, U + 1], steps [B, N, U], n / score [B, N], count [B]) -> per utterance
+    its first count[b] entries as ALSD-shaped hypotheses, best first.  An entry longer than U keeps its first U tokens, as
+    ``transcribe_alsd`` does."""
+    out = []
+    for b in range(y.shape[0]):
+        hyps = []
+        for e in range(int(count[b])):
+            k = int(n[b, e])
+            hyps.append(Hypothesis(y[b, e, : k + 1].to(torch.long), steps[b, e, :k].tolist(), float(score[b, e])))
+        out.append(hyps)
+    return out
 
 
 def _items(done, B: int):
@@ -587,6 +642,37 @@ def transcribe_batch(model, audios: Sequence[AudioData], config: Optional[Transc
         for i, hyp in enumerate(hyps):
             finish(i, hyp)
     return out
+
+
+def transcribe_nbest_batch(model, audios: Sequence[AudioData], n_best: int, config: Optional[TranscribeConfig] = None, *,
+                           log_likelihood: bool = False) -> List[List[TranscribeResult]]:
+    """The N-best lists of ALSD beam search (NeMo's BeamRNNTInfer with return_best_hypothesis=False), in input order: for each
+    audio at most ``n_best`` results, best first (ranked by score / len(y) as NeMo ranks its finished hypotheses); entry 0 is
+    what ``transcribe_batch`` returns.  The audio is prepared as ``transcribe`` prepares it, and every result comes from the
+    unchanged ``decode_hypothesis``.  ``result.hypothesis`` always carries the candidate: score = its beam score and, with
+    ``log_likelihood=True``, log_likelihood = log P(tokens | audio) from forced alignment (alignment.py), the usual score
+    for rescoring the list.  Needs a single-GPU model loaded with ``decoding="alsd"``; that, or ``n_best`` outside
+    1..64, raises ValueError before the GPU is touched."""
+    if getattr(model, "decoding", "greedy") != "alsd" or not hasattr(model, "transcribe_alsd_nbest"):
+        raise ValueError("N-best lists come from ALSD beam search on one GPU: use load_model(decoding=\"alsd\") without devices=")
+    if isinstance(n_best, bool) or not isinstance(n_best, (int, np.integer)) or not 1 <= int(n_best) <= MAX_NBEST:
+        raise ValueError(f"n_best must be an integer in 1..{MAX_NBEST}, got {n_best!r}")
+    waves = [_prepare(a) for a in audios]
+    out: List[List[TranscribeResult]] = []
+    for hyps in model.transcribe_alsd_nbest(waves, int(n_best), log_likelihood=log_likelihood):
+        results = []
+        for hyp in hyps:
+            r = decode_hypothesis(model, hyp)
+            r.hypothesis = hyp
+            results.append(r)
+        out.append(results)
+    return out
+
+
+def transcribe_nbest(model, audio: AudioData, n_best: int, config: Optional[TranscribeConfig] = None, *,
+                     log_likelihood: bool = False) -> List[TranscribeResult]:
+    """One utterance of ``transcribe_nbest_batch``."""
+    return transcribe_nbest_batch(model, [audio], n_best, config, log_likelihood=log_likelihood)[0]
 
 
 def _target_ids(model, text) -> List[int]:
