@@ -332,6 +332,21 @@ int rs_rnnt_align_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc
                           const int32_t* labels_dev, const int32_t* label_len_dev, int U_max,
                           float* lp_blank_dev, float* lp_emit_dev, void* stream);
 
+/* Segment alignment of given label sequences inside longer windows (semantics: reazonspeech_b200/alignment.py, "Segment
+ * alignment"): the same lattice as rs_rnnt_align, but the tokens may start and end at any frame and the frames outside
+ * the segment are not charged.  enc f32[B,T_max,d_model] + enc_len, labels i32[B,U_max] + label_len i32[B] (device) ->
+ * seg i32[B,2] (s, e: the segment's first and last frame), frames i32[B,U_max] (each token's emission frame on the best
+ * segment path), token_lp f32[B,U_max] (lp_emit[frame][u - 1] on that path), frame_lp f32[B,T_max] (for t in [s, e] the
+ * path's emissions at t plus the blank that leaves t, sum = viterbi; NaN outside [s, e]), viterbi f32[B] (the best segment
+ * path's log-probability), loglik f32[B] (log P(y | the frames [s, e])).  Entries at or beyond label_len[b] hold frame -1
+ * and NaN.  An utterance with label_len outside [1, U_max], a label outside [0, vocab_size) or enc_len outside [1, T_max]
+ * gets s = e = -1, frames -1 and NaN scores; the others are unaffected.  Scratch, limits (U_max <= 14527) and argument checks
+ * are rs_rnnt_align's; bad host arguments are rejected before any launch. */
+int rs_rnnt_align_segment(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max,
+                          const int32_t* labels_dev, const int32_t* label_len_dev, int U_max, int32_t* seg_dev,
+                          int32_t* frames_dev, float* token_lp_dev, float* frame_lp_dev, float* viterbi_dev,
+                          float* loglik_dev, void* stream);
+
 /* norm_audio on the device (pkg/nemo-asr/src/audio.py:54-68: resample to 16 kHz, then average the channels) fused with
  * transcribe()'s padding (audio.py:70-83): in [B, channels, L_in_max] f32 or int16 PCM at the native rate ->
  * out f32 [B, L_out_row], row b = pad zeros | resampled mono utterance | zeros, len_out[b] = resampled length + 2 pad;

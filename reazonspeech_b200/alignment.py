@@ -19,7 +19,25 @@ and U = 0 is the all-blank path.
 
 On the GPU (csrc/align.cu): a teacher-forced predictor, the lattice on wgmma (the joint's activation split into two IEEE-half
 terms and bf16-exact weights, as the greedy decode's joint: a cell's logits are the decode's for that (t, u) up to summation
-order) and one CTA per utterance for the recursions and the backtrace.  This module holds the host-side helpers."""
+order) and one CTA per utterance for the recursions and the backtrace.  This module holds the host-side helpers.
+
+Segment alignment (``rs_rnnt_align_segment``; captions.py uses it to locate a caption inside its audio window).  The
+lattice is the one above, of a window with T frames and labels y_1..y_U, U >= 1.  The predictor starts from the SOS state
+at u = 0, as in forced alignment: it does not see the text that precedes the caption.  The tokens may start at any frame
+and end at any frame, and the frames outside are not charged:
+
+    delta[t][0] = 0                                   for every t      (the caption may start at any frame)
+    delta[t][u] = max(delta[t-1][u] + lp_blank[t-1][u],  delta[t][u-1] + lp_emit[t][u-1])      u >= 1 (no blank term at t = 0)
+    score       = max_t  delta[t][U] + lp_blank[t][U]                  (the end is free too)
+
+The end frame e is the smallest maximising t; on an exact tie between predecessors the blank one wins.  The backtrace from
+(e, U) gives each token's emission frame; s is the frame of token 1, and the segment [s, e] holds U emissions and one blank
+per frame, the final blank at (e, U) included.  frame_lp[t] (t in [s, e]) is the sum of the path's steps charged to frame t
+(its emissions at t plus the blank that leaves t), so sum(frame_lp) = score.  loglik is the forward recursion above restricted
+to rows [s, e] (alpha[s][0] = 0, ending with the blank at (e, U)): log P(caption | the audio of its segment).  Hence
+loglik >= score >= the full-window Viterbi score of the same lattice.  U = 0, a label outside [0, V) or enc_len outside
+[1, T_max] gives s = e = -1, frames -1 and NaN scores.  On the GPU: rnnt_segment_dp_kernel, one CTA per window, on the
+lattice the forced alignment computes."""
 from __future__ import annotations
 
 from typing import List, Sequence, Tuple

@@ -6,6 +6,8 @@
 //   align_pred_proj_kernel   pred_proj[b][u] = joint.pred(h_u) for all B * (U_max + 1) rows
 //   rnnt_lattice_kernel      log softmax of the joint at every (t, u) cell of every utterance -> lp_blank, lp_emit (wgmma)
 //   rnnt_align_dp_kernel     forward (logaddexp) and Viterbi (max) recursions over the anti-diagonals + backtrace
+//   rnnt_segment_dp_kernel   the segment alignment of a caption inside its window: Viterbi with a free start and a free end,
+//                            backtrace, then the forward recursion over the segment's frames only
 //
 // The lattice kernel.  A CTA owns a tile of 128 cells of one utterance, 16 frames x 8 labels; row r of the tile is cell
 // (t0 + r / 8, u0 + r % 8).  The 24 fp32 source rows (16 enc_proj + 8 pred_proj) stay in shared memory for the whole tile,
@@ -360,6 +362,103 @@ __global__ void __launch_bounds__(256) rnnt_align_dp_kernel(const AlignArgs a) {
   }
 }
 
+// Segment alignment (alignment.py, "Segment alignment"): one CTA per utterance, over anti-diagonals as above.  Pass 1 is the
+// Viterbi recursion with row 0 free at every frame; the thread that owns u = U keeps the best end (it visits (t, U) in
+// increasing t, so a strict > keeps the smallest maximising frame).  The backtrace from (e, U) writes frames, token_lp and
+// frame_lp and finds s.  Pass 2 is the forward recursion of rnnt_align_dp_kernel on rows [s, e] only.
+__global__ void __launch_bounds__(256) rnnt_segment_dp_kernel(const AlignArgs a) {
+  extern __shared__ __align__(16) float s_dp[];                // [2 diagonals][U_max + 1] | (s, e)
+  const int b = blockIdx.x, tid = threadIdx.x, U1 = a.U_max + 1;
+  int* s_se = reinterpret_cast<int*>(s_dp + 2 * U1);         // dynamic: static shared memory would not fit beside the 227 KB opt-in
+  const int T = a.enc_len[b], U = a.label_len[b];
+  int bad = T < 1 || T > a.T_max || U < 1 || U > a.U_max;
+  if (!bad)
+    for (int i = tid; i < U; i += blockDim.x) {
+      const int y = a.labels[static_cast<size_t>(b) * a.U_max + i];
+      if (y < 0 || y >= a.V) bad = 1;
+    }
+  bad = __syncthreads_or(bad);
+  int32_t* frames = a.frames + static_cast<size_t>(b) * a.U_max;
+  float* token_lp = a.token_lp + static_cast<size_t>(b) * a.U_max;
+  float* frame_lp = a.frame_lp + static_cast<size_t>(b) * a.T_max;
+  for (int i = tid; i < a.U_max; i += blockDim.x)
+    if (bad || i >= U) { frames[i] = -1; token_lp[i] = NAN; }
+  for (int i = tid; i < a.T_max; i += blockDim.x) frame_lp[i] = NAN;   // the backtrace overwrites [s, e] after a barrier
+  if (bad) {
+    if (tid == 0) { a.viterbi[b] = NAN; a.loglik[b] = NAN; a.seg[2 * b] = -1; a.seg[2 * b + 1] = -1; }
+    return;
+  }
+  const size_t base = static_cast<size_t>(b) * a.T_max * U1;
+  const float* lpb = a.lp_blank + base;
+  const float* lpe = a.lp_emit + base;
+  uint8_t* choice = a.choice + base;
+  float* cur = s_dp;
+  float* prev = s_dp + U1;
+  float best = -INFINITY;
+  int end = 0;
+  for (int d = 0; d < T + U; ++d) {
+    for (int u = tid; u <= U; u += blockDim.x) {
+      const int t = d - u;
+      if (t < 0 || t >= T) continue;
+      float v = 0.f;                                           // u = 0: the caption may start at any frame
+      if (u > 0) {
+        const float ve = prev[u - 1] + lpe[static_cast<size_t>(t) * U1 + u - 1];
+        const float vb = t > 0 ? prev[u] + lpb[static_cast<size_t>(t - 1) * U1 + u] : -INFINITY;
+        const uint8_t ch = (t == 0 || ve > vb) ? 1 : 0;        // an exact tie goes to the blank predecessor
+        choice[static_cast<size_t>(t) * U1 + u] = ch;
+        v = ch ? ve : vb;
+        if (u == U) {
+          const float sc = v + lpb[static_cast<size_t>(t) * U1 + U];
+          if (sc > best) { best = sc; end = t; }
+        }
+      }
+      cur[u] = v;
+    }
+    __syncthreads();
+    float* x = cur; cur = prev; prev = x;
+  }
+  if (tid == U % blockDim.x) {                                 // the owner of u = U backtraces
+    a.viterbi[b] = best;
+    int t = end, u = U;
+    float acc = lpb[static_cast<size_t>(end) * U1 + U];        // frame t's steps: the blank leaving it, then its emissions
+    while (u > 0) {
+      if (choice[static_cast<size_t>(t) * U1 + u]) {
+        const float l = lpe[static_cast<size_t>(t) * U1 + u - 1];
+        frames[u - 1] = t;
+        token_lp[u - 1] = l;
+        acc += l;
+        --u;
+      } else {
+        frame_lp[t] = acc;
+        --t;
+        acc = lpb[static_cast<size_t>(t) * U1 + u];
+      }
+    }
+    frame_lp[t] = acc;                                         // t = s, the frame of token 1
+    a.seg[2 * b] = t; a.seg[2 * b + 1] = end;
+    s_se[0] = t; s_se[1] = end;
+  }
+  __syncthreads();
+  // pass 2: log P(y | the frames [s, e]) -- alpha[s][0] = 0, the final blank at (e, U)
+  const int s0 = s_se[0], n = s_se[1] - s_se[0] + 1;
+  for (int d = 0; d < n + U; ++d) {
+    for (int u = tid; u <= U; u += blockDim.x) {
+      const int t = d - u;
+      if (t < 0 || t >= n) continue;
+      float f = 0.f;
+      if (d > 0) {
+        const float fb = t > 0 ? prev[u] + lpb[static_cast<size_t>(s0 + t - 1) * U1 + u] : -INFINITY;
+        const float fe = u > 0 ? prev[u - 1] + lpe[static_cast<size_t>(s0 + t) * U1 + u - 1] : -INFINITY;
+        f = logaddexp(fb, fe);
+      }
+      cur[u] = f;
+    }
+    __syncthreads();
+    float* x = cur; cur = prev; prev = x;
+  }
+  if (tid == 0) a.loglik[b] = prev[U] + lpb[static_cast<size_t>(s0 + n - 1) * U1 + U];
+}
+
 }  // namespace
 
 size_t align_dp_smem(int U_max) { return static_cast<size_t>(4) * (U_max + 1) * sizeof(float); }
@@ -405,6 +504,17 @@ cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* e
   }
   const int tiles = ((a.T_max + kTileT - 1) / kTileT) * ((a.U_max + 1 + kTileU - 1) / kTileU);
   rnnt_lattice_kernel<<<a.B * tiles, kLatThreads, smem, stream>>>(tm, a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rnnt_segment_dp(const AlignArgs& a, cudaStream_t stream) {
+  static DeviceOnce attr_once;
+  if (attr_once.pending()) {
+    const cudaError_t e = cudaFuncSetAttribute(rnnt_segment_dp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_once.set();
+  }
+  rnnt_segment_dp_kernel<<<a.B, 256, static_cast<size_t>(2 * (a.U_max + 1) + 2) * sizeof(float), stream>>>(a);
   return cudaGetLastError();
 }
 

@@ -1001,12 +1001,13 @@ namespace {
 
 // Forced alignment (align.cu; semantics: reazonspeech_b200/alignment.py).  lp_blank / lp_emit set: the lattice seam (the
 // caller's buffers, no DP); otherwise the lattice lives in the scratch and the DP writes frames / token_lp / viterbi / loglik.
+// seg set: the segment alignment (rnnt_segment_dp_kernel), which also writes seg and frame_lp.
 int rnnt_align(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, const int32_t* labels,
                const int32_t* label_len, int U_max, float* lp_blank, float* lp_emit, int32_t* frames, float* token_lp, float* viterbi,
-               float* loglik, cudaStream_t s) {
+               float* loglik, cudaStream_t s, int32_t* seg = nullptr, float* frame_lp = nullptr) {
   const bool seam = lp_blank != nullptr;
   if (!e || !enc || !enc_len || !labels || !label_len || B <= 0 || T_max <= 0 || U_max <= 0 ||
-      (seam ? lp_emit == nullptr : (!frames || !token_lp || !viterbi || !loglik)))
+      (seam ? lp_emit == nullptr : (!frames || !token_lp || !viterbi || !loglik)) || (seg != nullptr && (seam || frame_lp == nullptr)))
     return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
   const rs_model_config& c = e->cfg;
   char msg[256] = "";
@@ -1035,7 +1036,7 @@ int rnnt_align(rs_engine* e, const char* fn, const float* enc, const int32_t* en
                   e->dec.gate_tab, e->dec.pred_w, e->dec.pred_b, B, T_max, U_max, Hj, Hp, c.vocab_size,
                   reinterpret_cast<float*>(ws + o_h), reinterpret_cast<float*>(ws + o_c), reinterpret_cast<float*>(ws + o_pp),
                   seam ? lp_blank : reinterpret_cast<float*>(ws + o_lpb), seam ? lp_emit : reinterpret_cast<float*>(ws + o_lpe),
-                  reinterpret_cast<uint8_t*>(ws + o_ch), frames, token_lp, viterbi, loglik};
+                  reinterpret_cast<uint8_t*>(ws + o_ch), frames, token_lp, viterbi, loglik, seg, frame_lp};
   // joint.enc over every frame, as in the greedy path
   RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, ws + o_xn, static_cast<int64_t>(M) * c.d_model, s));
   RS_TRY(gemm(e, {ws + o_xn, e->dec.enc_w, e->dec.enc_b, nullptr, ws + o_encp, M, Hj, c.d_model, RS_EPI_BIAS_F32, 1.f}, s));
@@ -1046,7 +1047,8 @@ int rnnt_align(rs_engine* e, const char* fn, const float* enc, const int32_t* en
     if (r != RS_OK && msg[0] != '\0') return fail(e, r, "%s: %s", fn, msg);
     RS_TRY(r);
   }
-  if (!seam) RS_LAUNCH(e, s, 1, rs::launch_rnnt_align_dp(g, s));
+  if (seg != nullptr) RS_LAUNCH(e, s, 1, rs::launch_rnnt_segment_dp(g, s));
+  else if (!seam) RS_LAUNCH(e, s, 1, rs::launch_rnnt_align_dp(g, s));
   return RS_OK;
 }
 
@@ -1066,6 +1068,14 @@ int rs_rnnt_align_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc
   if (lp_blank_dev == nullptr || lp_emit_dev == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_align_lattice: bad arguments");
   return rnnt_align(e, "rs_rnnt_align_lattice", enc_dev, enc_len_dev, B, T_max, labels_dev, label_len_dev, U_max, lp_blank_dev, lp_emit_dev,
                     nullptr, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_align_segment(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, const int32_t* labels_dev,
+                          const int32_t* label_len_dev, int U_max, int32_t* seg_dev, int32_t* frames_dev, float* token_lp_dev,
+                          float* frame_lp_dev, float* viterbi_dev, float* loglik_dev, void* stream) {
+  if (seg_dev == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_align_segment: bad arguments");
+  return rnnt_align(e, "rs_rnnt_align_segment", enc_dev, enc_len_dev, B, T_max, labels_dev, label_len_dev, U_max, nullptr, nullptr, frames_dev,
+                    token_lp_dev, viterbi_dev, loglik_dev, static_cast<cudaStream_t>(stream), seg_dev, frame_lp_dev);
 }
 
 int rs_resample_mono(rs_engine* e, const void* in_dev, int in_is_pcm16, const int32_t* len_in_dev, int B, int channels, int L_in_max,

@@ -144,6 +144,7 @@ struct AlignArgs {
   float* lp_blank; float* lp_emit;
   uint8_t* choice;            // Viterbi predecessor of every cell (1: the emission from (t, u - 1))
   int32_t* frames; float* token_lp; float* viterbi; float* loglik;
+  int32_t* seg; float* frame_lp;  // segment alignment only: (s, e) [B][2], f32 [B][T_max]
 };
 // shapes the kernels implement (false: err, >= 256 B, says why)
 bool align_supported(int Hj, int Hp, int V, int U_max, char* err);
@@ -154,6 +155,8 @@ cudaError_t launch_align_pred_proj(const AlignArgs& a, cudaStream_t stream);
 cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* err);
 // forward + Viterbi recursions and backtrace -> frames, token_lp, viterbi, loglik
 cudaError_t launch_rnnt_align_dp(const AlignArgs& a, cudaStream_t stream);
+// segment alignment (free start and end) -> seg, frames, token_lp, frame_lp, viterbi, loglik
+cudaError_t launch_rnnt_segment_dp(const AlignArgs& a, cudaStream_t stream);
 
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)
 struct ResampleArgs {

@@ -54,6 +54,7 @@ EXPORTS = [
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
     "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots", "rs_rnnt_alsd_nbest",
+    "rs_rnnt_align_segment",
 ]
 
 MAX_NBEST = 64                          # include/rs_engine.h RS_MAX_NBEST
@@ -128,6 +129,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_align.restype = ip
     lib.rs_rnnt_align_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp]
     lib.rs_rnnt_align_lattice.restype = ip
+    lib.rs_rnnt_align_segment.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp, vp, vp]
+    lib.rs_rnnt_align_segment.restype = ip
     lib.rs_stream_state_bytes.argtypes = [vp]
     lib.rs_stream_state_bytes.restype = C.c_size_t
     lib.rs_rnnt_greedy_resume.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
@@ -638,6 +641,22 @@ class Engine:
                                            frames.data_ptr(), token_lp.data_ptr(), viterbi.data_ptr(), loglik.data_ptr(),
                                            self._stream()), "rs_rnnt_align")
         return frames, token_lp, viterbi, loglik
+
+    def align_segment(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor):
+        """Segment alignment of labels[b, :label_len[b]] inside each row's frames (rs_rnnt_align_segment; semantics:
+        alignment.py) -> (seg i32 [B, 2], frames i32 [B, U], token_lp f32 [B, U], frame_lp f32 [B, T], viterbi f32 [B],
+        loglik f32 [B]) device tensors."""
+        B, T, labels, U = self._align_inputs(enc, enc_len, labels, label_len)
+        seg = torch.empty(B, 2, dtype=torch.int32, device=self.device)
+        frames = torch.empty(B, U, dtype=torch.int32, device=self.device)
+        token_lp = torch.empty(B, U, dtype=torch.float32, device=self.device)
+        frame_lp = torch.empty(B, T, dtype=torch.float32, device=self.device)
+        viterbi = torch.empty(B, dtype=torch.float32, device=self.device)
+        loglik = torch.empty(B, dtype=torch.float32, device=self.device)
+        self._check(self.lib.rs_rnnt_align_segment(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, labels.data_ptr(), label_len.data_ptr(), U,
+                                                   seg.data_ptr(), frames.data_ptr(), token_lp.data_ptr(), frame_lp.data_ptr(),
+                                                   viterbi.data_ptr(), loglik.data_ptr(), self._stream()), "rs_rnnt_align_segment")
+        return seg, frames, token_lp, frame_lp, viterbi, loglik
 
     def align_lattice(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor, out=None):
         """The lattice alone (rs_rnnt_align_lattice) -> (lp_blank, lp_emit) f32 [B, T, U + 1]; cells outside an utterance keep

@@ -32,6 +32,11 @@ Fifth extension, streaming (reazonspeech_b200/streaming.py): the one AUDIO argum
                        output (--to, -o) is written from the whole stream
   --chunk=S --left=S --right=S   chunk and context seconds (multiples of 0.08; default 1.6, 1.2, 1.2)
 Without the option the output is unchanged.
+Sixth extension, caption alignment (reazonspeech_b200/captions.py): the captions of the one AUDIO argument are located in
+its audio, each inside the window [start - before, end + after), and written as segments through the same writer
+  --captions=FILE      UTF-8 lines start<TAB>end<TAB>text in seconds, the format --to=tsv writes (its header line is skipped)
+  --before=S --after=S the window's margins in seconds (default 25 and 0: live captions trail the speech by about 25 s)
+Captions that cannot be located (an empty window, or no token) are skipped.  Without the option the output is unchanged.
 Audio decoding: soundfile when installed, scipy for WAV, librosa for compressed containers, see audio.audio_from_path.
 """
 import dataclasses
@@ -42,7 +47,8 @@ from dataclasses import dataclass, field
 from typing import List, Optional
 
 SHORT_OPTS = "ho:"
-LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=", "stream", "chunk=", "left=", "right=")
+LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=", "stream", "chunk=", "left=", "right=",
+             "captions=", "before=", "after=")
 
 
 @dataclass
@@ -60,6 +66,9 @@ class Options:
     chunk: float = 1.6
     left: float = 1.2
     right: float = 1.2
+    captions: Optional[str] = None
+    before: float = 25.0
+    after: float = 0.0
 
 
 def parse(argv) -> Options:
@@ -85,13 +94,22 @@ def parse(argv) -> Options:
             opt.text = value
         if flag == "--stream":
             opt.stream = True
-        if flag in ("--chunk", "--left", "--right"):
+        if flag in ("--chunk", "--left", "--right", "--before", "--after"):
             setattr(opt, flag[2:], float(value))
+        if flag == "--captions":
+            opt.captions = value
     if (opt.lm is None) != (opt.lm_alpha is None):
         raise ValueError("--lm and --lm-alpha go together: the LM weight has no default (try values around 0.3-0.5 and tune "
                          "on held-out audio)" if opt.lm is not None else "--lm-alpha needs an LM: --lm=FILE")
     if opt.stream and len(opt.audio) > 1:
         raise ValueError("--stream decodes one AUDIO argument (a file, or - for PCM on stdin)")
+    if opt.captions is not None:
+        if len(opt.audio) > 1:
+            raise ValueError("--captions locates the captions of one AUDIO argument")
+        if opt.stream or opt.text is not None:
+            raise ValueError("--captions goes with neither --stream nor --text")
+        if opt.before < 0 or opt.after < 0:
+            raise ValueError(f"--before and --after are margins in seconds >= 0, got {opt.before} and {opt.after}")
     return opt
 
 
@@ -114,6 +132,10 @@ def run(opt: Options) -> None:
     from .writer import get_writer
 
     texts = load_transcripts(opt.text, len(opt.audio)) if opt.text is not None else None
+    captions = None
+    if opt.captions is not None:
+        from ...captions import read_captions_tsv
+        captions = read_captions_tsv(opt.captions)
     sink = sys.stdout if opt.output is None else open(opt.output, "w")
     warnings.simplefilter("ignore")
     clips = [audio_from_path(path) for path in opt.audio] if not (opt.stream and opt.audio == ["-"]) else []
@@ -130,7 +152,9 @@ def run(opt: Options) -> None:
         from ...ngram_lm import NgramLMConfig
         extra["lm"] = NgramLMConfig(opt.lm, opt.lm_alpha)
     model = load_model(**extra)
-    if opt.stream:
+    if captions is not None:
+        results = [caption_segments(model, clips[0], captions, opt)]
+    elif opt.stream:
         results = [stream(model, opt, clips[0] if clips else None)]
     elif texts is not None:
         results = align_batch(model, clips, texts)
@@ -145,6 +169,15 @@ def run(opt: Options) -> None:
                 out.write(segment if offset == 0.0 else
                           dataclasses.replace(segment, start_seconds=segment.start_seconds + offset, end_seconds=segment.end_seconds + offset))
             offset += clips[k].seconds if k < len(clips) else 0.0
+
+
+def caption_segments(model, clip, captions, opt: Options):
+    """--captions: the located captions as one result whose segments are (start, end, caption text), in caption order."""
+    from .interface import Segment, TranscribeResult
+    from .transcribe import align_captions
+    found = [a for a in align_captions(model, clip, captions, before=opt.before, after=opt.after) if a is not None]
+    return TranscribeResult("".join(a.text for a in found), [w for a in found for w in a.subwords],
+                            [Segment(a.start_seconds, a.end_seconds, a.text) for a in found])
 
 
 def stream(model, opt: Options, clip=None):

@@ -24,7 +24,8 @@ from ...sharding import shard_indices
 
 class MultiGpuRnntModel:
     """``replicas``: ``B200RnntModel`` objects, one per device, same weights.  Duck-typed like a single replica:
-    ``iter_token_batches`` / ``transcribe_tokens`` / ``transcribe`` / ``align_tokens`` / ``tokenizer`` / ``cfg``."""
+    ``iter_token_batches`` / ``transcribe_tokens`` / ``transcribe`` / ``align_tokens`` / ``align_segment_tokens`` / ``tokenizer`` /
+    ``cfg``."""
 
     def __init__(self, replicas: Sequence):
         if len(replicas) == 0:
@@ -132,6 +133,21 @@ class MultiGpuRnntModel:
         batches = self._deal(waveforms, lambda replica, mine: replica.iter_align_batches([waveforms[i] for i in mine],
                                                                                           [token_lists[i] for i in mine], pad))
         for idx, items in batches:
+            for i, item in zip(idx, items):
+                results[i] = item
+        return results
+
+    def iter_align_segment_batches(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
+        """``B200RnntModel.iter_align_segment_batches`` over all devices: ``(indices into waveforms, items)`` per finished batch."""
+        from ...alignment import validate_labels
+        token_lists = validate_labels(token_lists, self.cfg.vocab_size, len(waveforms))
+        return self._deal(waveforms, lambda replica, mine: replica.iter_align_segment_batches([waveforms[i] for i in mine],
+                                                                                              [token_lists[i] for i in mine], pad))
+
+    def align_segment_tokens(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
+        """-> [(s, e, frames, token_lp, frame_lp, viterbi, loglik)] in input order, over all devices."""
+        results = [None] * len(waveforms)
+        for idx, items in self.iter_align_segment_batches(waveforms, token_lists, pad):
             for i, item in zip(idx, items):
                 results[i] = item
         return results

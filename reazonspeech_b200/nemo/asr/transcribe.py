@@ -10,7 +10,9 @@ transcribe()/decode_hypothesis() therefore run unmodified on it (see INTEGRATION
 from __future__ import annotations
 
 import contextlib
+import dataclasses
 import glob
+import math
 import os
 from dataclasses import dataclass
 from functools import partial
@@ -20,10 +22,12 @@ import numpy as np
 import torch
 
 from ...alignment import alignment_hypothesis, pack_labels, validate_labels
+from ...captions import AFTER_SECONDS, BEFORE_SECONDS, CONFIDENCE_FRAMES, AlignedCaption, Caption, caption_window
 from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables, combine_tables, config_key
 from ...config import ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
 from ...engine import MAX_NBEST, Engine
+from ...evaluation.utils import calculate_cer, normalize
 from ...ngram_lm import NgramLMConfig, NgramLMTables, build_lm_tables
 from ...tokenizer import PieceTableTokenizer, SentencePieceTokenizer, synthetic_pieces
 from ...weights import load_nemo_archive, random_state_dict
@@ -355,6 +359,43 @@ class B200RnntModel:
         """-> [(frames, token_lp, viterbi, loglik)] in input order (``iter_align_batches``)."""
         results = [None] * len(waveforms)
         for idx, items in self.iter_align_batches(waveforms, token_lists, pad):
+            for i, item in zip(idx, items):
+                results[i] = item
+        return results
+
+    # -- segment alignment of captions inside their windows (alignment.py, captions.py)
+    def iter_align_segment_batches(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
+        """Like ``iter_align_batches``, through rs_rnnt_align_segment: item = (s, e, frames, token_lp, frame_lp, viterbi,
+        loglik) of one window, frame_lp holding frames [s, e] only; a window whose tokens could not be placed (no token, or
+        no frame) has s = e = -1, empty lists and NaN scores."""
+        token_lists = validate_labels(token_lists, self.cfg.vocab_size, len(waveforms))
+        eng = self.engine
+        order = sorted(range(len(waveforms)), key=lambda i: len(waveforms[i]))
+        for lo in range(0, len(order), self.max_batch):
+            idx = order[lo:lo + self.max_batch]
+            wav, lens = self._staging[0].stage([waveforms[i] for i in idx], pad)
+            labels, label_len = pack_labels([token_lists[i] for i in idx])
+            with torch.cuda.device(eng.device):
+                x = wav.to(eng.device, non_blocking=True)
+                if x.dtype == torch.int16:
+                    x = x.to(torch.float32) * (1.0 / 32768.0)
+                mel, mel_len = eng.log_mel(x, lens.to(eng.device))
+                enc, enc_len = eng.encode(mel, mel_len)
+                seg, frames, token_lp, frame_lp, viterbi, loglik = [
+                    a.cpu() for a in eng.align_segment(enc, enc_len, torch.from_numpy(labels).to(eng.device),
+                                                       torch.from_numpy(label_len).to(eng.device))]
+            items = []
+            for r, n in enumerate(label_len.tolist()):
+                s0, e0 = int(seg[r, 0]), int(seg[r, 1])
+                n = n if s0 >= 0 else 0
+                items.append((s0, e0, frames[r, :n].tolist(), token_lp[r, :n].tolist(),
+                              frame_lp[r, s0:e0 + 1].tolist() if s0 >= 0 else [], float(viterbi[r]), float(loglik[r])))
+            yield idx, items
+
+    def align_segment_tokens(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
+        """-> [(s, e, frames, token_lp, frame_lp, viterbi, loglik)] in input order (``iter_align_segment_batches``)."""
+        results = [None] * len(waveforms)
+        for idx, items in self.iter_align_segment_batches(waveforms, token_lists, pad):
             for i, item in zip(idx, items):
                 results[i] = item
         return results
@@ -707,3 +748,47 @@ def align_batch(model, audios: Sequence[AudioData], texts: Sequence, config: Opt
 def align(model, audio: AudioData, text, config: Optional[TranscribeConfig] = None) -> TranscribeResult:
     """One utterance of ``align_batch``."""
     return align_batch(model, [audio], [text], config)[0]
+
+
+def align_captions(model, audio: AudioData, captions: Sequence[Caption], *, before: float = BEFORE_SECONDS,
+                   after: float = AFTER_SECONDS, confidence_frames: int = CONFIDENCE_FRAMES,
+                   transcribe: bool = False) -> List[Optional[AlignedCaption]]:
+    """Locate each caption of a long recording inside its audio window (captions.py): one ``AlignedCaption`` or None per
+    caption, in input order.  The windows [start - before, end + after) are cut from ``audio`` after norm_audio, prepared
+    as ``align_batch`` prepares an audio, batched by length and aligned on the GPU with the segment alignment of
+    alignment.py.  A caption whose window is empty (it lies outside the audio), whose text has no token, or whose window
+    has no encoder frame gets None.  The caption's text is tokenised with ``sentence_to_ids``.  Subwords and the segment
+    are in program seconds.  ``transcribe=True`` transcribes every located segment in one ``transcribe_batch`` call and
+    fills ``asr`` and ``cer`` (evaluation.utils.calculate_cer against the caption), the reference's corpus filter.
+    A caption that ends before it starts raises ValueError before the GPU is touched."""
+    from ...captions import confidence, segment_seconds, window_samples
+    wave = np.asarray(norm_audio(audio).waveform)
+    duration = len(wave) / SAMPLERATE
+    windows = [caption_window(c, duration, before, after) for c in captions]
+    jobs = []                                                   # (caption index, window, token ids)
+    for k, (c, w) in enumerate(zip(captions, windows)):
+        ids = model.tokenizer.sentence_to_ids(c.text) if w is not None else []
+        if ids:
+            jobs.append((k, w, ids))
+    validate_labels([ids for _, _, ids in jobs], model.cfg.vocab_size, len(jobs))
+    waves = []
+    for _, (w0, w1), _ in jobs:
+        lo, hi = window_samples(w0, w1, SAMPLERATE)
+        waves.append(wave[lo:hi])
+    out: List[Optional[AlignedCaption]] = [None] * len(captions)
+    items = model.align_segment_tokens(waves, [ids for _, _, ids in jobs], pad=int(PAD_SECONDS * SAMPLERATE)) if jobs else []
+    for (k, (w0, w1), ids), (s0, e0, frames, token_lp, frame_lp, viterbi, loglik) in zip(jobs, items):
+        if s0 < 0:
+            continue
+        r = decode_hypothesis(model, alignment_hypothesis(ids, frames, token_lp, viterbi, loglik, model.cfg.blank))
+        start, end = segment_seconds(s0, e0, w0, w1)
+        out[k] = AlignedCaption(captions[k], start, end, captions[k].text,
+                                [dataclasses.replace(sw, seconds=sw.seconds + w0) for sw in r.subwords],
+                                float(viterbi), float(loglik), confidence(frame_lp, confidence_frames))
+    if transcribe:
+        found = [a for a in out if a is not None]
+        spans = [AudioData(wave[slice(*window_samples(a.start_seconds, a.end_seconds, SAMPLERATE))], SAMPLERATE) for a in found]
+        for a, r in zip(found, transcribe_batch(model, spans, TranscribeConfig(verbose=False)) if spans else []):
+            a.asr = r.text
+            a.cer = calculate_cer(a.text, r.text)["cer"] if normalize(a.text) else math.nan
+    return out
