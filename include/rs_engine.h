@@ -211,8 +211,8 @@ int rs_set_phrase_boosting(rs_engine* e, const float* bonus_dev, const int32_t* 
  * clears them. */
 int rs_set_boost_roots(rs_engine* e, const int32_t* roots_host, int n);
 
-/* n-gram language-model shallow fusion of the greedy decode (reazonspeech_b200/ngram_lm.py builds the tables from an ARPA file
- * over BPE token ids and states the semantics).  The decision of every (utterance, frame) is the argmax of
+/* n-gram language-model shallow fusion of the greedy decode and of rs_rnnt_maes (reazonspeech_b200/ngram_lm.py builds the
+ * tables from an ARPA file over BPE token ids and states the semantics).  In the greedy decode the decision of every (utterance, frame) is the argmax of
  * logit_k + [k != blank] * (boosting bonus + LM term of k in the utterance's LM state); the state moves on emissions only and
  * starts at start_state in every call.  The LM term of token k in state s is cb[s] + arc_w[a] for the highest-level arc a of
  * token k on s's chain chain[s][0 .. order-1) (arcs of state o: arc_begin[o] .. arc_begin[o+1], sorted by arc_tok), or
@@ -311,6 +311,42 @@ typedef struct rs_alsd_trace {
 int rs_rnnt_alsd_trace(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, int beam,
                        double u_max_ratio, int score_norm, int recombine_returns_input, int32_t* y_dev, int32_t* step_dev,
                        int32_t* n_dev, double* score_dev, int U_cap, const rs_alsd_trace* trace, void* stream);
+
+/* MAES beam search (NeMo BeamRNNTInfer.modified_adaptive_expansion_search, Kim et al. 2020; semantics restated in
+ * oracle/maes_restated.py): enc f32[B,T_max,d_model] + enc_len -> NeMo's sort_nbest of the kept hypotheses after the last
+ * frame, best first.  Entry e of utterance b is row b * n_best + e of y [B][n_best][U_cap + 1] (leading blank, then the
+ * tokens), frames [B][n_best][U_cap] (the encoder frame that emitted each token), n [B][n_best] (its full token count; y and
+ * frames hold the first U_cap tokens) and score [B][n_best] (log-probability, with the LM terms when an LM is set).
+ * count[b] = min(n_best, kept hypotheses) entries are written; entries at or past count[b] are left untouched.  The ranking
+ * key is score / len(y) with score_norm (len(y) counts the leading blank), else score; equal keys keep the beam's order.
+ * enc_len[b] = 0 gives one entry: [blank], n 0, score 0.
+ * Parameters (NeMo's defaults in brackets): beam 1..8 (K = min(beam, vocab_size)); num_steps 2..4 [2] expansion rounds per
+ * frame; prefix_alpha 0..4 [1]; expansion_beta 0..4 [2] (C = K + beta candidates per hypothesis; K + beta <= vocab_size);
+ * expansion_gamma > 0 [2.3]; recombine_returns_input as for rs_rnnt_alsd; n_best 1..K.  An out-of-range parameter gives
+ * RS_ERR_INVALID_ARG, and a worst case of W = K * C^num_steps expansion rows per utterance above RS_MAX_MAES_ROWS gives
+ * RS_ERR_UNSUPPORTED, both before any launch (NeMo's defaults fit at every beam <= 8: 8 * 10^2 = 800).
+ * With an n-gram LM set (rs_set_ngram_lm) every token expansion adds the LM term of its token in the hypothesis's LM context
+ * (the greedy decode's lookup; the context starts at the LM's start state).  Phrase boosting is ignored.
+ * The host learns the number of live expansion rows of each round (their GEMMs' M) by one pinned 4-byte read per round.
+ * Needs the "alsd.*" weight tensors at rs_engine_create.  The workspace is engine-owned and grown on demand (the ALSD one).
+ * Synchronises before returning. */
+#define RS_MAX_MAES_ROWS 1024
+typedef struct rs_maes_params {
+  int32_t beam, num_steps, prefix_alpha, expansion_beta;
+  float expansion_gamma;
+  int32_t score_norm, recombine_returns_input;
+} rs_maes_params;
+int rs_rnnt_maes(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max,
+                 const rs_maes_params* p, int n_best,
+                 int32_t* y_dev,       /* [B][n_best][U_cap + 1] */
+                 int32_t* frames_dev,  /* [B][n_best][U_cap]     */
+                 int32_t* n_dev,       /* [B][n_best] full token count */
+                 double* score_dev,    /* [B][n_best]            */
+                 int32_t* count_dev,   /* [B] entries written = min(n_best, kept) */
+                 int U_cap, void* stream);
+/* Expansion rows of the last rs_rnnt_maes call on this engine: the sum over frames of the rows the expansion rounds ran
+ * through the predictor (*rows), and the frames searched (*frames: T_max of that call). */
+int rs_maes_last_rows(const rs_engine* e, int64_t* rows, int64_t* frames);
 
 /* Forced alignment of given label sequences on the standard RNN-T lattice (semantics: reazonspeech_b200/alignment.py):
  * enc f32[B,T_max,d_model] + enc_len, labels i32[B,U_max] + label_len i32[B] (device) ->

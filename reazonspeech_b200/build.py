@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(HERE, "librs_engine.so")
-SOURCES = ["gemm_wgmma.cu", "logmel.cu", "subsample.cu", "elementwise.cu", "resample.cu", "attention_tc.cu", "decode_spec.cu", "decode_alsd.cu", "align.cu", "host_staging.cu", "engine.cu"]
+SOURCES = ["gemm_wgmma.cu", "logmel.cu", "subsample.cu", "elementwise.cu", "resample.cu", "attention_tc.cu", "decode_spec.cu", "decode_alsd.cu", "decode_maes.cu", "align.cu", "host_staging.cu", "engine.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 FLAGS += os.environ.get("RS_BUILD_FLAGS", "").split()        # extra nvcc flags, build-time only (e.g. -Xptxas -v)

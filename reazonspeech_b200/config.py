@@ -12,6 +12,7 @@ from __future__ import annotations
 import dataclasses
 import math
 from dataclasses import dataclass
+from typing import Optional
 
 
 @dataclass(frozen=True)
@@ -44,6 +45,7 @@ class ModelConfig:
     pred_hidden: int = 640
     joint_hidden: int = 640
     max_symbols: int = 10
+    checkpoint_maes: Optional["MaesConfig"] = dataclasses.field(default=None, compare=False)   # decoding.beam.maes_* of model_config.yaml
     checkpoint_decoding: str = dataclasses.field(default="greedy", compare=False)   # the strategy model_config.yaml asks for (informational: load_model decides what runs)
 
     # ---- derived ----
@@ -217,7 +219,57 @@ class ModelConfig:
             joint_hidden=int(jointnet["joint_hidden"]),
             max_symbols=int(cfg.get("decoding", {}).get("greedy", {}).get("max_symbols", 10) or 10),
             checkpoint_decoding=ModelConfig.decoding_strategy(cfg),
+            checkpoint_maes=MaesConfig.from_beam_block((cfg.get("decoding", {}) or {}).get("beam", {}) or {}),
         )
+
+
+@dataclass(frozen=True)
+class MaesConfig:
+    """Parameters of the MAES beam search (NeMo's maes_* keys of decoding.beam, with NeMo's defaults): ``num_steps``
+    expansion rounds per frame (>= 2), ``prefix_alpha`` the longest prefix-search gap (>= 0), ``expansion_beta`` extra candidates
+    per hypothesis beyond the beam (>= 0), ``expansion_gamma`` the score window of the candidates kept (> 0).  The engine runs
+    num_steps <= 4 and prefix_alpha, expansion_beta <= 4, and at most 1024 expansion rows per utterance
+    (beam * (beam + expansion_beta)^num_steps)."""
+    num_steps: int = 2
+    prefix_alpha: int = 1
+    expansion_beta: int = 2
+    expansion_gamma: float = 2.3
+
+    def validate(self) -> "MaesConfig":
+        if int(self.num_steps) != self.num_steps or not 2 <= int(self.num_steps) <= 4:
+            raise ValueError(f"maes num_steps must be an integer in 2..4, got {self.num_steps!r}")
+        for name in ("prefix_alpha", "expansion_beta"):
+            v = getattr(self, name)
+            if int(v) != v or not 0 <= int(v) <= 4:
+                raise ValueError(f"maes {name} must be an integer in 0..4, got {v!r}")
+        g = float(self.expansion_gamma)
+        if not (math.isfinite(g) and g > 0.0):
+            raise ValueError(f"maes expansion_gamma must be finite and > 0, got {self.expansion_gamma!r}")
+        return self
+
+    def check_beam(self, beam: int, vocab_size: int) -> "MaesConfig":
+        """The limits that depend on the beam: 1..8, beam + expansion_beta <= vocab_size, at most 1024 expansion rows."""
+        self.validate()
+        if int(beam) != beam or not 1 <= int(beam) <= 8:
+            raise ValueError(f"beam_size must be an integer in 1..8 for MAES, got {beam!r}")
+        k = min(int(beam), int(vocab_size))
+        if k + self.expansion_beta > vocab_size:
+            raise ValueError(f"beam_size + expansion_beta = {k + self.expansion_beta} exceeds the vocabulary ({vocab_size})")
+        w = k * (k + self.expansion_beta) ** self.num_steps
+        if w > 1024:
+            raise ValueError(f"beam_size * (beam_size + expansion_beta)^num_steps = {w} expansion rows exceed the engine's 1024")
+        return self
+
+    @staticmethod
+    def from_beam_block(beam: dict) -> Optional["MaesConfig"]:
+        """NeMo's decoding.beam block -> the MaesConfig its maes_* keys give (None: it has none)."""
+        keys = {"maes_num_steps": "num_steps", "maes_prefix_alpha": "prefix_alpha", "maes_expansion_beta": "expansion_beta",
+                "maes_expansion_gamma": "expansion_gamma"}
+        kw = {f: beam[k] for k, f in keys.items() if beam.get(k) is not None}
+        if not kw:
+            return None
+        kw = {f: float(v) if f == "expansion_gamma" else int(v) for f, v in kw.items()}
+        return MaesConfig(**kw)
 
 
 def jointnet_probe(cfg: dict) -> dict:

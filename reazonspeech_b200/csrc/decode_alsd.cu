@@ -29,6 +29,7 @@
 #include <cfloat>
 
 #include "alsd.h"
+#include "beam_common.cuh"
 #include "common.cuh"
 #include "kernels.h"
 
@@ -37,14 +38,6 @@ namespace rs {
 namespace {
 
 constexpr int kMaxBeam = 8;
-
-// x -> three bf16 values with hi + mid + lo == x to 24 mantissa bits
-__device__ __forceinline__ void split3(float x, __nv_bfloat16& hi, __nv_bfloat16& mid, __nv_bfloat16& lo) {
-  hi = __float2bfloat16_rn(x);
-  const float r1 = x - __bfloat162float(hi);
-  mid = __float2bfloat16_rn(r1);
-  lo = __float2bfloat16_rn(r1 - __bfloat162float(mid));
-}
 
 // ---------------------------------------------------------------------------------------------- joint rows
 // grid (B * beam), block 128.  Row r = b * beam + k.  Dead rows (hypothesis absent, or past the last frame) are zero-filled:
@@ -79,69 +72,11 @@ __global__ void __launch_bounds__(256)
 alsd_reduce_kernel(const AlsdState st, const float* __restrict__ logits, int ld, int V) {
   const int r = blockIdx.x;
   if (st.row_t[r] < 0) return;
-  __shared__ float s_red[8];
-  __shared__ float s_val[8];
-  __shared__ int s_idx[8];
-  const float* x = logits + static_cast<size_t>(r) * ld;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int NC = V + 1;
-  float mx = -FLT_MAX;
-  for (int j = tid; j < NC; j += 256) mx = fmaxf(mx, x[j]);
-  mx = warp_max(mx);
-  if (lane == 0) s_red[warp] = mx;
-  __syncthreads();
-  mx = s_red[0];
-#pragma unroll
-  for (int w = 1; w < 8; ++w) mx = fmaxf(mx, s_red[w]);
-  __syncthreads();
-  float se = 0.f;
-  for (int j = tid; j < NC; j += 256) se += expf(x[j] - mx);
-  se = warp_sum(se);
-  if (lane == 0) s_red[warp] = se;
-  __syncthreads();
-  float tot = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) tot += s_red[w];
-  const float lse = mx + logf(tot);
-  if (tid == 0) st.cand_logp[r * (kMaxBeam + 1)] = x[V] - lse;            // blank
-  // top-`beam` non-blank classes: `beam` rounds of (max, lowest index), each round excluding what was taken before
-  float prev_v = FLT_MAX;
-  int prev_i = -1;
-  for (int round = 0; round < st.beam; ++round) {
-    float bv = -FLT_MAX;
-    int bi = 0x7fffffff;
-    for (int j = tid; j < V; j += 256) {
-      const float v = x[j];
-      const bool after = v < prev_v || (v == prev_v && j > prev_i);        // strictly after the previous pick in (value desc, index asc) order
-      if (after && (v > bv || (v == bv && j < bi))) { bv = v; bi = j; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-    }
-    __syncthreads();
-    if (lane == 0) { s_val[warp] = bv; s_idx[warp] = bi; }
-    __syncthreads();
-    bv = s_val[0]; bi = s_idx[0];
-#pragma unroll
-    for (int w = 1; w < 8; ++w)
-      if (s_val[w] > bv || (s_val[w] == bv && s_idx[w] < bi)) { bv = s_val[w]; bi = s_idx[w]; }
-    if (tid == 0) {
-      st.cand_logp[r * (kMaxBeam + 1) + 1 + round] = bv - lse;
-      st.cand_tok[r * kMaxBeam + round] = bi;
-    }
-    prev_v = bv; prev_i = bi;
-  }
+  beam_row_reduce(logits + static_cast<size_t>(r) * ld, V + 1, V, st.beam, nullptr, st.cand_logp + r * (kMaxBeam + 1),
+                  st.cand_logp + r * (kMaxBeam + 1) + 1, st.cand_tok + r * kMaxBeam);
 }
 
 // ---------------------------------------------------------------------------------------------- beam update
-__device__ __forceinline__ double logaddexp(double a, double b) {
-  const double hi = a > b ? a : b, lo = a > b ? b : a;
-  return hi + log1p(exp(lo - hi));
-}
-
 // grid (B), block 32 (lane 0 does the serial work: at most beam * (beam + 1) <= 72 candidates).
 // u_max = int(u_max_ratio * T) in double, as NeMo computes it: in fp32, ratio 1.16 at T = 25 gives 29 instead of 28.
 __global__ void __launch_bounds__(32)

@@ -19,6 +19,7 @@
 #include "alsd.h"
 #include "kernels.h"
 #include "logmel.h"
+#include "maes.h"
 
 namespace {
 
@@ -73,7 +74,8 @@ struct rs_engine {
   struct { const void *out_w3 = nullptr, *lstm_w3 = nullptr, *pred_w3 = nullptr; const float* out_b = nullptr; int n_pad = 0; } alsd;
   void* alsd_ws = nullptr;
   size_t alsd_ws_bytes = 0;
-  int* alsd_done_host = nullptr;
+  int* alsd_done_host = nullptr;       // also the per-round row count of MAES (rs_rnnt_maes)
+  int64_t maes_rows = 0, maes_frames = 0;   // rs_maes_last_rows
   // forced alignment (align.cu): scratch grown on demand like the ALSD workspace
   void* align_ws = nullptr;
   size_t align_ws_bytes = 0;
@@ -92,7 +94,7 @@ struct rs_engine {
   std::vector<int32_t> roots_host;
   int32_t* boost_roots = nullptr;
   int n_roots = 0, roots_cap = 0;
-  // n-gram LM shallow fusion (rs_set_ngram_lm): caller-owned device tables used by every greedy decode while set; order 0: none
+  // n-gram LM shallow fusion (rs_set_ngram_lm): caller-owned device tables used by every greedy decode and rs_rnnt_maes while set; order 0: none
   rs::NgramLM lm;
   void* ws = nullptr;
   size_t ws_bytes = 0;
@@ -993,6 +995,117 @@ int rs_rnnt_alsd_trace(rs_engine* e, const float* enc, const int32_t* enc_len, i
   if (trace == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_alsd_trace: bad arguments (no trace)");
   return rnnt_alsd(e, "rs_rnnt_alsd_trace", enc, enc_len, B, T_max, beam, u_max_ratio, score_norm, recombine_returns_input, 1, y_dev, step_dev,
                    n_dev, score_dev, nullptr, nullptr, nullptr, U_cap, trace, static_cast<cudaStream_t>(stream));
+}
+
+// MAES beam search over encoder outputs (decode_maes.cu; semantics: oracle/maes_restated.py).  Exactly T_max frames; each
+// expansion round's live rows are compacted on the device and their count read back through a pinned word, so every GEMM of the
+// round runs over the live rows only.
+int rs_rnnt_maes(rs_engine* e, const float* enc, const int32_t* enc_len, int B, int T_max, const rs_maes_params* p, int n_best,
+                 int32_t* y_dev, int32_t* frames_dev, int32_t* n_dev, double* score_dev, int32_t* count_dev, int U_cap, void* stream) {
+  static const char* fn = "rs_rnnt_maes";
+  if (!e || !enc || !enc_len || !p || !y_dev || !frames_dev || !n_dev || !score_dev || !count_dev || B <= 0 || T_max <= 0 || U_cap <= 0)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  const int V = e->cfg.vocab_size;
+  const int K = std::min(p->beam, V), S = p->num_steps, alpha = p->prefix_alpha, beta = p->expansion_beta;
+  if (p->beam < 1 || p->beam > 8 || S < 2 || S > rs::kMaesMaxSteps || alpha < 0 || alpha > 4 || beta < 0 || beta > 4 ||
+      !(p->expansion_gamma > 0.f) || !std::isfinite(p->expansion_gamma) || K + beta > V || n_best < 1 || n_best > K)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad parameters (beam 1..8, num_steps 2..4, prefix_alpha 0..4, expansion_beta 0..4, "
+                "expansion_gamma > 0, beam + expansion_beta <= vocab_size, n_best 1..beam)", fn);
+  const int C = K + beta;
+  int64_t W = K;
+  for (int n = 0; n < S; ++n) W *= C;
+  if (W > RS_MAX_MAES_ROWS)
+    return fail(e, RS_ERR_UNSUPPORTED, "%s: beam * (beam + expansion_beta)^num_steps = %lld expansion rows per utterance exceed %d", fn,
+                static_cast<long long>(W), RS_MAX_MAES_ROWS);
+  if (e->alsd.out_w3 == nullptr)
+    return fail(e, RS_ERR_UNSUPPORTED, "%s: the engine was created without the beam-search weight tensors (alsd.*)", fn);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  Nvtx range("rs::rnnt_maes");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const rs_model_config& c = e->cfg;
+  const int Hj = c.joint_hidden, Hp = c.pred_hidden, d = c.d_model, blank = V, n_pad = e->alsd.n_pad;
+  const int M_enc = B * T_max, R = B * K, P = std::max(alpha, 1);
+  const int max_nodes = 1 + T_max * K * S;
+  const int rows_max = std::max(R * P, B * static_cast<int>(W));
+  // ---- workspace: scratch, then the search state, laid out once to size it and once more to bind it
+  rs::Arena a;
+  const size_t o_xn = a.take(static_cast<size_t>(M_enc) * d * 2), o_encp = a.take(static_cast<size_t>(M_enc) * Hj * 4);
+  const size_t plane_cols = static_cast<size_t>(3 * Hj > 6 * Hp ? 3 * Hj : 6 * Hp);
+  const size_t o_planes = a.take(static_cast<size_t>(rows_max) * plane_cols * 2), o_logits = a.take(static_cast<size_t>(rows_max) * n_pad * 4);
+  const size_t o_gates = a.take(static_cast<size_t>(rows_max) * 4 * Hp * 4);
+  const size_t o_state = a.off;
+  rs::MaesState st{};
+  rs::Arena state_plan = a;
+  rs::maes_layout_state(st, state_plan, nullptr, B, K, C, S, P, Hp, Hj, max_nodes);
+  const size_t need_bytes = state_plan.off;
+  if (need_bytes > e->alsd_ws_bytes) {
+    RS_CUDA(e, cudaStreamSynchronize(s));
+    cudaFree(e->alsd_ws); e->alsd_ws = nullptr; e->alsd_ws_bytes = 0;
+    if (cudaMalloc(&e->alsd_ws, need_bytes) != cudaSuccess) {
+      cudaGetLastError();
+      e->alsd_ws = nullptr;
+      return fail(e, RS_ERR_WORKSPACE, "%s: could not allocate %zu bytes of search workspace", fn, need_bytes);
+    }
+    e->alsd_ws_bytes = need_bytes;
+  }
+  if (e->alsd_done_host == nullptr) RS_CUDA(e, cudaMallocHost(reinterpret_cast<void**>(&e->alsd_done_host), sizeof(int)));
+  char* ws = static_cast<char*>(e->alsd_ws);
+  void* xn = ws + o_xn; float* encp = reinterpret_cast<float*>(ws + o_encp); void* planes = ws + o_planes;
+  float* logits = reinterpret_cast<float*>(ws + o_logits); float* gates = reinterpret_cast<float*>(ws + o_gates);
+  RS_CUDA(e, cudaMemsetAsync(ws + o_state, 0, need_bytes - o_state, s));
+  rs::maes_layout_state(st, a, ws, B, K, C, S, P, Hp, Hj, max_nodes);
+  st.alpha = alpha; st.gamma = static_cast<double>(p->expansion_gamma); st.score_norm = p->score_norm != 0; st.rri = p->recombine_returns_input != 0;
+  rs::NgramLM lm = e->lm;
+  // ---- joint.enc over every frame (as in the greedy path)
+  RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, xn, static_cast<int64_t>(M_enc) * d, s));
+  RS_TRY(gemm(e, {xn, e->dec.enc_w, e->dec.enc_b, nullptr, encp, M_enc, Hj, d, RS_EPI_BIAS_F32, 1.f}, s));
+  // predictor of round n's M rows (h, c, then joint.pred into plane 0 of the rows' dec_out history)
+  auto predictor = [&](int n, int M) -> int {
+    RS_LAUNCH(e, s, 1, rs::maes_launch_lstm_in(st, n, M, e->dec.embed, Hp, Hj, blank, planes, s));
+    RS_TRY(gemm(e, {planes, e->alsd.lstm_w3, e->dec.lstm_b, nullptr, gates, M, 4 * Hp, 6 * Hp, RS_EPI_BIAS_F32, 1.f}, s));
+    RS_LAUNCH(e, s, 1, rs::maes_launch_cell(st, n, M, gates, Hp, planes, s));
+    RS_TRY(gemm(e, {planes, e->alsd.pred_w3, e->dec.pred_b, nullptr, st.rows[n].pp, M, Hj, 3 * Hp, RS_EPI_BIAS_F32, 1.f}, s));
+    return RS_OK;
+  };
+  auto joint = [&](int M) { return gemm(e, {planes, e->alsd.out_w3, e->alsd.out_b, nullptr, logits, M, n_pad, 3 * Hj, RS_EPI_BIAS_F32, 1.f}, s); };
+  RS_LAUNCH(e, s, 1, rs::maes_launch_init(st, blank, lm.order != 0 ? lm.start_state : 0, s));
+  RS_TRY(predictor(0, B));
+  RS_LAUNCH(e, s, 1, rs::maes_launch_init_kept(st, Hp, Hj, s));
+  int64_t live_rows = 0;
+  for (int t = 0; t < T_max; ++t) {
+    RS_CUDA(e, cudaMemsetAsync(st.m, 0, rs::kMaesMaxSteps * sizeof(int), s));
+    RS_LAUNCH(e, s, 1, rs::maes_launch_prefix_rows(st, encp, enc_len, T_max, Hj, t, planes, s));
+    RS_TRY(joint(R * P));
+    RS_LAUNCH(e, s, 1, rs::maes_launch_reduce(st, -1, R * P, logits, n_pad, V, s));
+    RS_LAUNCH(e, s, 1, rs::maes_launch_prefix(st, logits, n_pad, s));
+    for (int n = 0; n < S; ++n) {
+      RS_LAUNCH(e, s, 1, rs::maes_launch_expand(st, n, blank, lm, s));
+      RS_CUDA(e, cudaMemcpyAsync(e->alsd_done_host, st.m + n, sizeof(int), cudaMemcpyDeviceToHost, s));
+      RS_CUDA(e, cudaStreamSynchronize(s));
+      const int M = *e->alsd_done_host;
+      if (M == 0) break;                               // every utterance's frame ended in this round
+      live_rows += M;
+      RS_TRY(predictor(n, M));
+      RS_LAUNCH(e, s, 1, rs::maes_launch_rows(st, n, M, encp, T_max, Hj, t, planes, s));
+      RS_TRY(joint(M));
+      RS_LAUNCH(e, s, 1, rs::maes_launch_reduce(st, n, M, logits, n_pad, V, s));
+    }
+    RS_LAUNCH(e, s, 1, rs::maes_launch_select(st, t, s));
+    RS_LAUNCH(e, s, 1, rs::maes_launch_gather(st, Hp, Hj, s));
+    std::swap(st.cur, st.nx);
+  }
+  RS_LAUNCH(e, s, 1, rs::maes_launch_output(st, n_best, blank, y_dev, frames_dev, n_dev, score_dev, count_dev, U_cap, s));
+  RS_CUDA(e, cudaStreamSynchronize(s));
+  e->maes_rows = live_rows;
+  e->maes_frames = T_max;
+  return RS_OK;
+}
+
+int rs_maes_last_rows(const rs_engine* e, int64_t* rows, int64_t* frames) {
+  if (e == nullptr || rows == nullptr || frames == nullptr) return RS_ERR_INVALID_ARG;
+  *rows = e->maes_rows;
+  *frames = e->maes_frames;
+  return RS_OK;
 }
 
 }  // extern "C"

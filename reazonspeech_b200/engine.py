@@ -53,7 +53,7 @@ EXPORTS = [
     "rs_rnnt_greedy_confidence", "rs_transcribe_device_confidence", "rs_transcribe_batch_confidence",
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
-    "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots", "rs_rnnt_alsd_nbest",
+    "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots", "rs_rnnt_alsd_nbest", "rs_rnnt_maes", "rs_maes_last_rows",
     "rs_rnnt_align_segment",
 ]
 
@@ -73,6 +73,11 @@ class RsNgramLM(C.Structure):
     _fields_ = [("order", C.c_int), ("n_states", C.c_int), ("n_arcs", C.c_int), ("pitch", C.c_int), ("start_state", C.c_int),
                 ("cb", C.c_void_p), ("chain", C.c_void_p), ("arc_begin", C.c_void_p), ("arc_tok", C.c_void_p),
                 ("arc_to", C.c_void_p), ("arc_w", C.c_void_p), ("uni_w", C.c_void_p), ("uni_to", C.c_void_p)]
+
+
+class RsMaesParams(C.Structure):
+    _fields_ = [("beam", C.c_int32), ("num_steps", C.c_int32), ("prefix_alpha", C.c_int32), ("expansion_beta", C.c_int32),
+                ("expansion_gamma", C.c_float), ("score_norm", C.c_int32), ("recombine_returns_input", C.c_int32)]
 
 
 class RsAlsdTrace(C.Structure):
@@ -125,6 +130,10 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_alsd_trace.restype = ip
     lib.rs_rnnt_alsd_nbest.argtypes = [vp, vp, vp, ip, ip, ip, C.c_double, ip, ip, ip, vp, vp, vp, vp, vp, vp, vp, ip, vp]
     lib.rs_rnnt_alsd_nbest.restype = ip
+    lib.rs_rnnt_maes.argtypes = [vp, vp, vp, ip, ip, C.POINTER(RsMaesParams), ip, vp, vp, vp, vp, vp, ip, vp]
+    lib.rs_rnnt_maes.restype = ip
+    lib.rs_maes_last_rows.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    lib.rs_maes_last_rows.restype = ip
     lib.rs_rnnt_align.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp]
     lib.rs_rnnt_align.restype = ip
     lib.rs_rnnt_align_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp]
@@ -386,7 +395,7 @@ class Engine:
         self._check(self.lib.rs_set_boost_roots(self.h, r.ctypes.data if r.size else None, int(r.size)), "rs_set_boost_roots")
 
     def set_ngram_lm(self, tables) -> None:
-        """n-gram LM shallow fusion of every greedy decode (rs_set_ngram_lm): ``tables`` an ``ngram_lm.NgramLMTables``, or
+        """n-gram LM shallow fusion of every greedy decode and ``maes`` search (rs_set_ngram_lm): ``tables`` an ``ngram_lm.NgramLMTables``, or
         ``None`` to clear.  The engine keeps its device copies alive while they are set; replacing or clearing a table first
         waits for the work queued on this device's current stream, which may still read the old one."""
         new = None
@@ -587,6 +596,30 @@ class Engine:
                                                 int(recombine_returns_input), N, y.data_ptr(), steps.data_ptr(), n.data_ptr(), score.data_ptr(),
                                                 count.data_ptr(), pool.data_ptr(), from_final.data_ptr(), U, self._stream()), "rs_rnnt_alsd_nbest")
         return y, steps, n, score, count, pool, from_final
+
+    def maes(self, enc: torch.Tensor, enc_len: torch.Tensor, beam: int = 4, n_best: int = 1, num_steps: int = 2, prefix_alpha: int = 1,
+             expansion_beta: int = 2, expansion_gamma: float = 2.3, score_norm: bool = True, recombine_returns_input: bool = True,
+             U_cap: Optional[int] = None):
+        """MAES beam search over encoder outputs (rs_rnnt_maes), fused with the n-gram LM while one is set -> NeMo's sort_nbest
+        list, best first: (y [B, N, U_cap + 1] with the leading blank, frames [B, N, U_cap], n [B, N], score [B, N], count [B])
+        device tensors; entries at or past count[b] stay zero."""
+        B, T, _ = enc.shape
+        assert enc.dtype == torch.float32 and enc.is_contiguous() and enc_len.dtype == torch.int32
+        N = int(n_best)
+        U = U_cap or (T * int(num_steps) + 1)
+        y, frames, n, count = [torch.zeros(*shape, dtype=torch.int32, device=self.device) for shape in ((B, N, U + 1), (B, N, U), (B, N), (B,))]
+        score = torch.zeros(B, N, dtype=torch.float64, device=self.device)
+        p = RsMaesParams(int(beam), int(num_steps), int(prefix_alpha), int(expansion_beta), float(expansion_gamma), int(score_norm),
+                         int(recombine_returns_input))
+        self._check(self.lib.rs_rnnt_maes(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, C.byref(p), N, y.data_ptr(), frames.data_ptr(),
+                                          n.data_ptr(), score.data_ptr(), count.data_ptr(), U, self._stream()), "rs_rnnt_maes")
+        return y, frames, n, score, count
+
+    def maes_last_rows(self) -> Tuple[int, int]:
+        """(expansion rows run through the predictor, frames searched) of the last ``maes`` call (rs_maes_last_rows)."""
+        rows, frames = C.c_int64(), C.c_int64()
+        self._check(self.lib.rs_maes_last_rows(self.h, C.byref(rows), C.byref(frames)), "rs_maes_last_rows")
+        return rows.value, frames.value
 
     def alsd_trace(self, enc: torch.Tensor, enc_len: torch.Tensor, beam: int = 4, u_max_ratio: float = 2.0, score_norm: bool = True,
                    recombine_returns_input: bool = True, U_cap: Optional[int] = None, max_steps: Optional[int] = None):

@@ -37,6 +37,12 @@ its audio, each inside the window [start - before, end + after), and written as 
   --captions=FILE      UTF-8 lines start<TAB>end<TAB>text in seconds, the format --to=tsv writes (its header line is skipped)
   --before=S --after=S the window's margins in seconds (default 25 and 0: live captions trail the speech by about 25 s)
 Captions that cannot be located (an empty window, or no token) are skipped.  Without the option the output is unchanged.
+Seventh extension, beam search: the decoding strategy of the transcription
+  --decoding=D         greedy (default) | alsd (NeMo's ALSD beam search) | maes (NeMo's modified adaptive expansion search
+                       with its default parameters, or the checkpoint's maes_* settings); --lm / --lm-alpha fuse the LM into
+                       maes as into greedy; alsd takes no LM, no phrases; neither beam search streams
+  --beam=N             beam size of alsd / maes (default 4; maes: 1..8)
+Without the options the output is unchanged.
 Audio decoding: soundfile when installed, scipy for WAV, librosa for compressed containers, see audio.audio_from_path.
 """
 import dataclasses
@@ -48,7 +54,7 @@ from typing import List, Optional
 
 SHORT_OPTS = "ho:"
 LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=", "stream", "chunk=", "left=", "right=",
-             "captions=", "before=", "after=")
+             "captions=", "before=", "after=", "decoding=", "beam=")
 
 
 @dataclass
@@ -69,6 +75,8 @@ class Options:
     captions: Optional[str] = None
     before: float = 25.0
     after: float = 0.0
+    decoding: str = "greedy"
+    beam: Optional[int] = None
 
 
 def parse(argv) -> Options:
@@ -98,9 +106,24 @@ def parse(argv) -> Options:
             setattr(opt, flag[2:], float(value))
         if flag == "--captions":
             opt.captions = value
+        if flag == "--decoding":
+            opt.decoding = value
+        if flag == "--beam":
+            opt.beam = int(value)
     if (opt.lm is None) != (opt.lm_alpha is None):
         raise ValueError("--lm and --lm-alpha go together: the LM weight has no default (try values around 0.3-0.5 and tune "
                          "on held-out audio)" if opt.lm is not None else "--lm-alpha needs an LM: --lm=FILE")
+    if opt.decoding not in ("greedy", "alsd", "maes"):
+        raise ValueError(f"--decoding must be greedy, alsd or maes, got {opt.decoding!r}")
+    if opt.beam is not None and (opt.decoding == "greedy" or opt.beam < 1):
+        raise ValueError("--beam=N (N >= 1) sets the beam of --decoding=alsd or maes")
+    if opt.decoding != "greedy":
+        if opt.lm is not None and opt.decoding == "alsd":
+            raise ValueError("--lm is fused into --decoding=greedy or maes, not alsd")
+        if opt.phrases is not None or opt.phrase_score is not None:
+            raise ValueError("--phrases boosts the greedy decode only")
+        if opt.stream:
+            raise ValueError("--stream decodes greedily")
     if opt.stream and len(opt.audio) > 1:
         raise ValueError("--stream decodes one AUDIO argument (a file, or - for PCM on stdin)")
     if opt.captions is not None:
@@ -151,6 +174,10 @@ def run(opt: Options) -> None:
     if opt.lm is not None:
         from ...ngram_lm import NgramLMConfig
         extra["lm"] = NgramLMConfig(opt.lm, opt.lm_alpha)
+    if opt.decoding != "greedy":
+        extra["decoding"] = opt.decoding
+        if opt.beam is not None:
+            extra["beam_size"] = opt.beam
     model = load_model(**extra)
     if captions is not None:
         results = [caption_segments(model, clips[0], captions, opt)]

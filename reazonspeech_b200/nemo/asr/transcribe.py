@@ -24,7 +24,7 @@ import torch
 from ...alignment import alignment_hypothesis, pack_labels, validate_labels
 from ...captions import AFTER_SECONDS, BEFORE_SECONDS, CONFIDENCE_FRAMES, AlignedCaption, Caption, caption_window
 from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables, combine_tables, config_key
-from ...config import ModelConfig
+from ...config import MaesConfig, ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
 from ...engine import MAX_NBEST, Engine
 from ...evaluation.utils import calculate_cer, normalize
@@ -139,12 +139,13 @@ class B200RnntModel:
 
     def __init__(self, engine: Engine, tokenizer, max_batch: int = 64, decoding: str = "greedy", beam_size: int = 4,
                  confidence: Optional[ConfidenceConfig] = None, boosting: Optional[PhraseBoostingConfig] = None,
-                 lm: Optional[NgramLMConfig] = None):
+                 lm: Optional[NgramLMConfig] = None, maes: Optional[MaesConfig] = None):
         self.engine = engine
         self.cfg = engine.cfg
         self.tokenizer = tokenizer
         self.max_batch = max_batch
-        self.decoding, self.beam_size = decoding, beam_size       # "greedy" (north_star's parity target) or "alsd" (the checkpoint's default)
+        self.decoding, self.beam_size = decoding, beam_size       # "greedy" (north_star's parity target), "alsd" (the checkpoint's default) or "maes"
+        self.maes = (maes or MaesConfig()).check_beam(beam_size, engine.cfg.vocab_size) if decoding == "maes" else None
         if confidence is not None and decoding != "greedy":
             raise ValueError("confidence is computed by the greedy decode only (NeMo offers none for beam search)")
         self.confidence = confidence.validate() if confidence is not None else None
@@ -422,9 +423,28 @@ class B200RnntModel:
                 out[i] = Hypothesis(y[r, : k + 1].to(torch.long), steps[r, :k].tolist(), float(score[r]))
         return out
 
+    def _maes(self, enc: torch.Tensor, enc_len: torch.Tensor, n_best: int):
+        m = self.maes
+        y, frames, n, score, count = [a.cpu() for a in self.engine.maes(enc, enc_len, beam=self.beam_size, n_best=n_best, num_steps=m.num_steps,
+                                                                        prefix_alpha=m.prefix_alpha, expansion_beta=m.expansion_beta,
+                                                                        expansion_gamma=m.expansion_gamma)]
+        steps = frames + torch.arange(1, frames.shape[-1] + 1, dtype=frames.dtype)      # Hypothesis.from_greedy's timestamp convention
+        return y, steps, n, score, count
+
+    def transcribe_maes(self, waveforms: Sequence[np.ndarray], pad: int = 0) -> List[Hypothesis]:
+        """MAES beam search (NeMo's modified_adaptive_expansion_search, fused with the n-gram LM when one is set): the best
+        hypothesis of each waveform, shaped like ``transcribe_alsd``'s (timestamp[i] = frame_i + i + 1)."""
+        return [hyps[0] for hyps in self.transcribe_beam_nbest(waveforms, 1, pad)]
+
+    def transcribe_beam_nbest(self, waveforms: Sequence[np.ndarray], n_best: int, pad: int = 0,
+                              log_likelihood: bool = False) -> List[List[Hypothesis]]:
+        """The N-best lists of the model's beam search, ALSD or MAES by ``decoding`` (``transcribe_alsd_nbest`` runs either)."""
+        return self.transcribe_alsd_nbest(waveforms, n_best, pad, log_likelihood)
+
     def transcribe_alsd_nbest(self, waveforms: Sequence[np.ndarray], n_best: int, pad: int = 0,
                               log_likelihood: bool = False) -> List[List[Hypothesis]]:
-        """The N-best lists of ``transcribe_alsd``'s search (NeMo's return_best_hypothesis=False), best first, one list per
+        """The N-best lists of ``transcribe_alsd``'s search (NeMo's return_best_hypothesis=False; with ``decoding="maes"`` MAES's
+        sort_nbest of its kept hypotheses, n_best <= beam_size), best first, one list per
         waveform: at most ``n_best`` ALSD-shaped hypotheses each, ``score`` the candidate's beam score.  Entry 0 is
         ``transcribe_alsd``'s hypothesis.  ``log_likelihood``: every candidate is also force-aligned (``Engine.align``) on its
         batch's encoder output, so ``hypothesis.log_likelihood`` = log P(tokens | audio) (alignment.py), the score for
@@ -441,8 +461,10 @@ class B200RnntModel:
                     x = x.to(torch.float32) * (1.0 / 32768.0)
                 mel, mel_len = eng.log_mel(x, lens.to(eng.device))
                 enc, enc_len = eng.encode(mel, mel_len)
-                res = [a.cpu() for a in eng.alsd_nbest(enc, enc_len, n_best, beam=self.beam_size)]
-                lists = nbest_hypotheses(*res[:5])
+                if self.decoding == "maes":
+                    lists = nbest_hypotheses(*self._maes(enc, enc_len, n_best))
+                else:
+                    lists = nbest_hypotheses(*[a.cpu() for a in eng.alsd_nbest(enc, enc_len, n_best, beam=self.beam_size)][:5])
                 if log_likelihood:
                     self._candidate_log_likelihoods(enc, enc_len, lists)
             for r, i in enumerate(idx):
@@ -467,6 +489,8 @@ class B200RnntModel:
         waves = [a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a) for a in audio]
         if self.decoding == "alsd":
             out = self.transcribe_alsd(waves)
+        elif self.decoding == "maes":
+            out = self.transcribe_maes(waves)
         else:
             out = [greedy_hypothesis(self, item) for item in self.transcribe_tokens(waves)]
         if return_hypotheses:
@@ -505,8 +529,8 @@ def lm_tables(model, lm: Optional[NgramLMConfig]) -> Optional[NgramLMTables]:
     """Validated tables of ``lm`` for ``model``'s vocabulary (None: fusion off)."""
     if lm is None:
         return None
-    if getattr(model, "decoding", "greedy") != "greedy":
-        raise ValueError("n-gram LM fusion is applied by the greedy decode only (not by ALSD beam search)")
+    if getattr(model, "decoding", "greedy") not in ("greedy", "maes"):
+        raise ValueError("n-gram LM fusion is applied by the greedy decode and MAES beam search only (not by ALSD beam search)")
     return build_lm_tables(lm, model.cfg.vocab_size)
 
 
@@ -547,7 +571,8 @@ def _find_checkpoint() -> Optional[str]:
 def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Optional[bool] = None,
                config: Optional[ModelConfig] = None, seed: int = 0, max_batch: int = 64, devices: Optional[Sequence] = None,
                decoding: str = "greedy", beam_size: int = 4, confidence: Optional[ConfidenceConfig] = None,
-               boosting: Optional[PhraseBoostingConfig] = None, lm: Optional[NgramLMConfig] = None):
+               boosting: Optional[PhraseBoostingConfig] = None, lm: Optional[NgramLMConfig] = None,
+               maes: Optional[MaesConfig] = None):
     """Load the ReazonSpeech FastConformer-RNNT onto a B200.
 
     ``device``: None / "cuda" / "cuda:N" as in the reference (transcribe.py:9-22, eval.py:26).
@@ -563,18 +588,27 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
     ``boosting``: a ``PhraseBoostingConfig`` boosts its key phrases in the greedy decode (``boosting.py``); change or clear
     them later with ``model.set_phrase_boosting``; not available with ``decoding="alsd"``.
     ``lm``: an ``NgramLMConfig`` fuses its ARPA n-gram LM into the greedy decode (``ngram_lm.py``); change or clear it later
-    with ``model.set_ngram_lm``; not available with ``decoding="alsd"``."""
+    with ``model.set_ngram_lm``; not available with ``decoding="alsd"``.
+    ``decoding="maes"``: NeMo's modified adaptive expansion search with ``beam_size`` (csrc/decode_maes.cu), the beam search
+    the n-gram LM of ``lm`` is fused into; ``maes`` (a ``MaesConfig``) sets its parameters, by default the maes_* keys of the
+    checkpoint's decoding.beam block or NeMo's defaults.  Confidence, phrase boosting and ``devices`` are greedy-only."""
+    if decoding not in ("greedy", "alsd", "maes"):
+        raise ValueError(f"decoding must be 'greedy', 'alsd' or 'maes', got {decoding!r}")
+    if maes is not None:
+        if decoding != "maes":
+            raise ValueError("maes= sets the parameters of decoding='maes'")
+        maes.validate()
     if confidence is not None:
-        if decoding == "alsd":
+        if decoding in ("alsd", "maes"):
             raise ValueError("confidence is computed by the greedy decode only (NeMo offers none for beam search)")
         confidence.validate()
     if boosting is not None:
-        if decoding == "alsd":
-            raise ValueError("phrase boosting is applied by the greedy decode only (not by ALSD beam search)")
+        if decoding in ("alsd", "maes"):
+            raise ValueError("phrase boosting is applied by the greedy decode only (not by beam search)")
         boosting.validate()
     if lm is not None:
         if decoding == "alsd":
-            raise ValueError("n-gram LM fusion is applied by the greedy decode only (not by ALSD beam search)")
+            raise ValueError("n-gram LM fusion is applied by the greedy decode and MAES beam search only (not by ALSD beam search)")
         lm.validate()
     if device is None:
         device = "cuda"
@@ -598,11 +632,11 @@ def load_model(device=None, *, checkpoint: Optional[str] = None, synthetic: Opti
         raise FileNotFoundError(
             f"no .nemo checkpoint for {HF_REPO}: pass checkpoint=..., set ${ENV_CHECKPOINT}, populate the Hugging Face "
             f"cache, or request seeded synthetic weights with synthetic=True / ${ENV_SYNTHETIC}=1")
-    if decoding not in ("greedy", "alsd"):
-        raise ValueError(f"decoding must be 'greedy' or 'alsd', got {decoding!r}")
+    if decoding == "maes":
+        maes = (maes or cfg.checkpoint_maes or MaesConfig()).check_beam(beam_size, cfg.vocab_size)
     if devices is None:
-        return B200RnntModel(Engine(cfg, sd, str(device), alsd=decoding == "alsd"), tokenizer, max_batch=max_batch, decoding=decoding, beam_size=beam_size,
-                             confidence=confidence, boosting=boosting, lm=lm)
+        return B200RnntModel(Engine(cfg, sd, str(device), alsd=decoding in ("alsd", "maes")), tokenizer, max_batch=max_batch, decoding=decoding,
+                             beam_size=beam_size, confidence=confidence, boosting=boosting, lm=lm, maes=maes)
     if decoding != "greedy":
         raise ValueError("the one-process multi-GPU model decodes greedily; load one model per device for beam search")
     names = [d if isinstance(d, str) else f"cuda:{int(d)}" for d in devices]
@@ -692,12 +726,14 @@ def transcribe_nbest_batch(model, audios: Sequence[AudioData], n_best: int, conf
     what ``transcribe_batch`` returns.  The audio is prepared as ``transcribe`` prepares it, and every result comes from the
     unchanged ``decode_hypothesis``.  ``result.hypothesis`` always carries the candidate: score = its beam score and, with
     ``log_likelihood=True``, log_likelihood = log P(tokens | audio) from forced alignment (alignment.py), the usual score
-    for rescoring the list.  Needs a single-GPU model loaded with ``decoding="alsd"``; that, or ``n_best`` outside
-    1..64, raises ValueError before the GPU is touched."""
-    if getattr(model, "decoding", "greedy") != "alsd" or not hasattr(model, "transcribe_alsd_nbest"):
-        raise ValueError("N-best lists come from ALSD beam search on one GPU: use load_model(decoding=\"alsd\") without devices=")
+    for rescoring the list.  Needs a single-GPU model loaded with ``decoding="alsd"`` or ``"maes"``; that, or ``n_best``
+    outside 1..64 (MAES: 1..beam_size), raises ValueError before the GPU is touched."""
+    if getattr(model, "decoding", "greedy") not in ("alsd", "maes") or not hasattr(model, "transcribe_alsd_nbest"):
+        raise ValueError("N-best lists come from beam search on one GPU: use load_model(decoding=\"alsd\" or \"maes\") without devices=")
     if isinstance(n_best, bool) or not isinstance(n_best, (int, np.integer)) or not 1 <= int(n_best) <= MAX_NBEST:
         raise ValueError(f"n_best must be an integer in 1..{MAX_NBEST}, got {n_best!r}")
+    if model.decoding == "maes" and int(n_best) > model.beam_size:
+        raise ValueError(f"MAES keeps beam_size = {model.beam_size} hypotheses: n_best must be in 1..{model.beam_size}, got {n_best!r}")
     waves = [_prepare(a) for a in audios]
     out: List[List[TranscribeResult]] = []
     for hyps in model.transcribe_alsd_nbest(waves, int(n_best), log_likelihood=log_likelihood):
