@@ -383,6 +383,31 @@ int rs_rnnt_align_segment(rs_engine* e, const float* enc_dev, const int32_t* enc
                           int32_t* frames_dev, float* token_lp_dev, float* frame_lp_dev, float* viterbi_dev,
                           float* loglik_dev, void* stream);
 
+/* Keyword spotting (semantics: reazonspeech_b200/keywords.py): every occurrence of each of n_kw keywords in each of n_rec
+ * recordings, found on the lattice of every pair p = r * n_kw + k (the lattice of rs_rnnt_align; joint.enc runs once per
+ * recording and the predictor once per keyword).  enc f32[n_rec,T_max,d_model] + enc_len i32[n_rec], labels
+ * i32[n_kw,U_max] + label_len i32[n_kw] (device) -> for each pair, in pick order (largest mean per-frame log-probability
+ * first): span i32[pairs,max_hits,2] (s, e: the hit's first and last frame), score f32[pairs,max_hits] (E(e), the best
+ * segment path ending at e), confidence f32[pairs,max_hits] (m(e) = E(e) / (e - s + 1)), frames i32[pairs,max_hits,U_max]
+ * and token_lp f32[pairs,max_hits,U_max] (each token's frame and lp_emit on that path; -1 and NaN at u >= label_len),
+ * count i32[pairs] (hits written; the entries beyond it are untouched).  The candidates are the end frames with
+ * m(e) >= threshold.  Optional E f32[pairs,T_max] / S i32[pairs,T_max] (NULL: not written) receive E(e) and S(e), the frame of
+ * token 1 on that path (NaN and -1 at e >= enc_len).  A keyword with label_len outside [1, U_max] or a label outside
+ * [0, vocab_size), and a recording with enc_len outside [0, T_max], give count 0; the other pairs are unaffected.  Bad host
+ * arguments are rejected before any launch: U_max outside [1, 32], max_hits outside [1, 256], n_rec, T_max or n_kw < 1, a
+ * NaN or +inf threshold (-inf admits every end frame).  Scratch: 9 bytes per cell of pairs x T_max x (U_max + 1), 8 per
+ * frame of E / S when not given, and rs_rnnt_align's per-recording and per-keyword rows, engine-owned and grown on demand as
+ * rs_rnnt_align's (RS_ERR_WORKSPACE when that allocation fails; callers cut the keywords into groups). */
+int rs_rnnt_spot(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int n_rec, int T_max,
+                 const int32_t* labels_dev, const int32_t* label_len_dev, int n_kw, int U_max, float threshold,
+                 int max_hits, int32_t* span_dev, float* score_dev, float* confidence_dev, int32_t* frames_dev,
+                 float* token_lp_dev, int32_t* count_dev, float* E_dev, int32_t* S_dev, void* stream);
+/* Test seam: the pairs' lattice alone -> lp_blank / lp_emit f32[pairs, T_max, U_max + 1], as rs_rnnt_align_lattice writes
+ * it for recording r's encoder output and keyword k's labels (cells outside a pair untouched). */
+int rs_rnnt_spot_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int n_rec, int T_max,
+                         const int32_t* labels_dev, const int32_t* label_len_dev, int n_kw, int U_max,
+                         float* lp_blank_dev, float* lp_emit_dev, void* stream);
+
 /* norm_audio on the device (pkg/nemo-asr/src/audio.py:54-68: resample to 16 kHz, then average the channels) fused with
  * transcribe()'s padding (audio.py:70-83): in [B, channels, L_in_max] f32 or int16 PCM at the native rate ->
  * out f32 [B, L_out_row], row b = pad zeros | resampled mono utterance | zeros, len_out[b] = resampled length + 2 pad;

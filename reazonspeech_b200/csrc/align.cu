@@ -134,14 +134,18 @@ __global__ void __launch_bounds__(256) align_pred_proj_kernel(const AlignArgs a)
   }
 }
 
+// kPairs: the lattice of every (recording, keyword) pair p = r * B + k (keyword spotting, keywords.py): the encoder rows and
+// enc_len of recording r, the predictor rows, labels and label_len of keyword k, the cells of pair p.  Otherwise r = k = p.
+template <bool kPairs>
 __global__ void __launch_bounds__(kLatThreads, 1)
 rnnt_lattice_kernel(const __grid_constant__ CUtensorMap tm_w, const AlignArgs a) {
   extern __shared__ __align__(16) uint8_t ssm[];
   const int Hj = a.Hj, NC = a.V + 1, LDS = Hj + 8;
   const int tiles_t = (a.T_max + kTileT - 1) / kTileT, tiles_u = (a.U_max + 1 + kTileU - 1) / kTileU;
-  const int b = blockIdx.x / (tiles_t * tiles_u), rem = blockIdx.x % (tiles_t * tiles_u);
+  const int p = blockIdx.x / (tiles_t * tiles_u), rem = blockIdx.x % (tiles_t * tiles_u);
+  const int b = kPairs ? p % a.B : p, r = kPairs ? p / a.B : p;
   const int t0 = (rem / tiles_u) * kTileT, u0 = (rem % tiles_u) * kTileU;
-  const int Tb = min(max(a.enc_len[b], 0), a.T_max), Ub = utt_labels(a, b);
+  const int Tb = min(max(a.enc_len[r], 0), a.T_max), Ub = utt_labels(a, b);
   if (t0 >= Tb || u0 > Ub || a.label_len[b] < 0 || a.label_len[b] > a.U_max) return;   // no valid cell: nothing to write
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, tq = lane & 3, wg = warp >> 2;
@@ -170,15 +174,15 @@ rnnt_lattice_kernel(const __grid_constant__ CUtensorMap tm_w, const AlignArgs a)
   }
   // source rows (rows outside the utterance are zero; their cells are never written)
   for (int i = tid; i < (kTileT + kTileU) * (Hj / 4); i += kLatThreads) {
-    const int r = i / (Hj / 4), c4 = i % (Hj / 4);
+    const int i_r = i / (Hj / 4), c4 = i % (Hj / 4);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (r < kTileT) {
-      if (t0 + r < Tb) v = reinterpret_cast<const float4*>(a.enc_proj + (static_cast<size_t>(b) * a.T_max + t0 + r) * Hj)[c4];
-      *reinterpret_cast<float4*>(s_enc + r * LDS + 4 * c4) = v;
+    if (i_r < kTileT) {
+      if (t0 + i_r < Tb) v = reinterpret_cast<const float4*>(a.enc_proj + (static_cast<size_t>(r) * a.T_max + t0 + i_r) * Hj)[c4];
+      *reinterpret_cast<float4*>(s_enc + i_r * LDS + 4 * c4) = v;
     } else {
-      const int u = u0 + r - kTileT;
+      const int u = u0 + i_r - kTileT;
       if (u <= Ub) v = reinterpret_cast<const float4*>(a.pred_proj + (static_cast<size_t>(b) * (a.U_max + 1) + u) * Hj)[c4];
-      *reinterpret_cast<float4*>(s_pred + (r - kTileT) * LDS + 4 * c4) = v;
+      *reinterpret_cast<float4*>(s_pred + (i_r - kTileT) * LDS + 4 * c4) = v;
     }
   }
   for (int i = tid; i < n_tiles * kBN; i += kLatThreads) s_bias[i] = i < NC ? a.b_out[i] : -INFINITY;
@@ -280,7 +284,7 @@ rnnt_lattice_kernel(const __grid_constant__ CUtensorMap tm_w, const AlignArgs a)
     const int t = t0 + (h == 0 ? tA : tB), u = u0 + g;
     if (tq == 0 && t < Tb && u <= Ub) {
       const float lse = m[h] + logf(s);
-      const size_t cell = (static_cast<size_t>(b) * a.T_max + t) * (a.U_max + 1) + u;
+      const size_t cell = (static_cast<size_t>(p) * a.T_max + t) * (a.U_max + 1) + u;
       a.lp_blank[cell] = vb - lse;
       a.lp_emit[cell] = u < Ub ? ve - lse : -INFINITY;
     }
@@ -492,19 +496,26 @@ cudaError_t launch_align_pred_proj(const AlignArgs& a, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* err) {
+template <bool kPairs>
+static cudaError_t launch_lattice(const AlignArgs& a, int pairs, cudaStream_t stream, char* err) {
   CUtensorMap tm;
   if (!make_tmap_bf16(&tm, a.w_out, static_cast<uint64_t>(a.V) + 1, a.Hj, a.Hj, kBN, err)) return cudaErrorInvalidValue;
   const size_t smem = lattice_smem(a.Hj, a.V);
   static DeviceOnce attr_once;
   if (attr_once.pending()) {
-    const cudaError_t e = cudaFuncSetAttribute(rnnt_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    const cudaError_t e = cudaFuncSetAttribute(rnnt_lattice_kernel<kPairs>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     attr_once.set();
   }
   const int tiles = ((a.T_max + kTileT - 1) / kTileT) * ((a.U_max + 1 + kTileU - 1) / kTileU);
-  rnnt_lattice_kernel<<<a.B * tiles, kLatThreads, smem, stream>>>(tm, a);
+  rnnt_lattice_kernel<kPairs><<<pairs * tiles, kLatThreads, smem, stream>>>(tm, a);
   return cudaGetLastError();
+}
+
+cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* err) { return launch_lattice<false>(a, a.B, stream, err); }
+
+cudaError_t launch_rnnt_lattice_pairs(const AlignArgs& a, int n_rec, cudaStream_t stream, char* err) {
+  return launch_lattice<true>(a, n_rec * a.B, stream, err);
 }
 
 cudaError_t launch_rnnt_segment_dp(const AlignArgs& a, cudaStream_t stream) {

@@ -1112,6 +1112,20 @@ int rs_maes_last_rows(const rs_engine* e, int64_t* rows, int64_t* frames) {
 
 namespace {
 
+// The forced alignment's scratch holds at least `bytes` (growing it synchronises s).
+int grow_align_ws(rs_engine* e, const char* fn, size_t bytes, cudaStream_t s) {
+  if (bytes > e->align_ws_bytes) {
+    RS_CUDA(e, cudaStreamSynchronize(s));
+    cudaFree(e->align_ws); e->align_ws = nullptr; e->align_ws_bytes = 0;
+    if (cudaMalloc(&e->align_ws, bytes) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(e, RS_ERR_WORKSPACE, "%s: cannot allocate %zu bytes of alignment scratch (chunk long inputs)", fn, bytes);
+    }
+    e->align_ws_bytes = bytes;
+  }
+  return RS_OK;
+}
+
 // Forced alignment (align.cu; semantics: reazonspeech_b200/alignment.py).  lp_blank / lp_emit set: the lattice seam (the
 // caller's buffers, no DP); otherwise the lattice lives in the scratch and the DP writes frames / token_lp / viterbi / loglik.
 // seg set: the segment alignment (rnnt_segment_dp_kernel), which also writes seg and frame_lp.
@@ -1135,15 +1149,7 @@ int rnnt_align(rs_engine* e, const char* fn, const float* enc, const int32_t* en
   const size_t o_pp = a.take(static_cast<size_t>(B) * U1 * Hj * 4);
   size_t o_lpb = 0, o_lpe = 0, o_ch = 0;
   if (!seam) { o_lpb = a.take(cells * 4); o_lpe = a.take(cells * 4); o_ch = a.take(cells); }
-  if (a.off > e->align_ws_bytes) {
-    RS_CUDA(e, cudaStreamSynchronize(s));
-    cudaFree(e->align_ws); e->align_ws = nullptr; e->align_ws_bytes = 0;
-    if (cudaMalloc(&e->align_ws, a.off) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(e, RS_ERR_WORKSPACE, "%s: cannot allocate %zu bytes of alignment scratch (chunk long inputs)", fn, a.off);
-    }
-    e->align_ws_bytes = a.off;
-  }
+  RS_TRY(grow_align_ws(e, fn, a.off, s));
   char* ws = static_cast<char*>(e->align_ws);
   rs::AlignArgs g{reinterpret_cast<float*>(ws + o_encp), enc_len, labels, label_len, e->dec.out_w, e->dec.out_b, e->dec.lstm_w,
                   e->dec.gate_tab, e->dec.pred_w, e->dec.pred_b, B, T_max, U_max, Hj, Hp, c.vocab_size,
@@ -1165,9 +1171,92 @@ int rnnt_align(rs_engine* e, const char* fn, const float* enc, const int32_t* en
   return RS_OK;
 }
 
+// Keyword spotting (align.cu, spot.cu; semantics: reazonspeech_b200/keywords.py): joint.enc once per recording, the
+// predictor once per keyword, then the lattice, the recursion and the hits of every (recording, keyword) pair.
+int rnnt_spot(rs_engine* e, const float* enc, const int32_t* enc_len, int n_rec, int T_max, const int32_t* labels,
+              const int32_t* label_len, int n_kw, int U_max, float threshold, int max_hits, int32_t* span, float* score, float* conf,
+              int32_t* frames, float* token_lp, int32_t* count, float* E_out, int32_t* S_out, cudaStream_t s,
+              float* lp_blank = nullptr, float* lp_emit = nullptr) {
+  const bool seam = lp_blank != nullptr;
+  const char* fn = seam ? "rs_rnnt_spot_lattice" : "rs_rnnt_spot";
+  if (!e || !enc || !enc_len || !labels || !label_len ||
+      (seam ? lp_emit == nullptr : (!span || !score || !conf || !frames || !token_lp || !count)))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  if (n_rec < 1 || T_max < 1 || n_kw < 1 || U_max < 1 || U_max > rs::kSpotMaxLabels)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: n_rec=%d, T_max=%d, n_kw=%d must be >= 1 and U_max=%d in [1, %d]", fn, n_rec, T_max, n_kw, U_max,
+                rs::kSpotMaxLabels);
+  if (max_hits < 1 || max_hits > rs::kSpotMaxHits)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: max_hits=%d outside [1, %d]", fn, max_hits, rs::kSpotMaxHits);
+  if (std::isnan(threshold) || threshold == INFINITY)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: threshold must be finite or -inf", fn);
+  const rs_model_config& c = e->cfg;
+  const int U1 = U_max + 1, Hj = c.joint_hidden, Hp = c.pred_hidden;
+  const int64_t pairs = static_cast<int64_t>(n_rec) * n_kw;
+  const int64_t tiles = ((T_max + 15) / 16) * static_cast<int64_t>((U1 + 7) / 8);
+  if (pairs * tiles > INT32_MAX || static_cast<int64_t>(n_rec) * T_max > INT32_MAX)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: %lld pairs of %d frames exceed one launch (fewer keywords per call)", fn, static_cast<long long>(pairs), T_max);
+  char msg[256] = "";
+  if (!rs::align_supported(Hj, Hp, c.vocab_size, U_max, msg)) return fail(e, RS_ERR_UNSUPPORTED, "%s: %s", fn, msg);
+  if (!rs::spot_pick_fits(T_max, max_hits)) return fail(e, RS_ERR_UNSUPPORTED, "%s: T_max=%d exceeds the pick kernel's shared memory", fn, T_max);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  Nvtx range("rs::rnnt_spot");
+  const size_t M = static_cast<size_t>(n_rec) * T_max, cells = static_cast<size_t>(pairs) * T_max * U1;
+  rs::Arena a;
+  const size_t o_xn = a.take(M * c.d_model * 2), o_encp = a.take(M * Hj * 4);
+  const size_t o_h = a.take(static_cast<size_t>(n_kw) * U1 * Hp * 4), o_c = a.take(static_cast<size_t>(n_kw) * Hp * 4);
+  const size_t o_pp = a.take(static_cast<size_t>(n_kw) * U1 * Hj * 4);
+  size_t o_lpb = 0, o_lpe = 0, o_ch = 0, o_E = 0, o_S = 0;
+  if (!seam) {
+    o_lpb = a.take(cells * 4); o_lpe = a.take(cells * 4); o_ch = a.take(cells);
+    if (!E_out) o_E = a.take(static_cast<size_t>(pairs) * T_max * 4);
+    if (!S_out) o_S = a.take(static_cast<size_t>(pairs) * T_max * 4);
+  }
+  RS_TRY(grow_align_ws(e, fn, a.off, s));
+  char* ws = static_cast<char*>(e->align_ws);
+  rs::AlignArgs g{};
+  g.enc_proj = reinterpret_cast<float*>(ws + o_encp); g.enc_len = enc_len; g.labels = labels; g.label_len = label_len;
+  g.w_out = e->dec.out_w; g.b_out = e->dec.out_b; g.w_lstm = e->dec.lstm_w; g.gate_tab = e->dec.gate_tab;
+  g.w_pred = e->dec.pred_w; g.b_pred = e->dec.pred_b;
+  g.B = n_kw; g.T_max = T_max; g.U_max = U_max; g.Hj = Hj; g.Hp = Hp; g.V = c.vocab_size;
+  g.h = reinterpret_cast<float*>(ws + o_h); g.c = reinterpret_cast<float*>(ws + o_c); g.pred_proj = reinterpret_cast<float*>(ws + o_pp);
+  g.lp_blank = seam ? lp_blank : reinterpret_cast<float*>(ws + o_lpb); g.lp_emit = seam ? lp_emit : reinterpret_cast<float*>(ws + o_lpe);
+  g.choice = reinterpret_cast<uint8_t*>(ws + o_ch);
+  const rs::SpotArgs sp{n_rec, threshold, max_hits, E_out ? E_out : reinterpret_cast<float*>(ws + o_E),
+                        S_out ? S_out : reinterpret_cast<int32_t*>(ws + o_S), span, score, conf, frames, token_lp, count};
+  // joint.enc over every frame of every recording, as in the forced alignment
+  RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, ws + o_xn, static_cast<int64_t>(M) * c.d_model, s));
+  RS_TRY(gemm(e, {ws + o_xn, e->dec.enc_w, e->dec.enc_b, nullptr, ws + o_encp, static_cast<int>(M), Hj, c.d_model, RS_EPI_BIAS_F32, 1.f}, s));
+  for (int u = 0; u <= U_max; ++u) RS_LAUNCH(e, s, 1, rs::launch_align_lstm_step(g, u, s));
+  RS_LAUNCH(e, s, 1, rs::launch_align_pred_proj(g, s));
+  {
+    const int r = launch(e, s, "rnnt_lattice_kernel<pairs>", 1, 0.0, [&] { return rs::launch_rnnt_lattice_pairs(g, n_rec, s, msg); });
+    if (r != RS_OK && msg[0] != '\0') return fail(e, r, "%s: %s", fn, msg);
+    RS_TRY(r);
+  }
+  if (seam) return RS_OK;
+  RS_LAUNCH(e, s, 1, rs::launch_rnnt_spot_dp(g, sp, s));
+  RS_LAUNCH(e, s, 1, rs::launch_rnnt_spot_pick(g, sp, s));
+  return RS_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int rs_rnnt_spot(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int n_rec, int T_max, const int32_t* labels_dev,
+                 const int32_t* label_len_dev, int n_kw, int U_max, float threshold, int max_hits, int32_t* span_dev, float* score_dev,
+                 float* confidence_dev, int32_t* frames_dev, float* token_lp_dev, int32_t* count_dev, float* E_dev, int32_t* S_dev,
+                 void* stream) {
+  return rnnt_spot(e, enc_dev, enc_len_dev, n_rec, T_max, labels_dev, label_len_dev, n_kw, U_max, threshold, max_hits, span_dev, score_dev,
+                   confidence_dev, frames_dev, token_lp_dev, count_dev, E_dev, S_dev, static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_spot_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int n_rec, int T_max, const int32_t* labels_dev,
+                         const int32_t* label_len_dev, int n_kw, int U_max, float* lp_blank_dev, float* lp_emit_dev, void* stream) {
+  if (lp_blank_dev == nullptr || lp_emit_dev == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_spot_lattice: bad arguments");
+  return rnnt_spot(e, enc_dev, enc_len_dev, n_rec, T_max, labels_dev, label_len_dev, n_kw, U_max, -1.f, 1, nullptr, nullptr, nullptr, nullptr,
+                   nullptr, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream), lp_blank_dev, lp_emit_dev);
+}
 
 int rs_rnnt_align(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, const int32_t* labels_dev,
                   const int32_t* label_len_dev, int U_max, int32_t* frames_dev, float* token_lp_dev, float* viterbi_dev,

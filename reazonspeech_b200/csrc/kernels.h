@@ -158,6 +158,26 @@ cudaError_t launch_rnnt_align_dp(const AlignArgs& a, cudaStream_t stream);
 // segment alignment (free start and end) -> seg, frames, token_lp, frame_lp, viterbi, loglik
 cudaError_t launch_rnnt_segment_dp(const AlignArgs& a, cudaStream_t stream);
 
+// Keyword spotting (align.cu, spot.cu; semantics: reazonspeech_b200/keywords.py): the AlignArgs of the B keywords, whose enc_proj
+// and enc_len are the n_rec recordings'; pair p = r * B + k, and the lattice arrays are the pairs'.
+struct SpotArgs {
+  int n_rec;
+  float threshold; int max_hits;
+  float* E; int32_t* S;                       // [pairs][T_max]: E(e), S(e) (NaN, -1 where no segment ends)
+  int32_t* span; float* score; float* conf;   // [pairs][max_hits] (x2: s, e), E(e), m(e)
+  int32_t* frames; float* token_lp;           // [pairs][max_hits][U_max]
+  int32_t* count;                             // [pairs]
+};
+constexpr int kSpotMaxLabels = 32;
+constexpr int kSpotMaxHits = 256;
+// the lattice of every (recording, keyword) pair
+cudaError_t launch_rnnt_lattice_pairs(const AlignArgs& a, int n_rec, cudaStream_t stream, char* err);
+// the free-start recursion of every pair -> E, S and a.choice; then the hits of every pair -> span ... count
+cudaError_t launch_rnnt_spot_dp(const AlignArgs& a, const SpotArgs& sp, cudaStream_t stream);
+cudaError_t launch_rnnt_spot_pick(const AlignArgs& a, const SpotArgs& sp, cudaStream_t stream);
+// shared memory of the pick kernel (false when T_max frames do not fit)
+bool spot_pick_fits(int T_max, int max_hits);
+
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)
 struct ResampleArgs {
   const void* in; bool in_i16;          // [B, C, L_in_max] f32, or int16 PCM (scaled by 2^-15)

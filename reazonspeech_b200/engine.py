@@ -54,7 +54,7 @@ EXPORTS = [
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
     "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots", "rs_rnnt_alsd_nbest", "rs_rnnt_maes", "rs_maes_last_rows",
-    "rs_rnnt_align_segment",
+    "rs_rnnt_align_segment", "rs_rnnt_spot", "rs_rnnt_spot_lattice",
 ]
 
 MAX_NBEST = 64                          # include/rs_engine.h RS_MAX_NBEST
@@ -140,6 +140,10 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_align_lattice.restype = ip
     lib.rs_rnnt_align_segment.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp, vp, vp]
     lib.rs_rnnt_align_segment.restype = ip
+    lib.rs_rnnt_spot.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, ip, C.c_float, ip, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.rs_rnnt_spot.restype = ip
+    lib.rs_rnnt_spot_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, ip, vp, vp, vp]
+    lib.rs_rnnt_spot_lattice.restype = ip
     lib.rs_stream_state_bytes.argtypes = [vp]
     lib.rs_stream_state_bytes.restype = C.c_size_t
     lib.rs_rnnt_greedy_resume.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
@@ -700,6 +704,45 @@ class Engine:
         lp_blank, lp_emit = out
         self._check(self.lib.rs_rnnt_align_lattice(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, labels.data_ptr(), label_len.data_ptr(), U,
                                                    lp_blank.data_ptr(), lp_emit.data_ptr(), self._stream()), "rs_rnnt_align_lattice")
+        return lp_blank, lp_emit
+
+    def spot(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor, threshold: float = -1.0,
+             max_hits: int = 64, scores: bool = False):
+        """Keyword spotting (rs_rnnt_spot; semantics: keywords.py): every hit of each keyword labels[k, :label_len[k]] in each
+        recording enc[r, :enc_len[r]], pair p = r * n_kw + k -> (span i32 [P, H, 2], score f32 [P, H], confidence f32 [P, H],
+        frames i32 [P, H, U], token_lp f32 [P, H, U], count i32 [P]) device tensors, H = max_hits, hits in pick order; with
+        ``scores`` also E f32 [P, T] and S i32 [P, T], the best segment ending at every frame."""
+        R, T, _ = enc.shape
+        assert enc.dtype == torch.float32 and enc.is_contiguous() and enc_len.dtype == torch.int32
+        assert labels.dtype == torch.int32 and labels.dim() == 2 and label_len.dtype == torch.int32
+        labels = labels.contiguous()
+        K, U = labels.shape
+        P, H, dev = R * K, int(max_hits), self.device
+        span = torch.empty(P, H, 2, dtype=torch.int32, device=dev)
+        score = torch.empty(P, H, dtype=torch.float32, device=dev)
+        conf = torch.empty(P, H, dtype=torch.float32, device=dev)
+        frames = torch.empty(P, H, U, dtype=torch.int32, device=dev)
+        token_lp = torch.empty(P, H, U, dtype=torch.float32, device=dev)
+        count = torch.empty(P, dtype=torch.int32, device=dev)
+        E = torch.empty(P, T, dtype=torch.float32, device=dev) if scores else None
+        S = torch.empty(P, T, dtype=torch.int32, device=dev) if scores else None
+        self._check(self.lib.rs_rnnt_spot(self.h, enc.data_ptr(), enc_len.data_ptr(), R, T, labels.data_ptr(), label_len.data_ptr(), K, U,
+                                          float(threshold), H, span.data_ptr(), score.data_ptr(), conf.data_ptr(), frames.data_ptr(),
+                                          token_lp.data_ptr(), count.data_ptr(), E.data_ptr() if scores else None,
+                                          S.data_ptr() if scores else None, self._stream()), "rs_rnnt_spot")
+        out = (span, score, conf, frames, token_lp, count)
+        return out + (E, S) if scores else out
+
+    def spot_lattice(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor):
+        """The pairs' lattice alone (rs_rnnt_spot_lattice) -> (lp_blank, lp_emit) f32 [R * K, T, U + 1], pair p = r * K + k;
+        cells outside a pair are NaN."""
+        R, T, _ = enc.shape
+        K, U = labels.shape
+        lp_blank = torch.full((R * K, T, U + 1), float("nan"), device=self.device)
+        lp_emit = torch.full((R * K, T, U + 1), float("nan"), device=self.device)
+        self._check(self.lib.rs_rnnt_spot_lattice(self.h, enc.data_ptr(), enc_len.data_ptr(), R, T, labels.contiguous().data_ptr(),
+                                                  label_len.data_ptr(), K, U, lp_blank.data_ptr(), lp_emit.data_ptr(), self._stream()),
+                    "rs_rnnt_spot_lattice")
         return lp_blank, lp_emit
 
     def resample_mono(self, raw: torch.Tensor, lens: torch.Tensor, samplerate: int, pad: int = 0):

@@ -43,6 +43,14 @@ Seventh extension, beam search: the decoding strategy of the transcription
                        maes as into greedy; alsd takes no LM, no phrases; neither beam search streams
   --beam=N             beam size of alsd / maes (default 4; maes: 1..8)
 Without the options the output is unchanged.
+Eighth extension, keyword spotting (reazonspeech_b200/keywords.py): instead of transcribing, every occurrence of each keyword is
+searched in each AUDIO on the RNN-T lattice, and the hits are written as segments (text = the keyword, sorted by start)
+through the same writer with the same time offsets
+  --keywords=FILE      UTF-8 text, one keyword per line (blank lines ignored)
+  --keyword-threshold=X  the least mean per-frame log-probability of a hit (default -1.0; not calibrated, see keywords.py)
+  --max-hits=N         at most N hits per keyword per AUDIO, 1..256 (default 64)
+It goes with none of --text, --captions, --stream, --decoding, --beam, --phrases, --phrase-score and --lm.  Without it the
+output is unchanged.
 Audio decoding: soundfile when installed, scipy for WAV, librosa for compressed containers, see audio.audio_from_path.
 """
 import dataclasses
@@ -54,7 +62,7 @@ from typing import List, Optional
 
 SHORT_OPTS = "ho:"
 LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=", "stream", "chunk=", "left=", "right=",
-             "captions=", "before=", "after=", "decoding=", "beam=")
+             "captions=", "before=", "after=", "decoding=", "beam=", "keywords=", "keyword-threshold=", "max-hits=")
 
 
 @dataclass
@@ -77,6 +85,9 @@ class Options:
     after: float = 0.0
     decoding: str = "greedy"
     beam: Optional[int] = None
+    keywords: Optional[str] = None
+    keyword_threshold: Optional[float] = None
+    max_hits: Optional[int] = None
 
 
 def parse(argv) -> Options:
@@ -110,6 +121,12 @@ def parse(argv) -> Options:
             opt.decoding = value
         if flag == "--beam":
             opt.beam = int(value)
+        if flag == "--keywords":
+            opt.keywords = value
+        if flag == "--keyword-threshold":
+            opt.keyword_threshold = float(value)
+        if flag == "--max-hits":
+            opt.max_hits = int(value)
     if (opt.lm is None) != (opt.lm_alpha is None):
         raise ValueError("--lm and --lm-alpha go together: the LM weight has no default (try values around 0.3-0.5 and tune "
                          "on held-out audio)" if opt.lm is not None else "--lm-alpha needs an LM: --lm=FILE")
@@ -133,6 +150,15 @@ def parse(argv) -> Options:
             raise ValueError("--captions goes with neither --stream nor --text")
         if opt.before < 0 or opt.after < 0:
             raise ValueError(f"--before and --after are margins in seconds >= 0, got {opt.before} and {opt.after}")
+    if opt.keywords is None:
+        if opt.keyword_threshold is not None or opt.max_hits is not None:
+            raise ValueError("--keyword-threshold and --max-hits set the search of --keywords=FILE")
+    else:
+        clash = [f for f, _ in parsed if f in ("--text", "--captions", "--stream", "--decoding", "--beam", "--phrases", "--phrase-score", "--lm")]
+        if clash:
+            raise ValueError(f"--keywords searches the audio on the lattice: it goes with none of {', '.join(sorted(set(clash)))}")
+        from ...keywords import MAX_HITS, THRESHOLD, check_search
+        check_search(THRESHOLD if opt.keyword_threshold is None else opt.keyword_threshold, MAX_HITS if opt.max_hits is None else opt.max_hits)
     return opt
 
 
@@ -179,7 +205,9 @@ def run(opt: Options) -> None:
         if opt.beam is not None:
             extra["beam_size"] = opt.beam
     model = load_model(**extra)
-    if captions is not None:
+    if opt.keywords is not None:
+        results = keyword_segments(model, clips, load_keywords(opt.keywords), opt)
+    elif captions is not None:
         results = [caption_segments(model, clips[0], captions, opt)]
     elif opt.stream:
         results = [stream(model, opt, clips[0] if clips else None)]
@@ -205,6 +233,27 @@ def caption_segments(model, clip, captions, opt: Options):
     found = [a for a in align_captions(model, clip, captions, before=opt.before, after=opt.after) if a is not None]
     return TranscribeResult("".join(a.text for a in found), [w for a in found for w in a.subwords],
                             [Segment(a.start_seconds, a.end_seconds, a.text) for a in found])
+
+
+def load_keywords(path: str) -> List[str]:
+    """--keywords: one UTF-8 keyword per line, blank lines skipped."""
+    with open(path, encoding="utf-8") as f:
+        return [line.strip() for line in f.read().splitlines() if line.strip()]
+
+
+def keyword_segments(model, clips, keywords: List[str], opt: Options):
+    """--keywords: for each clip one result whose segments are (start, end, keyword) of every hit, sorted by start."""
+    from .interface import Segment, TranscribeResult
+    from .transcribe import find_keywords_batch
+    from ...keywords import MAX_HITS, THRESHOLD
+    found = find_keywords_batch(model, clips, keywords, threshold=THRESHOLD if opt.keyword_threshold is None else opt.keyword_threshold,
+                                max_hits=MAX_HITS if opt.max_hits is None else opt.max_hits)
+    results = []
+    for lists in found:
+        hits = sorted((h for row in lists for h in row), key=lambda h: (h.start_seconds, h.end_seconds))
+        results.append(TranscribeResult("".join(h.keyword for h in hits), [w for h in hits for w in h.subwords],
+                                        [Segment(h.start_seconds, h.end_seconds, h.keyword) for h in hits]))
+    return results
 
 
 def stream(model, opt: Options, clip=None):

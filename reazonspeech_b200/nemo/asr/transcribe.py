@@ -23,6 +23,8 @@ import torch
 
 from ...alignment import alignment_hypothesis, pack_labels, validate_labels
 from ...captions import AFTER_SECONDS, BEFORE_SECONDS, CONFIDENCE_FRAMES, AlignedCaption, Caption, caption_window
+from ...keywords import MAX_HITS as KW_MAX_HITS, SCRATCH_CAP_BYTES, THRESHOLD as KW_THRESHOLD, KeywordHit, check_search, \
+    hit_seconds, keyword_groups, keyword_ids
 from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables, combine_tables, config_key
 from ...config import MaesConfig, ModelConfig
 from ...confidence import ConfidenceConfig, measure, word_confidence
@@ -399,6 +401,40 @@ class B200RnntModel:
         for idx, items in self.iter_align_segment_batches(waveforms, token_lists, pad):
             for i, item in zip(idx, items):
                 results[i] = item
+        return results
+
+    # -- keyword spotting (keywords.py)
+    def spot_tokens(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0, *,
+                    threshold: float = KW_THRESHOLD, max_hits: int = KW_MAX_HITS, cap: int = SCRATCH_CAP_BYTES):
+        """16 kHz mono waveforms (``pad`` zero samples on both sides) and keyword token-id lists -> for each waveform, for each
+        keyword, its hits in pick order: (s, e, score, confidence, frames, token_lp).  Recordings are sorted by length and
+        encoded whole in batches of at most ``max_batch``; keywords are sorted by length and cut into groups whose lattice
+        scratch stays under ``cap`` bytes (keywords.keyword_groups), one rs_rnnt_spot call per group.  Any ``decoding`` works."""
+        token_lists = keyword_ids(token_lists, self.cfg.vocab_size)
+        check_search(threshold, max_hits)
+        eng = self.engine
+        results = [[[] for _ in token_lists] for _ in waveforms]
+        if not token_lists:
+            return results
+        order = sorted(range(len(waveforms)), key=lambda i: len(waveforms[i]))
+        for lo in range(0, len(order), self.max_batch):
+            idx = order[lo:lo + self.max_batch]
+            wav, lens = self._staging[0].stage([waveforms[i] for i in idx], pad)
+            with torch.cuda.device(eng.device):
+                x = wav.to(eng.device, non_blocking=True)
+                if x.dtype == torch.int16:
+                    x = x.to(torch.float32) * (1.0 / 32768.0)
+                enc, enc_len = eng.encode(*eng.log_mel(x, lens.to(eng.device)))
+                for group in keyword_groups([len(t) for t in token_lists], len(idx), enc.shape[1], cap):
+                    labels, label_len = pack_labels([token_lists[k] for k in group])
+                    span, score, conf, frames, token_lp, count = [
+                        a.cpu() for a in eng.spot(enc, enc_len, torch.from_numpy(labels).to(eng.device),
+                                                  torch.from_numpy(label_len).to(eng.device), threshold, max_hits)]
+                    for r, i in enumerate(idx):
+                        for j, k in enumerate(group):
+                            p, n = r * len(group) + j, int(label_len[j])
+                            results[i][k] = [(int(span[p, h, 0]), int(span[p, h, 1]), float(score[p, h]), float(conf[p, h]),
+                                              frames[p, h, :n].tolist(), token_lp[p, h, :n].tolist()) for h in range(int(count[p]))]
         return results
 
     # -- NeMo's call shape (transcribe.py:48-53): already padded tensors
@@ -828,3 +864,39 @@ def align_captions(model, audio: AudioData, captions: Sequence[Caption], *, befo
             a.asr = r.text
             a.cer = calculate_cer(a.text, r.text)["cer"] if normalize(a.text) else math.nan
     return out
+
+
+def find_keywords_batch(model, audios: Sequence[AudioData], keywords: Sequence, *, threshold: float = KW_THRESHOLD,
+                        max_hits: int = KW_MAX_HITS) -> List[List[List[KeywordHit]]]:
+    """Every occurrence of each keyword in each audio (keywords.py): for each audio, one list of ``KeywordHit`` per keyword,
+    in time order.  A keyword is text (tokenised as phrase boosting tokenises a phrase) or a sequence of token ids.  The audio
+    is prepared as ``transcribe`` prepares it and encoded whole, and the hits are found on the RNN-T lattice of every (audio,
+    keyword) pair on the GPU: the candidates are the end frames whose best segment scores at least ``threshold`` per frame
+    (NOT calibrated, see keywords.py), at most ``max_hits`` (1..256) per keyword per audio.  The decoder is not involved, so
+    any ``decoding`` works.  A model without ``spot_tokens`` (several GPUs, or a NeMo model), a bad keyword (empty, an id
+    outside the vocabulary, more than 32 tokens) or a bad threshold / max_hits raises ValueError before the GPU is touched."""
+    if not hasattr(model, "spot_tokens"):
+        raise ValueError("keyword spotting runs on one GPU: use load_model() without devices=")
+    ids = keyword_ids(keywords, model.cfg.vocab_size, model.tokenizer)
+    check_search(threshold, max_hits)
+    waves = [np.asarray(norm_audio(a).waveform) for a in audios]
+    found = model.spot_tokens(waves, ids, pad=int(PAD_SECONDS * SAMPLERATE), threshold=threshold, max_hits=max_hits)
+    out: List[List[List[KeywordHit]]] = []
+    for wave, per_kw in zip(waves, found):
+        duration = len(wave) / SAMPLERATE
+        lists = []
+        for kw, k_ids, hits in zip(keywords, ids, per_kw):
+            row = []
+            for s0, e0, score, conf, frames, token_lp in sorted(hits, key=lambda h: (h[0], h[1])):
+                r = decode_hypothesis(model, alignment_hypothesis(k_ids, frames, token_lp, score, math.nan, model.cfg.blank))
+                start, end = hit_seconds(s0, e0, duration)
+                row.append(KeywordHit(kw, start, end, score, conf, r.subwords))
+            lists.append(row)
+        out.append(lists)
+    return out
+
+
+def find_keywords(model, audio: AudioData, keywords: Sequence, *, threshold: float = KW_THRESHOLD,
+                  max_hits: int = KW_MAX_HITS) -> List[List[KeywordHit]]:
+    """One audio of ``find_keywords_batch``: one list of ``KeywordHit`` per keyword, in time order."""
+    return find_keywords_batch(model, [audio], keywords, threshold=threshold, max_hits=max_hits)[0]
