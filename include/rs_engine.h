@@ -368,6 +368,29 @@ int rs_rnnt_align_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc
                           const int32_t* labels_dev, const int32_t* label_len_dev, int U_max,
                           float* lp_blank_dev, float* lp_emit_dev, void* stream);
 
+/* Banded alignment (semantics: reazonspeech_b200/alignment.py, "Banded alignment"): rs_rnnt_align restricted to the cells
+ * band_lo[b][u] <= t < band_hi[b][u] of each label row u <= label_len[b], for transcripts too long for the full lattice (an
+ * hour of speech).  Inputs and outputs are rs_rnnt_align's, plus the band, HOST int32 [B][U_max + 1] each (rows beyond
+ * label_len[b] are not read), and edge i32[B] (device): the tokens whose emission frame lies on an interior band edge, a hint
+ * that the band cut the path.  A full band (lo = 0, hi = enc_len) gives rs_rnnt_align's results bit for bit.  The lengths and
+ * labels are read back (the call synchronises stream) and checked with the band before any launch: enc_len outside
+ * [1, T_max], label_len outside [0, U_max], a label outside [0, vocab_size), or a band that is empty in a row, leaves
+ * [0, enc_len), decreases, does not start at frame 0 in row 0 or end at enc_len in row label_len, or has two consecutive rows
+ * that do not overlap (lo[u + 1] >= hi[u]) gives RS_ERR_INVALID_ARG.  There is no limit on U_max: the DP keeps two
+ * diagonals of the band, so RS_ERR_UNSUPPORTED only when a diagonal meets more than 14528 rows.  Scratch: 9 bytes per band
+ * cell plus rs_rnnt_align's per-frame and per-row parts, grown on demand as rs_rnnt_align's. */
+int rs_rnnt_align_banded(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max,
+                         const int32_t* labels_dev, const int32_t* label_len_dev, int U_max,
+                         const int32_t* band_lo_host, const int32_t* band_hi_host, int32_t* frames_dev,
+                         float* token_lp_dev, float* viterbi_dev, float* loglik_dev, int32_t* edge_dev, void* stream);
+/* Test seam: the banded lattice alone -> lp_blank / lp_emit f32 in banded storage: row (b, u), u <= label_len[b], holds the
+ * frames [band_lo, band_hi) at off + (t - band_lo), off the prefix sum of the rows' widths in (b, u) order.  Every cell is
+ * rs_rnnt_align_lattice's at the same (t, u), bit for bit. */
+int rs_rnnt_align_banded_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max,
+                                 const int32_t* labels_dev, const int32_t* label_len_dev, int U_max,
+                                 const int32_t* band_lo_host, const int32_t* band_hi_host, float* lp_blank_dev,
+                                 float* lp_emit_dev, void* stream);
+
 /* Segment alignment of given label sequences inside longer windows (semantics: reazonspeech_b200/alignment.py, "Segment
  * alignment"): the same lattice as rs_rnnt_align, but the tokens may start and end at any frame and the frames outside
  * the segment are not charged.  enc f32[B,T_max,d_model] + enc_len, labels i32[B,U_max] + label_len i32[B] (device) ->

@@ -37,7 +37,25 @@ per frame, the final blank at (e, U) included.  frame_lp[t] (t in [s, e]) is the
 to rows [s, e] (alpha[s][0] = 0, ending with the blank at (e, U)): log P(caption | the audio of its segment).  Hence
 loglik >= score >= the full-window Viterbi score of the same lattice.  U = 0, a label outside [0, V) or enc_len outside
 [1, T_max] gives s = e = -1, frames -1 and NaN scores.  On the GPU: rnnt_segment_dp_kernel, one CTA per window, on the
-lattice the forced alignment computes."""
+lattice the forced alignment computes.
+
+Banded alignment (``rs_rnnt_align_banded``; longform.py builds the band for transcripts of long recordings).  The lattice,
+recursions, tie rule, outputs and their meaning are forced alignment's, but only the cells lo[u] <= t < hi[u] exist; every
+other cell is -inf.  The band is given per label row u in [0, U] and must satisfy 0 <= lo[u] < hi[u] <= T, lo and hi
+non-decreasing in u, lo[0] = 0, hi[U] = T, and lo[u + 1] < hi[u]: consecutive rows overlap, and every path's vertical step
+from row u to u + 1 (token u + 1) happens at a frame in [lo[u + 1], hi[u]).  Then every diagonal d = t + u meets the band in
+one contiguous run of rows, every cell but (0, 0) has a predecessor inside the band, and so:
+
+- a full band (lo = 0, hi = T) gives exactly forced alignment's results;
+- a band that contains the full lattice's Viterbi path gives the same Viterbi path and score;
+- for any valid band, viterbi_band <= viterbi_full and loglik_band <= loglik_full.
+
+edge counts the tokens whose emission frame t lies on an interior edge of the band's constraint on that step: token u (the
+step from row u - 1 to row u) with t = lo[u] > 0, or with t = hi[u - 1] - 1 < T - 1.  It signals that the band may have cut
+the path.  It is a heuristic: a path clear of the edges does not prove that the banded path is the global Viterbi path.  On
+the GPU: rnnt_lattice_kernel's banded instance computes the tiles of the full lattice's grid that meet the band (so every
+cell is bit-identical to the full lattice's) into banded storage, and rnnt_band_dp_kernel runs the recursions with shared
+memory bounded by the band's largest diagonal extent instead of U."""
 from __future__ import annotations
 
 from typing import List, Sequence, Tuple

@@ -6,6 +6,7 @@
 //   align_pred_proj_kernel   pred_proj[b][u] = joint.pred(h_u) for all B * (U_max + 1) rows
 //   rnnt_lattice_kernel      log softmax of the joint at every (t, u) cell of every utterance -> lp_blank, lp_emit (wgmma)
 //   rnnt_align_dp_kernel     forward (logaddexp) and Viterbi (max) recursions over the anti-diagonals + backtrace
+//   rnnt_band_dp_kernel      the same on the cells of a band (banded alignment), shared memory bounded by the band's width
 //   rnnt_segment_dp_kernel   the segment alignment of a caption inside its window: Viterbi with a free start and a free end,
 //                            backtrace, then the forward recursion over the segment's frames only
 //
@@ -136,15 +137,19 @@ __global__ void __launch_bounds__(256) align_pred_proj_kernel(const AlignArgs a)
 
 // kPairs: the lattice of every (recording, keyword) pair p = r * B + k (keyword spotting, keywords.py): the encoder rows and
 // enc_len of recording r, the predictor rows, labels and label_len of keyword k, the cells of pair p.  Otherwise r = k = p.
-template <bool kPairs>
+// kBand (banded alignment): CTA i computes tile a.band_tiles[i] = (utterance, t0, u0) of the same 16 x 8 grid, with the same
+// code, so every cell it writes is bit-identical to the full lattice's; only the cells inside the band are written, to
+// banded storage.
+template <bool kPairs, bool kBand = false>
 __global__ void __launch_bounds__(kLatThreads, 1)
 rnnt_lattice_kernel(const __grid_constant__ CUtensorMap tm_w, const AlignArgs a) {
   extern __shared__ __align__(16) uint8_t ssm[];
   const int Hj = a.Hj, NC = a.V + 1, LDS = Hj + 8;
   const int tiles_t = (a.T_max + kTileT - 1) / kTileT, tiles_u = (a.U_max + 1 + kTileU - 1) / kTileU;
-  const int p = blockIdx.x / (tiles_t * tiles_u), rem = blockIdx.x % (tiles_t * tiles_u);
+  const int4 bt = kBand ? a.band_tiles[blockIdx.x] : make_int4(0, 0, 0, 0);
+  const int p = kBand ? bt.x : blockIdx.x / (tiles_t * tiles_u), rem = blockIdx.x % (tiles_t * tiles_u);
   const int b = kPairs ? p % a.B : p, r = kPairs ? p / a.B : p;
-  const int t0 = (rem / tiles_u) * kTileT, u0 = (rem % tiles_u) * kTileU;
+  const int t0 = kBand ? bt.y : (rem / tiles_u) * kTileT, u0 = kBand ? bt.z : (rem % tiles_u) * kTileU;
   const int Tb = min(max(a.enc_len[r], 0), a.T_max), Ub = utt_labels(a, b);
   if (t0 >= Tb || u0 > Ub || a.label_len[b] < 0 || a.label_len[b] > a.U_max) return;   // no valid cell: nothing to write
 
@@ -284,9 +289,18 @@ rnnt_lattice_kernel(const __grid_constant__ CUtensorMap tm_w, const AlignArgs a)
     const int t = t0 + (h == 0 ? tA : tB), u = u0 + g;
     if (tq == 0 && t < Tb && u <= Ub) {
       const float lse = m[h] + logf(s);
-      const size_t cell = (static_cast<size_t>(p) * a.T_max + t) * (a.U_max + 1) + u;
-      a.lp_blank[cell] = vb - lse;
-      a.lp_emit[cell] = u < Ub ? ve - lse : -INFINITY;
+      size_t cell = (static_cast<size_t>(p) * a.T_max + t) * (a.U_max + 1) + u;
+      bool in = true;
+      if constexpr (kBand) {
+        const size_t row = static_cast<size_t>(b) * (a.U_max + 1) + u;
+        const int lo = a.band_lo[row];
+        in = t >= lo && t < a.band_hi[row];
+        cell = a.band_off[row] + (t - lo);
+      }
+      if (in) {
+        a.lp_blank[cell] = vb - lse;
+        a.lp_emit[cell] = u < Ub ? ve - lse : -INFINITY;
+      }
     }
   }
 }
@@ -363,6 +377,73 @@ __global__ void __launch_bounds__(256) rnnt_align_dp_kernel(const AlignArgs a) {
         --t;
       }
     }
+  }
+}
+
+// Banded alignment (alignment.py, "Banded alignment"): rnnt_align_dp_kernel's operations, in its order, on the band's cells
+// only.  Diagonal d meets the band in the rows [u0, u1] (u + lo[u] <= d < u + hi[u]; both ends only move up with d, so every
+// thread advances them in step), and the two live diagonals sit in shared memory at u - u0: band_pitch cells each, the
+// band's largest diagonal extent, whatever U is.  (t - 1, u) is in the band iff u <= u1 of the previous diagonal, (t, u - 1)
+// iff u - 1 >= its u0: with a full band these are t > 0 and u > 0.  The host has validated the band, the lengths and the labels.
+__global__ void __launch_bounds__(256) rnnt_band_dp_kernel(const AlignArgs a) {
+  extern __shared__ __align__(16) float s_dp[];                // [2 diagonals][2 (forward, Viterbi)][band_pitch]
+  const int b = blockIdx.x, tid = threadIdx.x, P = a.band_pitch;
+  const int T = a.enc_len[b], U = a.label_len[b];
+  const size_t r0 = static_cast<size_t>(b) * (a.U_max + 1);
+  const int32_t* lo = a.band_lo + r0;
+  const int32_t* hi = a.band_hi + r0;
+  const int64_t* off = a.band_off + r0;
+  int32_t* frames = a.frames + static_cast<size_t>(b) * a.U_max;
+  float* token_lp = a.token_lp + static_cast<size_t>(b) * a.U_max;
+  for (int i = U + tid; i < a.U_max; i += blockDim.x) { frames[i] = -1; token_lp[i] = NAN; }
+  float* cur = s_dp;
+  float* prev = s_dp + 2 * P;
+  int u0 = 0, u1 = 0, p0 = 0, p1 = -1;                         // rows of diagonals d and d - 1
+  for (int d = 0; d < T + U; ++d) {
+    while (u1 < U && u1 + 1 + lo[u1 + 1] <= d) ++u1;
+    while (u0 + hi[u0] <= d) ++u0;
+    for (int i = tid; i <= u1 - u0; i += blockDim.x) {
+      const int u = u0 + i, t = d - u;
+      float f = 0.f, v = 0.f;
+      uint8_t ch = 0;                                          // 1: the Viterbi predecessor is (t, u - 1), an emission
+      if (d > 0) {
+        float fb = -INFINITY, vb = -INFINITY, fe = -INFINITY, ve = -INFINITY;
+        const bool has_b = u <= p1;
+        if (has_b) {
+          const float l = a.lp_blank[off[u] + (t - 1 - lo[u])];
+          fb = prev[u - p0] + l; vb = prev[P + u - p0] + l;
+        }
+        if (u > p0) {
+          const float l = a.lp_emit[off[u - 1] + (t - lo[u - 1])];
+          fe = prev[u - 1 - p0] + l; ve = prev[P + u - 1 - p0] + l;
+        }
+        f = logaddexp(fb, fe);
+        ch = (!has_b || ve > vb) ? 1 : 0;                      // an exact tie goes to the blank predecessor
+        v = ch ? ve : vb;
+      }
+      a.choice[off[u] + (t - lo[u])] = ch;
+      cur[i] = f; cur[P + i] = v;
+    }
+    __syncthreads();
+    float* x = cur; cur = prev; prev = x;
+    p0 = u0; p1 = u1;
+  }
+  if (tid == 0) {
+    const float l = a.lp_blank[off[U] + (T - 1 - lo[U])];
+    a.loglik[b] = prev[U - p0] + l;
+    a.viterbi[b] = prev[P + U - p0] + l;
+    int t = T - 1, u = U, edge = 0;
+    while (u > 0) {
+      if (a.choice[off[u] + (t - lo[u])]) {
+        frames[u - 1] = t;
+        token_lp[u - 1] = a.lp_emit[off[u - 1] + (t - lo[u - 1])];
+        edge += (t == lo[u] && lo[u] > 0) || (t == hi[u - 1] - 1 && hi[u - 1] < T);
+        --u;
+      } else {
+        --t;
+      }
+    }
+    a.edge[b] = edge;
   }
 }
 
@@ -496,26 +577,46 @@ cudaError_t launch_align_pred_proj(const AlignArgs& a, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-template <bool kPairs>
-static cudaError_t launch_lattice(const AlignArgs& a, int pairs, cudaStream_t stream, char* err) {
+template <bool kPairs, bool kBand>
+static cudaError_t launch_lattice(const AlignArgs& a, int blocks, cudaStream_t stream, char* err) {
   CUtensorMap tm;
   if (!make_tmap_bf16(&tm, a.w_out, static_cast<uint64_t>(a.V) + 1, a.Hj, a.Hj, kBN, err)) return cudaErrorInvalidValue;
   const size_t smem = lattice_smem(a.Hj, a.V);
   static DeviceOnce attr_once;
   if (attr_once.pending()) {
-    const cudaError_t e = cudaFuncSetAttribute(rnnt_lattice_kernel<kPairs>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    const cudaError_t e = cudaFuncSetAttribute(rnnt_lattice_kernel<kPairs, kBand>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     attr_once.set();
   }
-  const int tiles = ((a.T_max + kTileT - 1) / kTileT) * ((a.U_max + 1 + kTileU - 1) / kTileU);
-  rnnt_lattice_kernel<kPairs><<<pairs * tiles, kLatThreads, smem, stream>>>(tm, a);
+  rnnt_lattice_kernel<kPairs, kBand><<<blocks, kLatThreads, smem, stream>>>(tm, a);
   return cudaGetLastError();
 }
 
-cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* err) { return launch_lattice<false>(a, a.B, stream, err); }
+static int lattice_tiles(const AlignArgs& a) { return ((a.T_max + kTileT - 1) / kTileT) * ((a.U_max + 1 + kTileU - 1) / kTileU); }
+
+cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* err) {
+  return launch_lattice<false, false>(a, a.B * lattice_tiles(a), stream, err);
+}
 
 cudaError_t launch_rnnt_lattice_pairs(const AlignArgs& a, int n_rec, cudaStream_t stream, char* err) {
-  return launch_lattice<true>(a, n_rec * a.B, stream, err);
+  return launch_lattice<true, false>(a, n_rec * a.B * lattice_tiles(a), stream, err);
+}
+
+cudaError_t launch_rnnt_lattice_band(const AlignArgs& a, int n_tiles, cudaStream_t stream, char* err) {
+  return launch_lattice<false, true>(a, n_tiles, stream, err);
+}
+
+size_t band_dp_smem(int pitch) { return static_cast<size_t>(4) * pitch * sizeof(float); }
+
+cudaError_t launch_rnnt_band_dp(const AlignArgs& a, cudaStream_t stream) {
+  static DeviceOnce attr_once;
+  if (attr_once.pending()) {
+    const cudaError_t e = cudaFuncSetAttribute(rnnt_band_dp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_once.set();
+  }
+  rnnt_band_dp_kernel<<<a.B, 256, band_dp_smem(a.band_pitch), stream>>>(a);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_rnnt_segment_dp(const AlignArgs& a, cudaStream_t stream) {

@@ -1171,6 +1171,113 @@ int rnnt_align(rs_engine* e, const char* fn, const float* enc, const int32_t* en
   return RS_OK;
 }
 
+// Banded alignment (align.cu; semantics: reazonspeech_b200/alignment.py, "Banded alignment").  The lengths and labels are read
+// back and checked with the host band before anything is launched; the host also lays out the banded storage (row (b, u) at
+// off[b][u], the prefix sum of the band widths), finds every diagonal's extent and lists the lattice tiles that meet the band.
+// lp_blank / lp_emit set: the lattice seam (the caller's banded buffers, no DP).
+int rnnt_align_banded(rs_engine* e, const char* fn, const float* enc, const int32_t* enc_len, int B, int T_max, const int32_t* labels,
+                      const int32_t* label_len, int U_max, const int32_t* band_lo, const int32_t* band_hi, float* lp_blank, float* lp_emit,
+                      int32_t* frames, float* token_lp, float* viterbi, float* loglik, int32_t* edge, cudaStream_t s) {
+  const bool seam = lp_blank != nullptr;
+  if (!e || !enc || !enc_len || !labels || !label_len || !band_lo || !band_hi || B <= 0 || T_max <= 0 || U_max <= 0 ||
+      (seam ? lp_emit == nullptr : (!frames || !token_lp || !viterbi || !loglik || !edge)))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  const rs_model_config& c = e->cfg;
+  char msg[256] = "";
+  if (!rs::align_supported(c.joint_hidden, c.pred_hidden, c.vocab_size, 1, msg)) return fail(e, RS_ERR_UNSUPPORTED, "%s: %s", fn, msg);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  const int U1 = U_max + 1, Hj = c.joint_hidden, Hp = c.pred_hidden;
+  std::vector<int32_t> T(B), U(B), y(static_cast<size_t>(B) * U_max);
+  RS_CUDA(e, cudaMemcpyAsync(T.data(), enc_len, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  RS_CUDA(e, cudaMemcpyAsync(U.data(), label_len, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  RS_CUDA(e, cudaMemcpyAsync(y.data(), labels, y.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  RS_CUDA(e, cudaStreamSynchronize(s));
+  std::vector<int64_t> off(static_cast<size_t>(B) * U1, 0);
+  std::vector<int4> tiles;
+  int64_t cells = 0;
+  int pitch = 1, U_top = 0;
+  for (int b = 0; b < B; ++b) {
+    const int Tb = T[b], Ub = U[b];
+    if (Tb < 1 || Tb > T_max || Ub < 0 || Ub > U_max)
+      return fail(e, RS_ERR_INVALID_ARG, "%s: utterance %d: enc_len=%d outside [1, %d] or label_len=%d outside [0, %d]", fn, b, Tb, T_max, Ub, U_max);
+    for (int u = 0; u < Ub; ++u) {
+      const int k = y[static_cast<size_t>(b) * U_max + u];
+      if (k < 0 || k >= c.vocab_size) return fail(e, RS_ERR_INVALID_ARG, "%s: utterance %d: label %d = %d outside [0, %d)", fn, b, u, k, c.vocab_size);
+    }
+    const int32_t* lo = band_lo + static_cast<size_t>(b) * U1;
+    const int32_t* hi = band_hi + static_cast<size_t>(b) * U1;
+    if (lo[0] != 0 || hi[Ub] != Tb)
+      return fail(e, RS_ERR_INVALID_ARG, "%s: utterance %d: the band must start at frame 0 in row 0 (got %d) and end at enc_len=%d in row %d (got %d)",
+                  fn, b, lo[0], Tb, Ub, hi[Ub]);
+    for (int u = 0; u <= Ub; ++u) {
+      if (lo[u] < 0 || lo[u] >= hi[u] || hi[u] > Tb)
+        return fail(e, RS_ERR_INVALID_ARG, "%s: utterance %d row %d: band [%d, %d) is empty or outside [0, %d)", fn, b, u, lo[u], hi[u], Tb);
+      if (u > 0 && (lo[u] < lo[u - 1] || hi[u] < hi[u - 1]))
+        return fail(e, RS_ERR_INVALID_ARG, "%s: utterance %d row %d: band [%d, %d) decreases from row %d's [%d, %d)", fn, b, u, lo[u], hi[u], u - 1,
+                    lo[u - 1], hi[u - 1]);
+      if (u > 0 && lo[u] >= hi[u - 1])
+        return fail(e, RS_ERR_INVALID_ARG, "%s: utterance %d: rows %d [%d, %d) and %d [%d, %d) do not overlap", fn, b, u - 1, lo[u - 1], hi[u - 1], u,
+                    lo[u], hi[u]);
+      off[static_cast<size_t>(b) * U1 + u] = cells;
+      cells += hi[u] - lo[u];
+    }
+    for (int d = 0, u0 = 0, u1 = 0; d < Tb + Ub; ++d) {        // diagonal d meets the rows [u0, u1]
+      while (u1 < Ub && u1 + 1 + lo[u1 + 1] <= d) ++u1;
+      while (u0 + hi[u0] <= d) ++u0;
+      pitch = std::max(pitch, u1 - u0 + 1);
+    }
+    for (int u0 = 0; u0 <= Ub; u0 += 8) {                       // rows [u0, u0 + 8) cover the frames [lo[u0], hi[last row])
+      const int ul = std::min(u0 + 7, Ub);
+      for (int t0 = lo[u0] / 16 * 16; t0 < hi[ul]; t0 += 16) tiles.push_back(make_int4(b, t0, u0, 0));
+    }
+    U_top = std::max(U_top, Ub);
+  }
+  if (tiles.size() > static_cast<size_t>(INT32_MAX)) return fail(e, RS_ERR_INVALID_ARG, "%s: %zu lattice tiles exceed one launch", fn, tiles.size());
+  if (!seam && rs::band_dp_smem(pitch) > 227 * 1024)
+    return fail(e, RS_ERR_UNSUPPORTED, "%s: a diagonal meets %d rows of the band, more than the DP's shared memory holds (%d)", fn, pitch,
+                static_cast<int>(227 * 1024 / rs::band_dp_smem(1)));
+  Nvtx range("rs::rnnt_align_banded");
+  const size_t M = static_cast<size_t>(B) * T_max, rows = static_cast<size_t>(B) * U1;
+  rs::Arena a;
+  const size_t o_xn = a.take(M * c.d_model * 2), o_encp = a.take(M * Hj * 4);
+  const size_t o_h = a.take(rows * Hp * 4), o_c = a.take(static_cast<size_t>(B) * Hp * 4), o_pp = a.take(rows * Hj * 4);
+  const size_t o_lo = a.take(rows * 4), o_hi = a.take(rows * 4), o_off = a.take(rows * 8), o_tiles = a.take(tiles.size() * sizeof(int4));
+  size_t o_lpb = 0, o_lpe = 0, o_ch = 0;
+  if (!seam) { o_lpb = a.take(cells * 4); o_lpe = a.take(cells * 4); o_ch = a.take(cells); }
+  RS_TRY(grow_align_ws(e, fn, a.off, s));
+  char* ws = static_cast<char*>(e->align_ws);
+  // pageable sources: each copy has read its source when it returns
+  RS_CUDA(e, cudaMemcpyAsync(ws + o_lo, band_lo, rows * 4, cudaMemcpyHostToDevice, s));
+  RS_CUDA(e, cudaMemcpyAsync(ws + o_hi, band_hi, rows * 4, cudaMemcpyHostToDevice, s));
+  RS_CUDA(e, cudaMemcpyAsync(ws + o_off, off.data(), rows * 8, cudaMemcpyHostToDevice, s));
+  RS_CUDA(e, cudaMemcpyAsync(ws + o_tiles, tiles.data(), tiles.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
+  rs::AlignArgs g{};
+  g.enc_proj = reinterpret_cast<float*>(ws + o_encp); g.enc_len = enc_len; g.labels = labels; g.label_len = label_len;
+  g.w_out = e->dec.out_w; g.b_out = e->dec.out_b; g.w_lstm = e->dec.lstm_w; g.gate_tab = e->dec.gate_tab;
+  g.w_pred = e->dec.pred_w; g.b_pred = e->dec.pred_b;
+  g.B = B; g.T_max = T_max; g.U_max = U_max; g.Hj = Hj; g.Hp = Hp; g.V = c.vocab_size;
+  g.h = reinterpret_cast<float*>(ws + o_h); g.c = reinterpret_cast<float*>(ws + o_c); g.pred_proj = reinterpret_cast<float*>(ws + o_pp);
+  g.lp_blank = seam ? lp_blank : reinterpret_cast<float*>(ws + o_lpb); g.lp_emit = seam ? lp_emit : reinterpret_cast<float*>(ws + o_lpe);
+  g.choice = reinterpret_cast<uint8_t*>(ws + o_ch);
+  g.frames = frames; g.token_lp = token_lp; g.viterbi = viterbi; g.loglik = loglik;
+  g.band_lo = reinterpret_cast<int32_t*>(ws + o_lo); g.band_hi = reinterpret_cast<int32_t*>(ws + o_hi);
+  g.band_off = reinterpret_cast<int64_t*>(ws + o_off); g.band_tiles = reinterpret_cast<int4*>(ws + o_tiles);
+  g.band_pitch = pitch; g.edge = edge;
+  // joint.enc over every frame and the teacher-forced predictor, as in the forced alignment
+  RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc, ws + o_xn, static_cast<int64_t>(M) * c.d_model, s));
+  RS_TRY(gemm(e, {ws + o_xn, e->dec.enc_w, e->dec.enc_b, nullptr, ws + o_encp, static_cast<int>(M), Hj, c.d_model, RS_EPI_BIAS_F32, 1.f}, s));
+  for (int u = 0; u <= U_top; ++u) RS_LAUNCH(e, s, 1, rs::launch_align_lstm_step(g, u, s));
+  RS_LAUNCH(e, s, 1, rs::launch_align_pred_proj(g, s));
+  {
+    const int n = static_cast<int>(tiles.size());
+    const int r = launch(e, s, "rnnt_lattice_kernel<band>", 1, 0.0, [&] { return rs::launch_rnnt_lattice_band(g, n, s, msg); });
+    if (r != RS_OK && msg[0] != '\0') return fail(e, r, "%s: %s", fn, msg);
+    RS_TRY(r);
+  }
+  if (!seam) RS_LAUNCH(e, s, 1, rs::launch_rnnt_band_dp(g, s));
+  return RS_OK;
+}
+
 // Keyword spotting (align.cu, spot.cu; semantics: reazonspeech_b200/keywords.py): joint.enc once per recording, the
 // predictor once per keyword, then the lattice, the recursion and the hits of every (recording, keyword) pair.
 int rnnt_spot(rs_engine* e, const float* enc, const int32_t* enc_len, int n_rec, int T_max, const int32_t* labels,
@@ -1270,6 +1377,23 @@ int rs_rnnt_align_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc
   if (lp_blank_dev == nullptr || lp_emit_dev == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_align_lattice: bad arguments");
   return rnnt_align(e, "rs_rnnt_align_lattice", enc_dev, enc_len_dev, B, T_max, labels_dev, label_len_dev, U_max, lp_blank_dev, lp_emit_dev,
                     nullptr, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_align_banded(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, const int32_t* labels_dev,
+                         const int32_t* label_len_dev, int U_max, const int32_t* band_lo_host, const int32_t* band_hi_host, int32_t* frames_dev,
+                         float* token_lp_dev, float* viterbi_dev, float* loglik_dev, int32_t* edge_dev, void* stream) {
+  return rnnt_align_banded(e, "rs_rnnt_align_banded", enc_dev, enc_len_dev, B, T_max, labels_dev, label_len_dev, U_max, band_lo_host,
+                           band_hi_host, nullptr, nullptr, frames_dev, token_lp_dev, viterbi_dev, loglik_dev, edge_dev,
+                           static_cast<cudaStream_t>(stream));
+}
+
+int rs_rnnt_align_banded_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, const int32_t* labels_dev,
+                                 const int32_t* label_len_dev, int U_max, const int32_t* band_lo_host, const int32_t* band_hi_host,
+                                 float* lp_blank_dev, float* lp_emit_dev, void* stream) {
+  if (lp_blank_dev == nullptr || lp_emit_dev == nullptr) return fail(e, RS_ERR_INVALID_ARG, "rs_rnnt_align_banded_lattice: bad arguments");
+  return rnnt_align_banded(e, "rs_rnnt_align_banded_lattice", enc_dev, enc_len_dev, B, T_max, labels_dev, label_len_dev, U_max, band_lo_host,
+                           band_hi_host, lp_blank_dev, lp_emit_dev, nullptr, nullptr, nullptr, nullptr, nullptr,
+                           static_cast<cudaStream_t>(stream));
 }
 
 int rs_rnnt_align_segment(rs_engine* e, const float* enc_dev, const int32_t* enc_len_dev, int B, int T_max, const int32_t* labels_dev,

@@ -145,6 +145,11 @@ struct AlignArgs {
   uint8_t* choice;            // Viterbi predecessor of every cell (1: the emission from (t, u - 1))
   int32_t* frames; float* token_lp; float* viterbi; float* loglik;
   int32_t* seg; float* frame_lp;  // segment alignment only: (s, e) [B][2], f32 [B][T_max]
+  // banded alignment only: row (b, u) holds the frames [band_lo, band_hi) at band_off + (t - band_lo) of lp_blank / lp_emit /
+  // choice ([B][U_max + 1] each); band_tiles lists the (utterance, t0, u0) lattice tiles that meet the band; the DP keeps
+  // band_pitch cells per live diagonal and writes edge [B]
+  const int32_t* band_lo; const int32_t* band_hi; const int64_t* band_off; const int4* band_tiles;
+  int band_pitch; int32_t* edge;
 };
 // shapes the kernels implement (false: err, >= 256 B, says why)
 bool align_supported(int Hj, int Hp, int V, int U_max, char* err);
@@ -157,6 +162,11 @@ cudaError_t launch_rnnt_lattice(const AlignArgs& a, cudaStream_t stream, char* e
 cudaError_t launch_rnnt_align_dp(const AlignArgs& a, cudaStream_t stream);
 // segment alignment (free start and end) -> seg, frames, token_lp, frame_lp, viterbi, loglik
 cudaError_t launch_rnnt_segment_dp(const AlignArgs& a, cudaStream_t stream);
+// banded alignment: the n_tiles tiles of a.band_tiles into banded storage; then the recursions and backtrace on the band's
+// cells -> frames, token_lp, viterbi, loglik, edge (band_dp_smem: shared memory for a.band_pitch)
+cudaError_t launch_rnnt_lattice_band(const AlignArgs& a, int n_tiles, cudaStream_t stream, char* err);
+cudaError_t launch_rnnt_band_dp(const AlignArgs& a, cudaStream_t stream);
+size_t band_dp_smem(int pitch);
 
 // Keyword spotting (align.cu, spot.cu; semantics: reazonspeech_b200/keywords.py): the AlignArgs of the B keywords, whose enc_proj
 // and enc_len are the n_rec recordings'; pair p = r * B + k, and the lattice arrays are the pairs'.

@@ -54,7 +54,7 @@ EXPORTS = [
     "rs_attention", "rs_conv_dw", "rs_sub_conv0_dw1", "rs_sub_dw", "rs_set_phrase_boosting",
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
     "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots", "rs_rnnt_alsd_nbest", "rs_rnnt_maes", "rs_maes_last_rows",
-    "rs_rnnt_align_segment", "rs_rnnt_spot", "rs_rnnt_spot_lattice",
+    "rs_rnnt_align_segment", "rs_rnnt_spot", "rs_rnnt_spot_lattice", "rs_rnnt_align_banded", "rs_rnnt_align_banded_lattice",
 ]
 
 MAX_NBEST = 64                          # include/rs_engine.h RS_MAX_NBEST
@@ -140,6 +140,10 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_align_lattice.restype = ip
     lib.rs_rnnt_align_segment.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp, vp, vp]
     lib.rs_rnnt_align_segment.restype = ip
+    lib.rs_rnnt_align_banded.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.rs_rnnt_align_banded.restype = ip
+    lib.rs_rnnt_align_banded_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, vp, vp, vp, vp, vp]
+    lib.rs_rnnt_align_banded_lattice.restype = ip
     lib.rs_rnnt_spot.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, ip, C.c_float, ip, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.rs_rnnt_spot.restype = ip
     lib.rs_rnnt_spot_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, ip, vp, vp, vp]
@@ -705,6 +709,44 @@ class Engine:
         self._check(self.lib.rs_rnnt_align_lattice(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, labels.data_ptr(), label_len.data_ptr(), U,
                                                    lp_blank.data_ptr(), lp_emit.data_ptr(), self._stream()), "rs_rnnt_align_lattice")
         return lp_blank, lp_emit
+
+    @staticmethod
+    def _band_rows(band, B: int, U: int) -> np.ndarray:
+        """A host band [B, <= U + 1] as the int32 [B, U + 1] the C call reads (the padding rows are never read)."""
+        band = np.asarray(band, dtype=np.int32)
+        assert band.ndim == 2 and band.shape[0] == B and band.shape[1] <= U + 1
+        out = np.zeros((B, U + 1), dtype=np.int32)
+        out[:, : band.shape[1]] = band
+        return out
+
+    def align_banded(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor, band_lo, band_hi):
+        """Banded alignment of labels[b, :label_len[b]] inside the band band_lo[b][u] <= t < band_hi[b][u] (host int32 arrays
+        [B, >= label_len + 1]; rs_rnnt_align_banded; semantics: alignment.py) -> (frames i32 [B, U], token_lp f32 [B, U],
+        viterbi f32 [B], loglik f32 [B], edge i32 [B]) device tensors."""
+        B, T, labels, U = self._align_inputs(enc, enc_len, labels, label_len)
+        lo, hi = self._band_rows(band_lo, B, U), self._band_rows(band_hi, B, U)
+        frames = torch.empty(B, U, dtype=torch.int32, device=self.device)
+        token_lp = torch.empty(B, U, dtype=torch.float32, device=self.device)
+        viterbi = torch.empty(B, dtype=torch.float32, device=self.device)
+        loglik = torch.empty(B, dtype=torch.float32, device=self.device)
+        edge = torch.empty(B, dtype=torch.int32, device=self.device)
+        self._check(self.lib.rs_rnnt_align_banded(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, labels.data_ptr(), label_len.data_ptr(), U,
+                                                  lo.ctypes.data, hi.ctypes.data, frames.data_ptr(), token_lp.data_ptr(), viterbi.data_ptr(),
+                                                  loglik.data_ptr(), edge.data_ptr(), self._stream()), "rs_rnnt_align_banded")
+        return frames, token_lp, viterbi, loglik, edge
+
+    def align_banded_lattice(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor, band_lo,
+                             band_hi, cells: int):
+        """The banded lattice alone (rs_rnnt_align_banded_lattice) -> (lp_blank, lp_emit) f32 [cells] in banded storage
+        (longform.band_offsets gives each row's offset; ``cells`` is their total)."""
+        B, T, labels, U = self._align_inputs(enc, enc_len, labels, label_len)
+        lo, hi = self._band_rows(band_lo, B, U), self._band_rows(band_hi, B, U)
+        lp_blank = torch.full((max(cells, 1),), float("nan"), device=self.device)
+        lp_emit = torch.full((max(cells, 1),), float("nan"), device=self.device)
+        self._check(self.lib.rs_rnnt_align_banded_lattice(self.h, enc.data_ptr(), enc_len.data_ptr(), B, T, labels.data_ptr(),
+                                                          label_len.data_ptr(), U, lo.ctypes.data, hi.ctypes.data, lp_blank.data_ptr(),
+                                                          lp_emit.data_ptr(), self._stream()), "rs_rnnt_align_banded_lattice")
+        return lp_blank[:cells], lp_emit[:cells]
 
     def spot(self, enc: torch.Tensor, enc_len: torch.Tensor, labels: torch.Tensor, label_len: torch.Tensor, threshold: float = -1.0,
              max_hits: int = 64, scores: bool = False):

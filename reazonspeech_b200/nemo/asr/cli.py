@@ -25,6 +25,9 @@ With neither option the output is unchanged.
 Fourth extension, forced alignment of known transcripts (reazonspeech_b200/alignment.py): instead of transcribing, each AUDIO is
 aligned to its given transcript and the segments are written through the same writer with the same time offsets
   --text=FILE          UTF-8 text, one transcript line per AUDIO argument, in order (a count mismatch is an error)
+  --band=SECONDS       long-form alignment (reazonspeech_b200/longform.py) of the one AUDIO argument: FILE is its whole
+                       transcript (the non-blank lines are joined), aligned in a band of SECONDS around the recording's greedy
+                       transcript (4 is the library's default; not calibrated).  Needs --text and exactly one AUDIO argument
 Without the option the output is unchanged.
 Fifth extension, streaming (reazonspeech_b200/streaming.py): the one AUDIO argument is decoded chunk by chunk as a live stream
   --stream             AUDIO is a file, or - for raw 16-bit little-endian 16 kHz mono PCM on stdin; every chunk's final
@@ -62,7 +65,7 @@ from typing import List, Optional
 
 SHORT_OPTS = "ho:"
 LONG_OPTS = ("help", "output=", "to=", "phrases=", "phrase-score=", "lm=", "lm-alpha=", "text=", "stream", "chunk=", "left=", "right=",
-             "captions=", "before=", "after=", "decoding=", "beam=", "keywords=", "keyword-threshold=", "max-hits=")
+             "captions=", "before=", "after=", "decoding=", "beam=", "keywords=", "keyword-threshold=", "max-hits=", "band=")
 
 
 @dataclass
@@ -88,6 +91,7 @@ class Options:
     keywords: Optional[str] = None
     keyword_threshold: Optional[float] = None
     max_hits: Optional[int] = None
+    band: Optional[float] = None
 
 
 def parse(argv) -> Options:
@@ -127,6 +131,8 @@ def parse(argv) -> Options:
             opt.keyword_threshold = float(value)
         if flag == "--max-hits":
             opt.max_hits = int(value)
+        if flag == "--band":
+            opt.band = float(value)
     if (opt.lm is None) != (opt.lm_alpha is None):
         raise ValueError("--lm and --lm-alpha go together: the LM weight has no default (try values around 0.3-0.5 and tune "
                          "on held-out audio)" if opt.lm is not None else "--lm-alpha needs an LM: --lm=FILE")
@@ -150,6 +156,13 @@ def parse(argv) -> Options:
             raise ValueError("--captions goes with neither --stream nor --text")
         if opt.before < 0 or opt.after < 0:
             raise ValueError(f"--before and --after are margins in seconds >= 0, got {opt.before} and {opt.after}")
+    if opt.band is not None:
+        if opt.text is None:
+            raise ValueError("--band=SECONDS aligns the whole transcript given by --text=FILE")
+        if len(opt.audio) > 1:
+            raise ValueError("--band aligns the transcript of one AUDIO argument")
+        from ...longform import band_frames
+        band_frames(opt.band)
     if opt.keywords is None:
         if opt.keyword_threshold is not None or opt.max_hits is not None:
             raise ValueError("--keyword-threshold and --max-hits set the search of --keywords=FILE")
@@ -175,12 +188,20 @@ def load_transcripts(path: str, n_audio: int) -> List[str]:
     return lines
 
 
+def load_long_transcript(path: str) -> str:
+    """--text with --band: the whole transcript of one recording, its non-blank lines joined."""
+    with open(path, encoding="utf-8") as f:
+        return "".join(line.strip() for line in f.read().splitlines() if line.strip())
+
+
 def run(opt: Options) -> None:
     from .audio import audio_from_path
-    from .transcribe import align_batch, load_model, transcribe, transcribe_batch
+    from .transcribe import align_batch, align_long, load_model, transcribe, transcribe_batch
     from .writer import get_writer
 
-    texts = load_transcripts(opt.text, len(opt.audio)) if opt.text is not None else None
+    texts = None
+    if opt.text is not None:
+        texts = [load_long_transcript(opt.text)] if opt.band is not None else load_transcripts(opt.text, len(opt.audio))
     captions = None
     if opt.captions is not None:
         from ...captions import read_captions_tsv
@@ -211,6 +232,8 @@ def run(opt: Options) -> None:
         results = [caption_segments(model, clips[0], captions, opt)]
     elif opt.stream:
         results = [stream(model, opt, clips[0] if clips else None)]
+    elif opt.band is not None:
+        results = [align_long(model, clips[0], texts[0], band_seconds=opt.band)]
     elif texts is not None:
         results = align_batch(model, clips, texts)
     else:

@@ -23,6 +23,7 @@ import torch
 
 from ...alignment import alignment_hypothesis, pack_labels, validate_labels
 from ...captions import AFTER_SECONDS, BEFORE_SECONDS, CONFIDENCE_FRAMES, AlignedCaption, Caption, caption_window
+from ...longform import BAND_SECONDS, MAX_WIDEN, align_widening, anchors, band_frames, build_band, check_extent, check_widen
 from ...keywords import MAX_HITS as KW_MAX_HITS, SCRATCH_CAP_BYTES, THRESHOLD as KW_THRESHOLD, KeywordHit, check_search, \
     hit_seconds, keyword_groups, keyword_ids
 from ...boosting import PhraseBoostingConfig, PhraseBoostingTables, build_tables, combine_tables, config_key
@@ -54,6 +55,8 @@ class Hypothesis:
     word_confidence: Optional[List[float]] = None
     log_likelihood: Optional[float] = None          # forced alignment: log P(y | x) of the given transcript (alignment.py)
     token_logprob: Optional[List[float]] = None     # forced alignment: each token's log-probability on the Viterbi path
+    edge: Optional[int] = None                      # long-form alignment: tokens on an interior band edge (alignment.py)
+    band_frames: Optional[int] = None               # long-form alignment: the band half-width W used, in frames (longform.py)
 
     @staticmethod
     def from_greedy(tokens: Sequence[int], frames: Sequence[int], blank: int) -> "Hypothesis":
@@ -365,6 +368,37 @@ class B200RnntModel:
             for i, item in zip(idx, items):
                 results[i] = item
         return results
+
+    # -- long-form alignment of a whole transcript in a band around the greedy path (alignment.py, longform.py)
+    def align_long_tokens(self, waveform: np.ndarray, ids: Sequence[int], pad: int = 0, *, band_seconds: float = BAND_SECONDS,
+                          max_widen: int = MAX_WIDEN):
+        """One 16 kHz mono recording (``pad`` zero samples on both sides) and its whole transcript -> (frames, token_lp, viterbi,
+        loglik, edge, W, alignments run): log-mel -> encode -> the greedy decode of the same encoder output (the transcript
+        ``transcribe_tokens`` gives) -> anchors and band (longform.py) -> rs_rnnt_align_banded, widened while edge > 0.  A band
+        whose diagonal is too wide for the DP raises ValueError naming the stretch of tokens."""
+        ids = validate_labels([ids], self.cfg.vocab_size, 1)[0]
+        W0, max_widen = band_frames(band_seconds), check_widen(max_widen)
+        eng = self.engine
+        wav, lens = self._staging[0].stage([waveform], pad)
+        with torch.cuda.device(eng.device):
+            x = wav.to(eng.device, non_blocking=True)
+            if x.dtype == torch.int16:
+                x = x.to(torch.float32) * (1.0 / 32768.0)
+            enc, enc_len = eng.encode(*eng.log_mel(x, lens.to(eng.device)))
+            tk, fr, nt = [a.cpu() for a in eng.greedy(enc, enc_len)]
+            T, n = int(enc_len[0]), int(nt[0])
+            anchor = anchors(ids, tk[0, :n].tolist(), fr[0, :n].tolist())
+            labels, label_len = pack_labels([ids])
+            labels_d, label_len_d = torch.from_numpy(labels).to(eng.device), torch.from_numpy(label_len).to(eng.device)
+
+            def run(W):
+                lo, hi = build_band(anchor, T, W)
+                check_extent(lo, hi, T)
+                return [a.cpu() for a in eng.align_banded(enc, enc_len, labels_d, label_len_d, lo[None], hi[None])]
+
+            (frames, token_lp, viterbi, loglik, edge), W, runs = align_widening(run, W0, max_widen)
+        U = len(ids)
+        return frames[0, :U].tolist(), token_lp[0, :U].tolist(), float(viterbi[0]), float(loglik[0]), int(edge[0]), W, runs
 
     # -- segment alignment of captions inside their windows (alignment.py, captions.py)
     def iter_align_segment_batches(self, waveforms: Sequence[np.ndarray], token_lists: Sequence[Sequence[int]], pad: int = 0):
@@ -820,6 +854,41 @@ def align_batch(model, audios: Sequence[AudioData], texts: Sequence, config: Opt
 def align(model, audio: AudioData, text, config: Optional[TranscribeConfig] = None) -> TranscribeResult:
     """One utterance of ``align_batch``."""
     return align_batch(model, [audio], [text], config)[0]
+
+
+def align_long_batch(model, audios: Sequence[AudioData], texts: Sequence, *, band_seconds: float = BAND_SECONDS,
+                     max_widen: int = MAX_WIDEN, config: Optional[TranscribeConfig] = None) -> List[TranscribeResult]:
+    """Long-form forced alignment (longform.py): ``texts[i]`` (a str, or a sequence of token ids), the whole transcript of a long
+    recording without timestamps, against ``audios[i]``, results in input order.  Each recording's greedy transcript anchors
+    the text and the alignment runs in a band of ``band_seconds`` (NOT calibrated, see longform.py) around the anchors on the
+    GPU, the band doubled and the text aligned again while a token lies on the band's edge, at most ``max_widen`` times.  The
+    audio is prepared and the result built as ``align_batch`` does (a band that covers the whole lattice gives ``align``'s
+    result); ``result.hypothesis`` also carries edge (alignment.py) and band_frames, the half-width W used.  Bad token ids, a
+    count mismatch, a bad band_seconds / max_widen or a model on several GPUs raise ValueError before the GPU is touched."""
+    if not hasattr(model, "align_long_tokens"):
+        raise ValueError("long-form alignment runs on one GPU: use load_model() without devices=")
+    if len(texts) != len(audios):
+        raise ValueError(f"{len(texts)} transcripts for {len(audios)} audio inputs")
+    band_frames(band_seconds)
+    check_widen(max_widen)
+    ids = validate_labels([_target_ids(model, t) for t in texts], model.cfg.vocab_size, len(audios))
+    pad = int(PAD_SECONDS * SAMPLERATE)
+    out: List[TranscribeResult] = []
+    for k, a in zip(ids, audios):
+        frames, token_lp, viterbi, loglik, edge, W, _ = model.align_long_tokens(np.asarray(norm_audio(a).waveform), k, pad=pad,
+                                                                                band_seconds=band_seconds, max_widen=max_widen)
+        hyp = alignment_hypothesis(k, frames, token_lp, viterbi, loglik, model.cfg.blank)
+        hyp.edge, hyp.band_frames = edge, W
+        result = decode_hypothesis(model, hyp)
+        result.hypothesis = hyp
+        out.append(result)
+    return out
+
+
+def align_long(model, audio: AudioData, text, *, band_seconds: float = BAND_SECONDS, max_widen: int = MAX_WIDEN,
+               config: Optional[TranscribeConfig] = None) -> TranscribeResult:
+    """One recording of ``align_long_batch``."""
+    return align_long_batch(model, [audio], [text], band_seconds=band_seconds, max_widen=max_widen, config=config)[0]
 
 
 def align_captions(model, audio: AudioData, captions: Sequence[Caption], *, before: float = BEFORE_SECONDS,

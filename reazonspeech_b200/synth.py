@@ -29,3 +29,19 @@ def synth_clip(index: int, seconds: float, seed: int = 1234) -> np.ndarray:
 
 def synth_batch(count: int, seconds: float, seed: int = 1234):
     return [synth_clip(i, seconds, seed) for i in range(count)]
+
+
+def edit_tokens(tokens, vocab_size: int, seed: int, sub: float = 0.05, dele: float = 0.05, ins: float = 0.05):
+    """A transcript that differs from ``tokens`` by seeded edits: each token is substituted by a random id with probability
+    ``sub`` or deleted with probability ``dele``, and a random id is inserted after it with probability ``ins``."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for k in tokens:
+        r = rng.random()
+        if r < sub:
+            out.append(int(rng.integers(0, vocab_size)))
+        elif r >= sub + dele:
+            out.append(int(k))
+        if rng.random() < ins:
+            out.append(int(rng.integers(0, vocab_size)))
+    return out
