@@ -431,6 +431,54 @@ int rs_rnnt_spot_lattice(rs_engine* e, const float* enc_dev, const int32_t* enc_
                          const int32_t* labels_dev, const int32_t* label_len_dev, int n_kw, int U_max,
                          float* lp_blank_dev, float* lp_emit_dev, void* stream);
 
+/* Streaming keyword spotting: keyword hits on live streams, decided chunk by chunk on the encoder output the streaming decode
+ * produces (semantics: reazonspeech_b200/keywords.py, "Streaming"; frame grid: streaming.py).
+ *
+ * rs_set_spot_keywords installs the engine's keyword set: labels_host i32[n_kw, U_max], label_len_host i32[n_kw] (each in
+ * [1, U_max], labels in [0, vocab_size)), U_max in [1, 32], the threshold (finite or -inf), the alert delay D = delay_frames
+ * >= 0 and the chunk C = chunk_frames >= 1 (the most frames one row decodes per call).  It runs the teacher-forced predictor
+ * of every keyword once, into engine-owned memory, and synchronises `stream`; replacing or clearing the set (n_kw = 0) first
+ * waits for the device.  RS_ERR_INVALID_ARG for a bad label or length, U_max outside 1..32, a NaN or +inf threshold, a
+ * ring of D + C entries above 14 528 (the pick kernel's shared memory), and n_kw x (D + C) above 33 554 431 (one row's
+ * share of a call's hit list).  Every failure, an allocation or launch failure included, keeps the previous set: the new
+ * set is built before the old one is freed.
+ *
+ * State: one record per (stream slot, keyword), rs_spot_state_bytes() bytes each (0 without a set), 16-byte aligned, in
+ * caller-owned device memory [n_slots][n_kw]: a 32-byte header (frames seen, barrier + 1, forced cuts, ring head, ring size),
+ * the carried column (12 U_max bytes), the token lists of every row (8 U_max^2 bytes) and a ring of D + C pending candidates
+ * of 12 + 8 U_max bytes: 32 + 12 U + 8 U^2 + (D + C)(12 + 8 U) bytes rounded up to 16 (about 12 KB at U_max = 8 and 48 KB
+ * at 32 with D = 125, C = 20).  Only the header is part of the interface: header[2] counts the stream's forced cuts.  An
+ * all-zero record is a stream that has not started.  Row b must continue its stream: its first frame is the stream's frame
+ * "frames seen" (not checked: the records are on the device).
+ *
+ * Hits: every call decides the hits of its rows and returns them in host arrays of max_out >= rs_spot_max_hits(B) entries
+ * (B x n_kw x (D + C), the worst case; a call whose B makes that exceed INT32_MAX is rejected), sorted by (row, keyword, e): meta i32[5] = (row, keyword, s, e, forced), val f32[2] =
+ * (score E(e), confidence m(e)), frames i32[U_max] and token_lp f32[U_max] (the keyword's tokens on the hit's path; -1 and NaN
+ * beyond its length), and *n_hits.  Frames are the stream's frames.  last[b] != 0 says row b's call decodes the stream's last
+ * frame: everything pending is decided.  Both calls synchronise.
+ *
+ * rs_rnnt_spot_resume: the device-level seam, shaped like rs_rnnt_greedy_resume: enc f32[B,T_max,d_model], dec_begin /
+ * dec_end / slot / last device i32[B] (read back and checked before any launch: slots distinct in [0, n_slots), 0 <=
+ * dec_begin <= dec_end <= T_max, at most C frames).  Optional E f32 / S i32 [B, n_kw, T_max] receive E(e) and S(e) at the
+ * buffer frames [dec_begin, dec_end) (the rest untouched), sigma i32[B, n_kw] the bound sigma(t) after the call (-1 before the
+ * stream's first frame).
+ * rs_stream_step_spot: rs_stream_step plus the resumed spot on the same joint.enc rows, in one call: host last_host i32[B], the
+ * spot records, and the hit outputs; the decode's tokens, frames and statistics are rs_stream_step's.  A call without an
+ * installed set, bad slots or ranges, or a small max_out is rejected before any launch. */
+int rs_set_spot_keywords(rs_engine* e, const int32_t* labels_host, const int32_t* label_len_host, int n_kw, int U_max, float threshold,
+                         int delay_frames, int chunk_frames, void* stream);
+size_t rs_spot_state_bytes(const rs_engine* e);
+int rs_spot_max_hits(const rs_engine* e, int B);
+int rs_rnnt_spot_resume(rs_engine* e, const float* enc_dev, const int32_t* dec_begin_dev, const int32_t* dec_end_dev, const int32_t* slot_dev,
+                        const int32_t* last_dev, void* records_dev, int n_slots, int B, int T_max, int max_out, int32_t* hit_meta_host,
+                        float* hit_val_host, int32_t* hit_frames_host, float* hit_token_lp_host, int32_t* n_hits_host, float* E_dev,
+                        int32_t* S_dev, int32_t* sigma_dev, void* stream);
+int rs_stream_step_spot(rs_engine* e, const void* wav_host, int wav_is_pcm16, const int32_t* len_host, const int32_t* dec_begin_host,
+                        const int32_t* dec_end_host, const int32_t* slot_host, void* states_dev, int B, int L_max, int32_t* tokens_host,
+                        int32_t* frames_host, int32_t* n_tok_host, int U_max, float alpha, float* stats_host, const int32_t* last_host,
+                        void* spot_records_dev, int n_slots, int max_out, int32_t* hit_meta_host, float* hit_val_host,
+                        int32_t* hit_frames_host, float* hit_token_lp_host, int32_t* n_hits_host, void* stream);
+
 /* norm_audio on the device (pkg/nemo-asr/src/audio.py:54-68: resample to 16 kHz, then average the channels) fused with
  * transcribe()'s padding (audio.py:70-83): in [B, channels, L_in_max] f32 or int16 PCM at the native rate ->
  * out f32 [B, L_out_row], row b = pad zeros | resampled mono utterance | zeros, len_out[b] = resampled length + 2 pad;

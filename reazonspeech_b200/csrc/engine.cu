@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <map>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -82,6 +83,12 @@ struct rs_engine {
   // rs_stream_step: device copies of the step's dec_begin | dec_end | slot, grown on demand
   void* stream_args = nullptr;
   size_t stream_args_bytes = 0;
+  // streaming keyword spotting (rs_set_spot_keywords): the installed keyword set, its labels and its teacher-forced predictor
+  // rows (pred_proj [n_kw][U_max + 1][Hj]) in one engine-owned allocation; the calls' scratch grown on demand
+  struct { int n_kw = 0, U_max = 0, delay = 0, chunk = 0, ring_cap = 0; float threshold = 0.f; void* mem = nullptr;
+           const int32_t* labels = nullptr; const int32_t* label_len = nullptr; float* pred_proj = nullptr; } spot;
+  void* spot_ws = nullptr;
+  size_t spot_ws_bytes = 0;
   unsigned int* lm_tickets = nullptr;   // per-utterance CTA tickets of the log-mel statistics (engine-owned, kept zero between launches)
   static constexpr int kMaxBatch = 1 << 16;
   struct { const float *c0w, *c0b, *d1w, *d1b, *p1b, *d2w, *d2b, *p2b, *ob; const void *p1w, *p2w, *ow; } sub;
@@ -505,6 +512,8 @@ void rs_engine_destroy(rs_engine* e) {
   cudaFree(e->alsd_ws);
   cudaFree(e->align_ws);
   cudaFree(e->stream_args);
+  cudaFree(e->spot.mem);
+  cudaFree(e->spot_ws);
   cudaFree(e->boost_roots);
   if (e->alsd_done_host) cudaFreeHost(e->alsd_done_host);
   delete e;
@@ -696,6 +705,155 @@ int rs_rnnt_greedy_resume(rs_engine* e, const float* enc, const int32_t* dec_beg
 
 namespace {
 
+int grow_align_ws(rs_engine* e, const char* fn, size_t bytes, cudaStream_t s);
+
+// Streaming keyword spotting (spot_stream.cu; semantics: reazonspeech_b200/keywords.py, "Streaming").  One call's rows: host
+// copies of dec_begin / dec_end / slot / last (checked before any launch), the records, and the host outputs.
+struct SpotCall {
+  const int32_t *dec_begin, *dec_end, *slot, *last;
+  void* records; int n_slots;
+  int max_out; int32_t* meta; float* val; int32_t* frames; float* token_lp; int32_t* n_out;
+  float* E; int32_t* S; int32_t* sigma;          // device, optional (the test seam)
+};
+
+int spot_capacity(const rs_engine* e, int B) {
+  const int64_t n = static_cast<int64_t>(B) * e->spot.n_kw * e->spot.ring_cap;
+  return n > INT32_MAX ? -1 : static_cast<int>(n);
+}
+
+// Rows bounded by T_lim frames (the seam: T_max; a step: rs_stream_step's own checks come first).
+int check_spot_call(rs_engine* e, const char* fn, int B, int T_lim, const SpotCall& c) {
+  if (e->spot.n_kw == 0) return fail(e, RS_ERR_INVALID_ARG, "%s: no keyword set is installed (rs_set_spot_keywords)", fn);
+  if (!c.records || (reinterpret_cast<uintptr_t>(c.records) & 15u) || c.n_slots < 1 || !c.meta || !c.val || !c.frames || !c.token_lp ||
+      !c.n_out || ((c.E != nullptr) != (c.S != nullptr)))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments (records 16-byte aligned, n_slots >= 1, every hit output set, E and S both or neither)", fn);
+  const int cap = spot_capacity(e, B);
+  if (cap < 0)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: B=%d rows x %d keywords x %d ring entries exceed one call's hit list: fewer rows per call", fn, B,
+                e->spot.n_kw, e->spot.ring_cap);
+  if (c.max_out < cap)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: max_out=%d is below rs_spot_max_hits(B=%d) = %d", fn, c.max_out, B, cap);
+  std::vector<int32_t> seen(c.slot, c.slot + B);
+  std::sort(seen.begin(), seen.end());
+  if (seen[0] < 0 || seen.back() >= c.n_slots || std::adjacent_find(seen.begin(), seen.end()) != seen.end())
+    return fail(e, RS_ERR_INVALID_ARG, "%s: slots must be distinct and in [0, n_slots = %d)", fn, c.n_slots);
+  for (int b = 0; b < B; ++b)
+    if (c.dec_begin[b] < 0 || c.dec_begin[b] > c.dec_end[b] || c.dec_end[b] > T_lim || c.dec_end[b] - c.dec_begin[b] > e->spot.chunk)
+      return fail(e, RS_ERR_INVALID_ARG, "%s: row %d: need 0 <= dec_begin (%d) <= dec_end (%d) <= %d and at most %d frames (the installed chunk)",
+                  fn, b, c.dec_begin[b], c.dec_end[b], T_lim, e->spot.chunk);
+  return RS_OK;
+}
+
+// The compact block's frames per row: the longest range (at least 1)
+int spot_frames(int B, const SpotCall& c) {
+  int C = 1;
+  for (int b = 0; b < B; ++b) C = std::max(C, c.dec_end[b] - c.dec_begin[b]);
+  return C;
+}
+
+// The scratch of one call: staged row arguments, the gathered block and lengths, the pairs' lattice, and the hit list
+struct SpotLayout { size_t args, blk, len, lpb, lpe, n, meta, val, fr, lp, total; int cap; };
+SpotLayout spot_layout(const rs_engine* e, int B, int C) {
+  const auto& ks = e->spot;
+  const size_t cells = static_cast<size_t>(B) * ks.n_kw * C * (ks.U_max + 1);
+  SpotLayout L;
+  L.cap = spot_capacity(e, B);
+  const size_t cap = static_cast<size_t>(L.cap);
+  rs::Arena a;
+  L.args = a.take(static_cast<size_t>(4) * B * 4); L.blk = a.take(static_cast<size_t>(B) * C * e->cfg.joint_hidden * 4);
+  L.len = a.take(static_cast<size_t>(B) * 4); L.lpb = a.take(cells * 4); L.lpe = a.take(cells * 4); L.n = a.take(4);
+  L.meta = a.take(cap * rs::kSpotHitInts * 4); L.val = a.take(cap * 8);
+  L.fr = a.take(cap * ks.U_max * 4); L.lp = a.take(cap * ks.U_max * 4);
+  L.total = a.off;
+  return L;
+}
+
+// Enqueues the gather, the pairs' lattice, the resumed recursion and the streaming pick on `encp` (joint.enc of every frame,
+// f32 [B][T_max][Hj]).  args_dev: dec_begin | dec_end | slot | last on the device, or nullptr to stage the host copies.
+int spot_enqueue(rs_engine* e, const char* fn, const float* encp, int T_max, int B, const SpotCall& c, const int32_t* args_dev,
+                 cudaStream_t s) {
+  const rs_model_config& cfg = e->cfg;
+  const auto& ks = e->spot;
+  const int Hj = cfg.joint_hidden, C = spot_frames(B, c);
+  const SpotLayout L = spot_layout(e, B, C);
+  if (L.total > e->spot_ws_bytes) {
+    RS_CUDA(e, cudaStreamSynchronize(s));
+    cudaFree(e->spot_ws); e->spot_ws = nullptr; e->spot_ws_bytes = 0;
+    if (cudaMalloc(&e->spot_ws, L.total) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(e, RS_ERR_WORKSPACE, "%s: cannot allocate %zu bytes of keyword scratch", fn, L.total);
+    }
+    e->spot_ws_bytes = L.total;
+  }
+  char* ws = static_cast<char*>(e->spot_ws);
+  if (args_dev == nullptr) {                       // pageable sources: each copy has read its source when it returns
+    int32_t* d = reinterpret_cast<int32_t*>(ws + L.args);
+    const int32_t* src[4] = {c.dec_begin, c.dec_end, c.slot, c.last};
+    for (int i = 0; i < 4; ++i) RS_CUDA(e, cudaMemcpyAsync(d + i * B, src[i], static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, s));
+    args_dev = d;
+  }
+  rs::SpotStreamArgs sa{};
+  sa.dec_begin = args_dev; sa.dec_end = args_dev + B; sa.slot = args_dev + 2 * B; sa.last = args_dev + 3 * B;
+  sa.B = B; sa.n_kw = ks.n_kw; sa.U_max = ks.U_max; sa.C = C; sa.delay = ks.delay; sa.ring_cap = ks.ring_cap; sa.threshold = ks.threshold;
+  sa.label_len = ks.label_len; sa.records = static_cast<uint8_t*>(c.records); sa.len = reinterpret_cast<int32_t*>(ws + L.len);
+  sa.E_out = c.E; sa.S_out = c.S; sa.T_out = T_max; sa.sigma_out = c.sigma;
+  sa.n_hits = reinterpret_cast<int32_t*>(ws + L.n); sa.hit_cap = L.cap;
+  sa.hit_meta = reinterpret_cast<int32_t*>(ws + L.meta); sa.hit_val = reinterpret_cast<float*>(ws + L.val);
+  sa.hit_frames = reinterpret_cast<int32_t*>(ws + L.fr); sa.hit_lp = reinterpret_cast<float*>(ws + L.lp);
+  float* blk = reinterpret_cast<float*>(ws + L.blk);
+  rs::AlignArgs g{};
+  g.enc_proj = blk; g.enc_len = sa.len; g.labels = ks.labels; g.label_len = ks.label_len;
+  g.w_out = e->dec.out_w; g.b_out = e->dec.out_b;
+  g.B = ks.n_kw; g.T_max = C; g.U_max = ks.U_max; g.Hj = Hj; g.Hp = cfg.pred_hidden; g.V = cfg.vocab_size;
+  g.pred_proj = ks.pred_proj; g.lp_blank = reinterpret_cast<float*>(ws + L.lpb); g.lp_emit = reinterpret_cast<float*>(ws + L.lpe);
+  Nvtx range("rs::rnnt_spot_resume");
+  RS_CUDA(e, cudaMemsetAsync(sa.n_hits, 0, 4, s));
+  RS_LAUNCH(e, s, 1, rs::launch_spot_gather(encp, T_max, Hj, sa, blk, s));
+  {
+    char msg[256] = "";
+    const int r = launch(e, s, "rnnt_lattice_kernel<pairs>", 1, 0.0, [&] { return rs::launch_rnnt_lattice_pairs(g, B, s, msg); });
+    if (r != RS_OK && msg[0] != '\0') return fail(e, r, "%s: %s", fn, msg);
+    RS_TRY(r);
+  }
+  RS_LAUNCH(e, s, 1, rs::launch_rnnt_spot_resume_dp(g, sa, s));
+  RS_LAUNCH(e, s, 1, rs::launch_rnnt_spot_resume_pick(sa, s));
+  return RS_OK;
+}
+
+// Copies the decided hits back, sorted by (row, keyword, e); synchronises.
+int spot_collect(rs_engine* e, int B, const SpotCall& c, cudaStream_t s) {
+  const int UM = e->spot.U_max;
+  const SpotLayout L = spot_layout(e, B, spot_frames(B, c));
+  const int cap = L.cap;
+  const char* ws = static_cast<const char*>(e->spot_ws);
+  int32_t n = 0;
+  RS_CUDA(e, cudaMemcpyAsync(&n, ws + L.n, 4, cudaMemcpyDeviceToHost, s));
+  RS_CUDA(e, cudaStreamSynchronize(s));
+  n = std::min(n, cap);
+  std::vector<int32_t> meta(static_cast<size_t>(n) * rs::kSpotHitInts), fr(static_cast<size_t>(n) * UM);
+  std::vector<float> val(static_cast<size_t>(n) * 2), lp(static_cast<size_t>(n) * UM);
+  if (n > 0) {
+    RS_CUDA(e, cudaMemcpyAsync(meta.data(), ws + L.meta, meta.size() * 4, cudaMemcpyDeviceToHost, s));
+    RS_CUDA(e, cudaMemcpyAsync(val.data(), ws + L.val, val.size() * 4, cudaMemcpyDeviceToHost, s));
+    RS_CUDA(e, cudaMemcpyAsync(fr.data(), ws + L.fr, fr.size() * 4, cudaMemcpyDeviceToHost, s));
+    RS_CUDA(e, cudaMemcpyAsync(lp.data(), ws + L.lp, lp.size() * 4, cudaMemcpyDeviceToHost, s));
+    RS_CUDA(e, cudaStreamSynchronize(s));
+  }
+  std::vector<int> order(n);
+  for (int i = 0; i < n; ++i) order[i] = i;
+  const auto key = [&](int i) { const int32_t* m = &meta[static_cast<size_t>(i) * rs::kSpotHitInts]; return std::make_tuple(m[0], m[1], m[3]); };
+  std::sort(order.begin(), order.end(), [&](int x, int y) { return key(x) < key(y); });
+  for (int j = 0; j < n; ++j) {
+    const size_t i = order[j];
+    std::copy_n(&meta[i * rs::kSpotHitInts], rs::kSpotHitInts, c.meta + static_cast<size_t>(j) * rs::kSpotHitInts);
+    std::copy_n(&val[i * 2], 2, c.val + static_cast<size_t>(j) * 2);
+    std::copy_n(&fr[i * UM], UM, c.frames + static_cast<size_t>(j) * UM);
+    std::copy_n(&lp[i * UM], UM, c.token_lp + static_cast<size_t>(j) * UM);
+  }
+  *c.n_out = n;
+  return RS_OK;
+}
+
 int check_transcribe_args(rs_engine* e, const char* fn, const void* wav, const int32_t* len, int B, int L_max, const int32_t* tokens,
                           const int32_t* frames, const int32_t* n_tok, int U_max) {
   if (!e || !wav || !len || !tokens || !frames || !n_tok || B <= 0 || L_max <= 0 || U_max <= 0)
@@ -748,7 +906,7 @@ int transcribe_device(rs_engine* e, const char* fn, const void* wav, bool i16, c
 // into an engine-owned device buffer first.
 int transcribe_batch(rs_engine* e, const char* fn, const void* wav_host, bool i16, const int32_t* len_host, int B, int L_max,
                      int32_t* tokens_host, int32_t* frames_host, int32_t* n_tok_host, int U_max, float* stats_host, float alpha,
-                     cudaStream_t s, const Resume* rs_host = nullptr) {
+                     cudaStream_t s, const Resume* rs_host = nullptr, const SpotCall* spot = nullptr) {
   RS_TRY(check_transcribe_args(e, fn, wav_host, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max));
   Plan p = make_plan(e, B, L_max, U_max);
   RS_TRY(check_ws(e, p));
@@ -792,12 +950,14 @@ int transcribe_batch(rs_engine* e, const char* fn, const void* wav_host, bool i1
   RS_TRY(run_pipeline(e, p, wav, i16, len, n_chunks, n_chunks > 1 ? e->copy_ev : nullptr, at<int32_t>(e, p.tokens),
                       at<int32_t>(e, p.frames), at<int32_t>(e, p.ntok), U_max, stats_host ? at<float>(e, p.stats) : nullptr, alpha, s,
                       rs_host ? &rs_dev : nullptr));
+  if (spot) RS_TRY(spot_enqueue(e, fn, at<float>(e, p.encp), p.T3, B, *spot, nullptr, s));   // on the decode's joint.enc rows
   RS_CUDA(e, cudaMemcpyAsync(tokens_host, at<int32_t>(e, p.tokens), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(frames_host, at<int32_t>(e, p.frames), static_cast<size_t>(B) * U_max * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaMemcpyAsync(n_tok_host, at<int32_t>(e, p.ntok), static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
   if (stats_host)
     RS_CUDA(e, cudaMemcpyAsync(stats_host, at<float>(e, p.stats), static_cast<size_t>(B) * U_max * 4 * 4, cudaMemcpyDeviceToHost, s));
   RS_CUDA(e, cudaStreamSynchronize(s));
+  if (spot) RS_TRY(spot_collect(e, B, *spot, s));
   return RS_OK;
 }
 
@@ -863,6 +1023,146 @@ int rs_stream_step(rs_engine* e, const void* wav_host, int wav_is_pcm16, const i
   const Resume rs{dec_begin_host, dec_end_host, slot_host, states};
   return transcribe_batch(e, fn, wav_host, wav_is_pcm16 != 0, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max,
                           stats_host, alpha, static_cast<cudaStream_t>(stream), &rs);
+}
+
+int rs_set_spot_keywords(rs_engine* e, const int32_t* labels_host, const int32_t* label_len_host, int n_kw, int U_max, float threshold,
+                         int delay_frames, int chunk_frames, void* stream) {
+  const char* fn = "rs_set_spot_keywords";
+  if (e == nullptr) return RS_ERR_INVALID_ARG;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (n_kw == 0) {
+    if (e->spot.mem) {                       // a call still queued may read the old set
+      RS_CUDA(e, cudaSetDevice(e->device));
+      RS_CUDA(e, cudaDeviceSynchronize());
+      cudaFree(e->spot.mem);
+    }
+    e->spot = {};
+    return RS_OK;
+  }
+  if (n_kw < 0 || !labels_host || !label_len_host || U_max < 1 || U_max > rs::kSpotMaxLabels)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments (n_kw >= 0, labels and lengths set, U_max=%d in [1, %d])", fn, U_max, rs::kSpotMaxLabels);
+  if (std::isnan(threshold) || threshold == INFINITY) return fail(e, RS_ERR_INVALID_ARG, "%s: threshold must be finite or -inf", fn);
+  if (delay_frames < 0 || chunk_frames < 1) return fail(e, RS_ERR_INVALID_ARG, "%s: delay_frames=%d must be >= 0 and chunk_frames=%d >= 1", fn, delay_frames, chunk_frames);
+  const int64_t ring = static_cast<int64_t>(delay_frames) + chunk_frames;
+  if (ring > 227 * 1024 / 16 || rs::spot_pick_stream_smem(static_cast<int>(ring)) > 227 * 1024)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: a ring of delay + chunk = %lld entries does not fit the pick kernel's shared memory (at most %d)", fn,
+                static_cast<long long>(ring), 227 * 1024 / 16);
+  if (static_cast<int64_t>(n_kw) * ring > INT32_MAX / 64)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: n_kw x (delay + chunk) = %lld pending entries per stream exceed the hit list of one call (at most %d)", fn,
+                static_cast<long long>(n_kw) * ring, INT32_MAX / 64);
+  const rs_model_config& c = e->cfg;
+  for (int k = 0; k < n_kw; ++k) {
+    if (label_len_host[k] < 1 || label_len_host[k] > U_max)
+      return fail(e, RS_ERR_INVALID_ARG, "%s: keyword %d: length %d outside [1, %d]", fn, k, label_len_host[k], U_max);
+    for (int u = 0; u < label_len_host[k]; ++u) {
+      const int y = labels_host[static_cast<size_t>(k) * U_max + u];
+      if (y < 0 || y >= c.vocab_size) return fail(e, RS_ERR_INVALID_ARG, "%s: keyword %d: label %d = %d outside [0, %d)", fn, k, u, y, c.vocab_size);
+    }
+  }
+  char msg[256] = "";
+  if (!rs::align_supported(c.joint_hidden, c.pred_hidden, c.vocab_size, U_max, msg)) return fail(e, RS_ERR_UNSUPPORTED, "%s: %s", fn, msg);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  const int U1 = U_max + 1, Hj = c.joint_hidden, Hp = c.pred_hidden;
+  rs::Arena a;
+  const size_t o_lab = a.take(static_cast<size_t>(n_kw) * U_max * 4), o_len = a.take(static_cast<size_t>(n_kw) * 4);
+  const size_t o_h = a.take(static_cast<size_t>(n_kw) * U1 * Hp * 4), o_c = a.take(static_cast<size_t>(n_kw) * Hp * 4);
+  const size_t o_pp = a.take(static_cast<size_t>(n_kw) * U1 * Hj * 4);
+  // the new set is built next to the old one, so a failure below leaves the installed set as it was
+  void* mem = nullptr;
+  if (cudaMalloc(&mem, a.off) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(e, RS_ERR_WORKSPACE, "%s: cannot allocate %zu bytes for %d keywords (the installed set is kept)", fn, a.off, n_kw);
+  }
+  char* m = static_cast<char*>(mem);
+  rs::AlignArgs g{};
+  g.labels = reinterpret_cast<int32_t*>(m + o_lab); g.label_len = reinterpret_cast<int32_t*>(m + o_len);
+  g.w_lstm = e->dec.lstm_w; g.gate_tab = e->dec.gate_tab; g.w_pred = e->dec.pred_w; g.b_pred = e->dec.pred_b;
+  g.B = n_kw; g.U_max = U_max; g.Hj = Hj; g.Hp = Hp; g.V = c.vocab_size;
+  g.h = reinterpret_cast<float*>(m + o_h); g.c = reinterpret_cast<float*>(m + o_c); g.pred_proj = reinterpret_cast<float*>(m + o_pp);
+  const auto predictor = [&]() -> int {        // the teacher-forced predictor of every keyword, once, as rs_rnnt_spot runs it per call
+    RS_CUDA(e, cudaMemcpyAsync(m + o_lab, labels_host, static_cast<size_t>(n_kw) * U_max * 4, cudaMemcpyHostToDevice, s));
+    RS_CUDA(e, cudaMemcpyAsync(m + o_len, label_len_host, static_cast<size_t>(n_kw) * 4, cudaMemcpyHostToDevice, s));
+    for (int u = 0; u <= U_max; ++u) RS_LAUNCH(e, s, 1, rs::launch_align_lstm_step(g, u, s));
+    RS_LAUNCH(e, s, 1, rs::launch_align_pred_proj(g, s));
+    RS_CUDA(e, cudaStreamSynchronize(s));
+    return RS_OK;
+  };
+  const int r = predictor();
+  if (r != RS_OK) {
+    cudaStreamSynchronize(s);
+    cudaFree(mem);
+    return r;
+  }
+  if (e->spot.mem) {
+    RS_CUDA(e, cudaDeviceSynchronize());     // a call still queued may read the old set
+    cudaFree(e->spot.mem);
+  }
+  e->spot = {};
+  e->spot.mem = mem;
+  e->spot.n_kw = n_kw; e->spot.U_max = U_max; e->spot.delay = delay_frames; e->spot.chunk = chunk_frames;
+  e->spot.ring_cap = static_cast<int>(ring); e->spot.threshold = threshold;
+  e->spot.labels = g.labels; e->spot.label_len = g.label_len; e->spot.pred_proj = g.pred_proj;
+  return RS_OK;
+}
+
+size_t rs_spot_state_bytes(const rs_engine* e) {
+  return e && e->spot.n_kw > 0 ? rs::spot_record(e->spot.U_max, e->spot.ring_cap).total : 0;
+}
+
+int rs_spot_max_hits(const rs_engine* e, int B) { return e && e->spot.n_kw > 0 && B > 0 ? spot_capacity(e, B) : 0; }
+
+int rs_rnnt_spot_resume(rs_engine* e, const float* enc_dev, const int32_t* dec_begin_dev, const int32_t* dec_end_dev, const int32_t* slot_dev,
+                        const int32_t* last_dev, void* records_dev, int n_slots, int B, int T_max, int max_out, int32_t* hit_meta_host,
+                        float* hit_val_host, int32_t* hit_frames_host, float* hit_token_lp_host, int32_t* n_hits_host, float* E_dev,
+                        int32_t* S_dev, int32_t* sigma_dev, void* stream) {
+  const char* fn = "rs_rnnt_spot_resume";
+  if (!e || !enc_dev || !dec_begin_dev || !dec_end_dev || !slot_dev || !last_dev || B <= 0 || T_max <= 0)
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  RS_CUDA(e, cudaSetDevice(e->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<int32_t> h(static_cast<size_t>(4) * B);
+  const int32_t* src[4] = {dec_begin_dev, dec_end_dev, slot_dev, last_dev};
+  for (int i = 0; i < 4; ++i) RS_CUDA(e, cudaMemcpyAsync(h.data() + i * B, src[i], static_cast<size_t>(B) * 4, cudaMemcpyDeviceToHost, s));
+  RS_CUDA(e, cudaStreamSynchronize(s));
+  const SpotCall c{h.data(), h.data() + B, h.data() + 2 * B, h.data() + 3 * B, records_dev, n_slots, max_out, hit_meta_host, hit_val_host,
+                   hit_frames_host, hit_token_lp_host, n_hits_host, E_dev, S_dev, sigma_dev};
+  RS_TRY(check_spot_call(e, fn, B, T_max, c));
+  const rs_model_config& cfg = e->cfg;
+  const size_t M = static_cast<size_t>(B) * T_max;
+  rs::Arena a;
+  const size_t o_xn = a.take(M * cfg.d_model * 2), o_encp = a.take(M * cfg.joint_hidden * 4), o_args = a.take(static_cast<size_t>(4) * B * 4);
+  RS_TRY(grow_align_ws(e, fn, a.off, s));
+  char* ws = static_cast<char*>(e->align_ws);
+  int32_t* args = reinterpret_cast<int32_t*>(ws + o_args);
+  for (int i = 0; i < 4; ++i) RS_CUDA(e, cudaMemcpyAsync(args + i * B, src[i], static_cast<size_t>(B) * 4, cudaMemcpyDeviceToDevice, s));
+  // joint.enc over every frame, as in the greedy path
+  RS_LAUNCH(e, s, 1, rs::launch_f32_to_bf16(enc_dev, ws + o_xn, static_cast<int64_t>(M) * cfg.d_model, s));
+  RS_TRY(gemm(e, {ws + o_xn, e->dec.enc_w, e->dec.enc_b, nullptr, ws + o_encp, static_cast<int>(M), cfg.joint_hidden, cfg.d_model, RS_EPI_BIAS_F32, 1.f}, s));
+  RS_TRY(spot_enqueue(e, fn, reinterpret_cast<float*>(ws + o_encp), T_max, B, c, args, s));
+  return spot_collect(e, B, c, s);
+}
+
+int rs_stream_step_spot(rs_engine* e, const void* wav_host, int wav_is_pcm16, const int32_t* len_host, const int32_t* dec_begin_host,
+                        const int32_t* dec_end_host, const int32_t* slot_host, void* states, int B, int L_max, int32_t* tokens_host,
+                        int32_t* frames_host, int32_t* n_tok_host, int U_max, float alpha, float* stats_host, const int32_t* last_host,
+                        void* spot_records_dev, int n_slots, int max_out, int32_t* hit_meta_host, float* hit_val_host,
+                        int32_t* hit_frames_host, float* hit_token_lp_host, int32_t* n_hits_host, void* stream) {
+  const char* fn = "rs_stream_step_spot";
+  if (!e || !dec_begin_host || !dec_end_host || !slot_host || !states || !len_host || !last_host || B <= 0 || (stats_host && !alpha_ok(alpha)))
+    return fail(e, RS_ERR_INVALID_ARG, "%s: bad arguments (dec_begin, dec_end, slot, last, len and states must be set; with stats, alpha > 0 and finite)", fn);
+  if (reinterpret_cast<uintptr_t>(states) & 15u) return fail(e, RS_ERR_INVALID_ARG, "%s: states must be 16-byte aligned", fn);
+  for (int b = 0; b < B; ++b) {
+    const int n = len_host[b] < 0 || len_host[b] > L_max ? -1 : rs_enc_valid(e, len_host[b]);
+    if (n < 0 || dec_begin_host[b] < 0 || dec_begin_host[b] > dec_end_host[b] || dec_end_host[b] > n)
+      return fail(e, RS_ERR_INVALID_ARG, "%s: row %d: need 0 <= dec_begin (%d) <= dec_end (%d) <= rs_enc_valid(len = %d) = %d and len <= L_max",
+                  fn, b, dec_begin_host[b], dec_end_host[b], len_host[b], n);
+  }
+  const SpotCall c{dec_begin_host, dec_end_host, slot_host, last_host, spot_records_dev, n_slots, max_out, hit_meta_host, hit_val_host,
+                   hit_frames_host, hit_token_lp_host, n_hits_host, nullptr, nullptr, nullptr};
+  RS_TRY(check_spot_call(e, fn, B, INT32_MAX, c));   // also: the slots are distinct and >= 0, as rs_stream_step requires
+  const Resume rs{dec_begin_host, dec_end_host, slot_host, states};
+  return transcribe_batch(e, fn, wav_host, wav_is_pcm16 != 0, len_host, B, L_max, tokens_host, frames_host, n_tok_host, U_max,
+                          stats_host, alpha, static_cast<cudaStream_t>(stream), &rs, &c);
 }
 
 }  // extern "C"

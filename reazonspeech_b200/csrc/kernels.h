@@ -188,6 +188,40 @@ cudaError_t launch_rnnt_spot_pick(const AlignArgs& a, const SpotArgs& sp, cudaSt
 // shared memory of the pick kernel (false when T_max frames do not fit)
 bool spot_pick_fits(int T_max, int max_hits);
 
+// Streaming keyword spotting (spot_stream.cu; semantics: keywords.py, "Streaming").  One record per (stream slot, keyword) of
+// spot_record(U_max, ring_cap).total bytes; pair p = b * n_kw + k of a call is row b's stream (record slot[b]) and keyword k.
+struct SpotRecord { size_t column, lists, ring, total; };
+__host__ __device__ inline size_t spot_entry_bytes(int U_max) { return 12 + static_cast<size_t>(8) * U_max; }
+__host__ __device__ inline SpotRecord spot_record(int U_max, int ring_cap) {
+  SpotRecord r;
+  r.column = 32;                                                    // header int32[8]
+  r.lists = r.column + static_cast<size_t>(12) * U_max;
+  r.ring = r.lists + static_cast<size_t>(8) * U_max * U_max;
+  r.total = (r.ring + ring_cap * spot_entry_bytes(U_max) + 15) & ~static_cast<size_t>(15);
+  return r;
+}
+constexpr int kSpotHitInts = 5;                                     // a decided hit: row, keyword, s, e, forced
+struct SpotStreamArgs {
+  const int32_t* dec_begin; const int32_t* dec_end; const int32_t* slot; const int32_t* last;   // device [B]
+  int B, n_kw, U_max, C;                      // C: the compact block's frames per row (>= every dec_end - dec_begin)
+  int delay, ring_cap;                        // D frames; ring entries per pair
+  float threshold;
+  const int32_t* label_len;                   // [n_kw]
+  uint8_t* records;                           // [n_slots][n_kw] records
+  int32_t* len;                               // [B] dec_end - dec_begin (written by the gather)
+  float* E_out; int32_t* S_out; int T_out;    // optional [B][n_kw][T_out] at buffer frames [dec_begin, dec_end)
+  int32_t* sigma_out;                         // optional [B][n_kw]: sigma(t) after the step (-1: no frame seen)
+  int32_t* n_hits; int hit_cap;               // the decided hits: [hit_cap] x (meta i32[5], (score, confidence) f32[2],
+  int32_t* hit_meta; float* hit_val;          //   frames i32[U_max], token_lp f32[U_max])
+  int32_t* hit_frames; float* hit_lp;
+};
+// rows [dec_begin, dec_end) of encp f32 [B][T_max][Hj] -> out f32 [B][C][Hj], len
+cudaError_t launch_spot_gather(const float* encp, int T_max, int Hj, const SpotStreamArgs& s, float* out, cudaStream_t stream);
+// a: the pairs' lattice (rnnt_lattice_kernel<true> over the gathered block: B = n_kw keywords, T_max = C, enc_len = s.len)
+cudaError_t launch_rnnt_spot_resume_dp(const AlignArgs& a, const SpotStreamArgs& s, cudaStream_t stream);
+cudaError_t launch_rnnt_spot_resume_pick(const SpotStreamArgs& s, cudaStream_t stream);
+size_t spot_pick_stream_smem(int ring_cap);
+
 // norm_audio on the device: polyphase resampling to 16 kHz + channel average + transcribe()'s zero padding (resample.cu)
 struct ResampleArgs {
   const void* in; bool in_i16;          // [B, C, L_in_max] f32, or int16 PCM (scaled by 2^-15)

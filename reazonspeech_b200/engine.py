@@ -55,6 +55,7 @@ EXPORTS = [
     "rs_set_ngram_lm", "rs_ngram_lm_eval", "rs_rnnt_align", "rs_rnnt_align_lattice", "rs_rnnt_alsd_trace",
     "rs_stream_state_bytes", "rs_rnnt_greedy_resume", "rs_stream_step", "rs_set_boost_roots", "rs_rnnt_alsd_nbest", "rs_rnnt_maes", "rs_maes_last_rows",
     "rs_rnnt_align_segment", "rs_rnnt_spot", "rs_rnnt_spot_lattice", "rs_rnnt_align_banded", "rs_rnnt_align_banded_lattice",
+    "rs_set_spot_keywords", "rs_spot_state_bytes", "rs_spot_max_hits", "rs_rnnt_spot_resume", "rs_stream_step_spot",
 ]
 
 MAX_NBEST = 64                          # include/rs_engine.h RS_MAX_NBEST
@@ -148,6 +149,13 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
     lib.rs_rnnt_spot.restype = ip
     lib.rs_rnnt_spot_lattice.argtypes = [vp, vp, vp, ip, ip, vp, vp, ip, ip, vp, vp, vp]
     lib.rs_rnnt_spot_lattice.restype = ip
+    lib.rs_set_spot_keywords.argtypes = [vp, vp, vp, ip, ip, C.c_float, ip, ip, vp]
+    lib.rs_spot_state_bytes.argtypes = [vp]
+    lib.rs_spot_state_bytes.restype = C.c_size_t
+    lib.rs_spot_max_hits.argtypes = [vp, ip]
+    lib.rs_rnnt_spot_resume.argtypes = [vp, vp, vp, vp, vp, vp, vp, ip, ip, ip, ip, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.rs_stream_step_spot.argtypes = [vp, vp, ip, vp, vp, vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp, vp, ip, ip,
+                                        vp, vp, vp, vp, vp, vp]
     lib.rs_stream_state_bytes.argtypes = [vp]
     lib.rs_stream_state_bytes.restype = C.c_size_t
     lib.rs_rnnt_greedy_resume.argtypes = [vp, vp, vp, vp, vp, vp, ip, ip, vp, vp, vp, ip, C.c_float, vp, vp]
@@ -526,6 +534,98 @@ class Engine:
                                             frames.data_ptr(), ntok.data_ptr(), U_max, float(alpha or 0.0),
                                             out[3].data_ptr() if alpha is not None else None, self._stream()), "rs_stream_step")
         return out
+
+    # -- streaming keyword spotting (keywords.py, "Streaming")
+    def set_spot_keywords(self, keywords: Sequence[Sequence[int]], threshold: float, delay_frames: int, chunk_frames: int) -> None:
+        """Install the keyword set of the streaming spot (rs_set_spot_keywords): token-id lists of 1..32 ids, the threshold, the
+        delay D and the chunk C in frames; the keywords' predictor rows are computed once, here.  An empty list clears the set."""
+        self._spot_owner = None                  # whoever installs a set claims it afterwards (StreamingTranscriber)
+        if not keywords:
+            self._check(self.lib.rs_set_spot_keywords(self.h, None, None, 0, 1, 0.0, 0, 1, self._stream()), "rs_set_spot_keywords")
+            self._spot_U = self._spot_kw = 0
+            return
+        U = max(len(k) for k in keywords)
+        labels = np.zeros((len(keywords), max(U, 1)), dtype=np.int32)
+        for i, k in enumerate(keywords):
+            labels[i, : len(k)] = k
+        lens = np.array([len(k) for k in keywords], dtype=np.int32)
+        self._check(self.lib.rs_set_spot_keywords(self.h, labels.ctypes.data, lens.ctypes.data, len(keywords), max(U, 1), float(threshold),
+                                                  int(delay_frames), int(chunk_frames), self._stream()), "rs_set_spot_keywords")
+        self._spot_U, self._spot_kw = max(U, 1), len(keywords)
+
+    def _check_records(self, records: torch.Tensor) -> None:
+        """The spot records must be uint8 [n_slots, n_kw of the installed set, spot_state_bytes] on this device: the kernels
+        index them as [slot][keyword]."""
+        n_kw = getattr(self, "_spot_kw", 0)
+        if not (records.dtype == torch.uint8 and records.is_contiguous() and records.dim() == 3 and records.device == self.device
+                and records.shape[1] == n_kw and records.shape[2] == self.spot_state_bytes and n_kw > 0):
+            raise ValueError(f"spot records must be contiguous uint8 [n_slots, {n_kw}, {self.spot_state_bytes}] on {self.device} "
+                             f"(the installed keyword set), got {records.dtype} {tuple(records.shape)} on {records.device}")
+
+    @property
+    def spot_state_bytes(self) -> int:
+        """Bytes of one (stream, keyword) record of the installed set (rs_spot_state_bytes; 0 without a set)."""
+        return int(self.lib.rs_spot_state_bytes(self.h))
+
+    def _spot_outputs(self, B: int):
+        n = int(self.lib.rs_spot_max_hits(self.h, B))
+        U = getattr(self, "_spot_U", 0) or 1
+        cached = getattr(self, "_spot_out", None)
+        if cached is None or cached[0].shape[0] < n or cached[2].shape[1] != U:
+            cached = (np.empty((max(n, 1), 5), np.int32), np.empty((max(n, 1), 2), np.float32), np.empty((max(n, 1), U), np.int32),
+                      np.empty((max(n, 1), U), np.float32), np.zeros(1, np.int32))
+            self._spot_out = cached
+        return cached
+
+    @staticmethod
+    def _spot_hits(out):
+        n = int(out[4][0])
+        return tuple(a[:n].copy() for a in out[:4])
+
+    def spot_resume(self, enc: torch.Tensor, dec_begin: torch.Tensor, dec_end: torch.Tensor, slot: torch.Tensor, last: torch.Tensor,
+                    records: torch.Tensor, scores: bool = False):
+        """The resumed keyword spot (rs_rnnt_spot_resume): row b continues its stream from records[slot[b]] (device uint8
+        [n_slots, n_kw, spot_state_bytes]) over frames [dec_begin[b], dec_end[b]) of ``enc`` -> the decided hits as host arrays
+        (meta i32 [n, 5] = (row, keyword, s, e, forced), val f32 [n, 2] = (score, confidence), frames i32 [n, U], token_lp
+        f32 [n, U]) sorted by (row, keyword, e); with ``scores`` also E f32 / S i32 [B, n_kw, T] (NaN / -1 outside the ranges)
+        and sigma i32 [B, n_kw] device tensors."""
+        B, T, _ = enc.shape
+        assert enc.dtype == torch.float32 and enc.is_contiguous()
+        self._check_records(records)
+        n_kw = records.shape[1]
+        args = [a.to(self.device, torch.int32).contiguous() for a in (dec_begin, dec_end, slot, last)]
+        out = self._spot_outputs(B)
+        E = torch.full((B, n_kw, T), float("nan"), device=self.device) if scores else None
+        S = torch.full((B, n_kw, T), -1, dtype=torch.int32, device=self.device) if scores else None
+        sigma = torch.full((B, n_kw), -2, dtype=torch.int32, device=self.device) if scores else None
+        ptr = lambda x: None if x is None else x.data_ptr()
+        self._check(self.lib.rs_rnnt_spot_resume(self.h, enc.data_ptr(), *[a.data_ptr() for a in args], records.data_ptr(), records.shape[0],
+                                                 B, T, out[0].shape[0], *[a.ctypes.data for a in out], ptr(E), ptr(S), ptr(sigma),
+                                                 self._stream()), "rs_rnnt_spot_resume")
+        hits = self._spot_hits(out)
+        return hits + (E, S, sigma) if scores else hits
+
+    def stream_step_spot(self, wav: torch.Tensor, lens: torch.Tensor, dec_begin: torch.Tensor, dec_end: torch.Tensor, slot: torch.Tensor,
+                         states: torch.Tensor, U_max: int, out, last: torch.Tensor, records: torch.Tensor, alpha: Optional[float] = None):
+        """``stream_step`` plus the resumed keyword spot on the same joint.enc rows (rs_stream_step_spot): ``last`` host int32 [B]
+        (row b decodes its stream's last frame), ``records`` the spot records -> the decided hits as ``spot_resume`` returns them;
+        ``out`` is filled as ``stream_step`` fills it."""
+        B, L = wav.shape
+        assert wav.device.type == "cpu" and wav.dtype in (torch.float32, torch.int16) and wav.is_contiguous()
+        assert states.dtype == torch.uint8 and states.is_contiguous() and states.shape[-1] == self.stream_state_bytes
+        self._check_records(records)
+        host = [a.to(torch.int32).contiguous() for a in (lens, dec_begin, dec_end, slot, last)]
+        assert all(a.device.type == "cpu" for a in host)
+        self.ensure_workspace(B, L)
+        tokens, frames, ntok = out[:3]
+        hits = self._spot_outputs(B)
+        self._check(self.lib.rs_stream_step_spot(self.h, wav.data_ptr(), int(wav.dtype == torch.int16), host[0].data_ptr(), host[1].data_ptr(),
+                                                 host[2].data_ptr(), host[3].data_ptr(), states.data_ptr(), B, L, tokens.data_ptr(),
+                                                 frames.data_ptr(), ntok.data_ptr(), U_max, float(alpha or 0.0),
+                                                 out[3].data_ptr() if alpha is not None else None, host[4].data_ptr(), records.data_ptr(),
+                                                 records.shape[0], hits[0].shape[0], *[a.ctypes.data for a in hits], self._stream()),
+                    "rs_stream_step_spot")
+        return self._spot_hits(hits)
 
     def transcribe_device(self, wav: torch.Tensor, lens: torch.Tensor, U_max: Optional[int] = None, out=None, alpha: Optional[float] = None):
         """With ``alpha``: also the confidence statistics (``greedy``), ``out`` then holds four tensors."""

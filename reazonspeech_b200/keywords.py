@@ -39,7 +39,45 @@ released checkpoint before trusting a hit list.
 
 On the GPU (rs_rnnt_spot): joint.enc once per recording, the teacher-forced predictor once per keyword, the lattice of every
 pair on wgmma (rnnt_lattice_kernel<true>), one warp per pair for the recursion (rnnt_spot_dp_kernel) and one CTA per pair for
-the hit policy and the backtraces (rnnt_spot_pick_kernel).  This module holds the host-side helpers."""
+the hit policy and the backtraces (rnnt_spot_pick_kernel).  This module holds the host-side helpers.
+
+Streaming.  Keyword hits on live streams (``StreamingTranscriber(keywords=StreamKeywordsConfig(...))``), decided chunk by
+chunk on the encoder output the streaming decode produces.  Nothing above changes: lattice, recursion, E(e), S(e), m(e), the
+threshold and the pick rule are the offline ones.  A stream's frames are the streaming frame grid (streaming.py), and the
+lattice of a chunk's frames is the lattice of the same frames offline, cell for cell.
+
+  1. Carried recursion.  delta[t][u] depends on frames <= t only.  So a (stream, keyword) pair carries one column from step
+     to step: delta[t][u], the start frame start[t][u] and lp_blank[t][u] for u = 1..U at its last decoded frame t, and each
+     step extends the recursion over its frames.  E(e) and S(e) of every frame are bit-identical to rs_rnnt_spot's on the
+     same lattice cells: the same fp32 operations in the same order, the same tie rule.
+  2. Frontier bound.  sigma(t) = min over u in 1..U of start[t][u].  Every candidate that ends after t has S >= sigma(t): the
+     best path to (e', U), e' > t, either emits token 1 after t (S > t >= sigma(t)), or leaves frame t from some cell (t, u)
+     with u >= 1, and the prefix of that path up to (t, u) is that cell's best path (the recursion's backtrace), whose first
+     token is at start[t][u] >= sigma(t).  sigma never decreases: start[t + 1][u] is start[t][u] (blank) or start[t + 1][u - 1]
+     (emission), by induction over u >= sigma(t) with start[t + 1][0] = t + 1.
+  3. Exact decisions (the natural cut).  After each step, L = sigma(t), then L <- min(L, min{S(e) : pending candidate with
+     e >= L}) until it stops changing.  No known or future candidate at or after L can intersect a candidate that ends before
+     L, so the candidates with e < L form complete overlap components, and the offline greedy rule (the largest m first, the
+     smaller e on a tie, drop whatever intersects a hit) applied to them gives exactly the offline decisions, provided the
+     offline list did not reach ``max_hits`` (the stream has no such limit).  When a stream is closed and its last frame
+     decoded, L = infinity.
+  4. Bounded delay (the forced cut).  ``max_delay_seconds`` = D frames (default 10 s, NOT calibrated) bounds the time from a
+     candidate's end frame to its decision: if a pending candidate has t - e >= D, the cut becomes max(L, t + 1 - D).  The
+     candidates before the cut are decided by the same greedy rule among themselves, and every later candidate whose span
+     reaches back to a reported hit is dropped (the barrier: the largest reported end frame).  Hits decided beyond the natural
+     cut carry ``forced = True``, and the stream counts its forced cuts.  A stream without a forced cut reproduces the offline
+     hits exactly; after one, only this is promised: hits never overlap, and each is a true segment path with its score.
+     Forcing will be common on real audio, though none is reachable here to measure it: blanks in silence are nearly free, so
+     stretching a span over silence raises m(e).  The offline rule therefore likes long spans, and sigma lags while a channel
+     is silent.
+  5. Hits.  The fields of ``find_keywords`` (span, score = E(e), confidence = m(e), the tokens' frames and lp_emit) plus
+     ``forced``; seconds from ``hit_seconds`` over the audio pushed so far (the trailing pad exists only after close).
+
+On the GPU (rs_stream_step_spot, rs_rnnt_spot_resume; spot_stream.cu): the chunk's joint.enc rows gathered into a compact
+block, the pairs' lattice on rnnt_lattice_kernel<true>, the recursion resumed from a per-(stream, keyword) record with a
+forward traceback instead of predecessor bytes (a hit's span can be much longer than any window kept on the device), the
+candidates appended to a ring of D + C entries per pair, and one warp per pair for the cuts and the pick.  The keywords'
+predictor rows are computed once, when the set is installed."""
 from __future__ import annotations
 
 import math
@@ -48,6 +86,7 @@ from dataclasses import dataclass, field
 from typing import Any, List, Sequence, Union
 
 from .captions import segment_seconds
+from .streaming import _frames
 
 THRESHOLD = -1.0
 MAX_HITS = 64
@@ -69,6 +108,34 @@ class KeywordHit:
     score: float = math.nan
     confidence: float = math.nan
     subwords: List[Any] = field(default_factory=list)
+    forced: bool = False      # streaming: decided by the bounded delay, beyond the natural cut (the offline list may differ)
+
+
+@dataclass(frozen=True)
+class StreamKeywordsConfig:
+    """The keywords of a ``StreamingTranscriber``: text or token-id sequences (validated by ``keyword_ids`` when the
+    transcriber is built), the per-frame threshold, and the alert delay, a non-negative multiple of 0.08 s (default 10 s,
+    NOT calibrated)."""
+    keywords: Sequence[Keyword]
+    threshold: float = THRESHOLD
+    max_delay_seconds: float = 10.0
+
+    def __post_init__(self):
+        check_search(self.threshold, 1)
+        self.delay_frames()
+        if len(self.keywords) == 0:
+            raise ValueError("StreamKeywordsConfig needs at least one keyword")
+
+    def delay_frames(self) -> int:
+        """D in encoder frames."""
+        return _frames(self.max_delay_seconds, "max_delay_seconds")
+
+
+def stream_record_bytes(U_max: int, delay_frames: int, chunk_frames: int) -> int:
+    """Bytes of one (stream, keyword) record (rs_spot_state_bytes): header, carried column, token lists, and a ring of D + C
+    candidates of 12 + 8 U_max bytes, rounded up to 16."""
+    n = 32 + 12 * U_max + 8 * U_max * U_max + (delay_frames + chunk_frames) * (12 + 8 * U_max)
+    return (n + 15) // 16 * 16
 
 
 def keyword_ids(keywords: Sequence[Keyword], vocab_size: int, tokenizer=None) -> List[List[int]]:

@@ -19,7 +19,16 @@ model's global list; ``boosting.stack_tables``), restacked at the next ``step()`
 record's automaton state is then moved from its list's old region to its new one (``remap_boost_states``), so a stream's
 open partial match survives other streams opening and closing.  A list is built and checked in ``open()``: one with bad
 token ids, or one that would take the open streams' lists and the global list past ``MAX_STATES`` states together, raises
-ValueError there and takes no slot; ``model.set_phrase_boosting`` likewise refuses a global list that would not fit."""
+ValueError there and takes no slot; ``model.set_phrase_boosting`` likewise refuses a global list that would not fit.
+
+``StreamingTranscriber(model, keywords=StreamKeywordsConfig([...]))`` also spots the keywords on every stream (keywords.py,
+"Streaming"): each step runs ``rs_stream_step_spot`` instead of ``rs_stream_step``, the same decode plus the resumed spot on
+the same joint.enc rows.  ``take_hits()`` returns the hits decided since its last call, ``hits(id)`` all of a drained stream's
+hits shaped like ``find_keywords``.  The spot records live in one device tensor ``[max_streams, n_kw, rs_spot_state_bytes]``.
+They are allocated when the transcriber is built, max_streams x n_kw x rs_spot_state_bytes bytes (for example 300 MB at the
+default 256 streams, 100 keywords of up to 8 tokens and the 10 s delay; 1.2 GB with keywords of 32 tokens), so size
+``max_streams`` to the streams actually served.  The keyword set is installed in the engine when the transcriber is built (and
+again before a step if another transcriber installed its own since)."""
 from __future__ import annotations
 
 import contextlib
@@ -31,7 +40,9 @@ import numpy as np
 import torch
 
 from ...boosting import MAX_STATES, PhraseBoostingConfig, build_tables, config_key, stack_tables
+from ...alignment import alignment_hypothesis
 from ...confidence import measure
+from ...keywords import KeywordHit, StreamKeywordsConfig, hit_seconds, keyword_ids
 from ...streaming import P, PAD_SAMPLES, StreamingConfig, plan_row, stream_frames
 from .decode import PAD_SECONDS, SECONDS_PER_STEP, decode_hypothesis
 from .interface import Subword, TranscribeResult
@@ -53,12 +64,14 @@ class _Stream:
     frames: List[int] = field(default_factory=list)
     stats: List[np.ndarray] = field(default_factory=list)
     boosting: Optional[PhraseBoostingConfig] = None    # the stream's own phrase list; None: the model's global list
+    hits: List[tuple] = field(default_factory=list)    # (keyword index, KeywordHit) decided so far (with keywords)
 
 
 class StreamingTranscriber:
     """Live streams on one single-GPU greedy model (``B200RnntModel``).  Use one transcriber per device for several GPUs."""
 
-    def __init__(self, model, config: StreamingConfig = StreamingConfig(), max_streams: int = 256):
+    def __init__(self, model, config: StreamingConfig = StreamingConfig(), max_streams: int = 256,
+                 keywords: Optional[StreamKeywordsConfig] = None):
         if not isinstance(model, B200RnntModel):
             raise ValueError("StreamingTranscriber runs on one GPU: pass a single-device model (one transcriber per device)")
         if model.decoding != "greedy":
@@ -79,6 +92,16 @@ class StreamingTranscriber:
         self._layout_key = None                      # (global list key, the open streams' distinct list keys); None: rebuild
         self._tables = None                          # (device tables, roots by list key) while a stream has its own list
         self._built = {}                             # list key -> its build_tables, for the lists of the open streams
+        self.keywords = keywords
+        if keywords is not None:
+            if not isinstance(keywords, StreamKeywordsConfig):
+                raise ValueError(f"keywords must be a StreamKeywordsConfig or None, got {type(keywords).__name__}")
+            self._kw_ids = keyword_ids(keywords.keywords, model.cfg.vocab_size, model.tokenizer)
+            self._spot_key = object()
+            self._install_keywords()
+            self.spot_states = torch.zeros(max_streams, len(self._kw_ids), eng.spot_state_bytes, dtype=torch.uint8, device=eng.device)
+            self._taken: Dict[int, List[KeywordHit]] = {}
+            self._finished_hits: Dict[int, List[List[KeywordHit]]] = {}
         model.__dict__.setdefault("_table_listeners", []).append(weakref.WeakMethod(self._tables_changed))
         model.__dict__.setdefault("_boost_checks", []).append(weakref.WeakMethod(self._check_global))
 
@@ -105,6 +128,9 @@ class StreamingTranscriber:
         self._free.remove(slot)
         self.states[slot].zero_()
         self._finished.pop(slot, None)
+        if self.keywords is not None:
+            self.spot_states[slot].zero_()
+            self._finished_hits.pop(slot, None)
         self._live[slot] = _Stream(slot, np.zeros(PAD_SAMPLES, np.int16), boosting=boosting)
         return slot
 
@@ -154,6 +180,22 @@ class StreamingTranscriber:
             raise KeyError(f"stream {sid} has not drained (close it and step until done)")
         return self._finished[sid]
 
+    def take_hits(self) -> Dict[int, List[KeywordHit]]:
+        """{stream id: the keyword hits decided since the last call}, each list in decision order (per step: keyword, then
+        end frame).  Empty without keywords."""
+        if self.keywords is None:
+            return {}
+        out, self._taken = self._taken, {}
+        return out
+
+    def hits(self, sid: int) -> List[List[KeywordHit]]:
+        """All of a drained stream's keyword hits: one time-ordered list per keyword, shaped like ``find_keywords``."""
+        if self.keywords is None:
+            raise ValueError("this transcriber spots no keywords (StreamingTranscriber(..., keywords=...))")
+        if sid not in self._finished_hits:
+            raise KeyError(f"stream {sid} has not drained (close it and step until done)")
+        return self._finished_hits[sid]
+
     @property
     def open_streams(self) -> List[int]:
         return sorted(self._live)
@@ -183,6 +225,30 @@ class StreamingTranscriber:
             self._finish(sid)
         return out
 
+    # -- keyword spotting
+    def _install_keywords(self) -> None:
+        eng = self.model.engine
+        if getattr(eng, "_spot_owner", None) is not self._spot_key:
+            eng.set_spot_keywords(self._kw_ids, self.keywords.threshold, self.keywords.delay_frames(), self.frames_cfg[0])
+            eng._spot_owner = self._spot_key
+
+    def _collect(self, sids, hits) -> None:
+        """The hits of one engine call (rows are ``sids``) -> KeywordHit, appended to the streams and to take_hits()."""
+        model = self.model
+        meta, val, frames, token_lp = hits
+        for i in range(meta.shape[0]):
+            r, k, s0, e0, forced = (int(x) for x in meta[i])
+            sid, ids = sids[r], self._kw_ids[k]
+            st = self._live[sid]
+            n = len(ids)
+            fr, tl, score = frames[i, :n].tolist(), token_lp[i, :n].tolist(), float(val[i, 0])
+            res = decode_hypothesis(model, alignment_hypothesis(ids, fr, tl, score, float("nan"), model.cfg.blank))
+            pushed = st.n - PAD_SAMPLES - (PAD_SAMPLES if st.closed else 0)
+            start, end = hit_seconds(s0, e0, pushed / 16000)
+            h = KeywordHit(self.keywords.keywords[k], start, end, score, float(val[i, 1]), res.subwords, bool(forced))
+            st.hits.append((k, h))
+            self._taken.setdefault(sid, []).append(h)
+
     def _run(self, batch) -> Dict[int, List[Subword]]:
         model, eng = self.model, self.model.engine
         C = self.frames_cfg[0]
@@ -201,7 +267,17 @@ class StreamingTranscriber:
                 dev, root_of = self._tables
                 stack.enter_context(model.phrase_tables_set(dev))
                 eng.set_boost_roots([root_of[config_key(self._live[sid].boosting)] for sid, _ in batch])
-            eng.stream_step(wav, lens, col("dec_begin"), col("dec_end"), slot, self.states, U, out, alpha=alpha)
+            if self.keywords is None:
+                eng.stream_step(wav, lens, col("dec_begin"), col("dec_end"), slot, self.states, U, out, alpha=alpha)
+            else:
+                self._install_keywords()
+                # A closed stream always ends with a step of its own that decodes frame F - 1, and that step decides what is
+                # pending: before close() a stream has decoded at most rs_enc_valid(n) frames, and the 0.5 s of zeros that
+                # close() appends adds at least 6 to F = rs_enc_valid(n + 8000).
+                last = [self._live[sid].closed and row.dec_end + row.offset >= stream_frames(self._live[sid].n, True) for sid, row in batch]
+                hits = eng.stream_step_spot(wav, lens, col("dec_begin"), col("dec_end"), slot, self.states, U, out,
+                                            torch.tensor(last, dtype=torch.int32), self.spot_states, alpha=alpha)
+                self._collect([sid for sid, _ in batch], hits)
         tokens, frames, ntok = out[:3]
         res: Dict[int, List[Subword]] = {}
         for r, (sid, row) in enumerate(batch):
@@ -243,6 +319,9 @@ class StreamingTranscriber:
         res = decode_hypothesis(self.model, hyp)
         res.hypothesis = hyp
         self._finished[sid] = res
+        if self.keywords is not None:
+            self._finished_hits[sid] = [sorted((h for j, h in s.hits if j == k), key=lambda h: (h.start_seconds, h.end_seconds))
+                                        for k in range(len(self._kw_ids))]
         self._free.append(s.slot)
 
     def _tables_changed(self, word: int) -> None:
